@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — the reference's headline hot path on B200: SGPT-125M bi-encoder, batch 256 x seq_len 128 encode
+"""bench.py — the reference's headline hot path on one H100: SGPT-125M bi-encoder, batch 256 x seq_len 128 encode
 (GPT-Neo forward + weighted-mean pool) and exact top-1001 cosine retrieval of 128 queries over a 1M-doc corpus shard.
 
 One "step" = encode one batch of 256 synthetic documents  +  search 128 synthetic queries against the resident
@@ -7,9 +7,12 @@ One "step" = encode one batch of 256 synthetic documents  +  search 128 syntheti
 top-1001 lists are exchanged ONCE (kernel-to-kernel over NVLink peer mappings; NCCL all-gather of packed entries as the
 other transport) and merged on every rank; the merged result is verified against a single-rank search of the whole of
 a small planted corpus: `merge_verified`).  Extra keys (N=1): BASELINE configs 3-5 at full size, the fp32 top-k overlap,
-the 10M-doc strong-scaling legs.  Prints ONE JSON line (rank 0).
+the strong-scaling legs over one 10M-doc corpus (D = 768) and one 5M-doc corpus (D = 4096, 41 GB: what fits an 80 GB
+H100 next to the rest).  Prints ONE JSON line (rank 0).  --dump-outputs DIR writes what the last timed step computed (the
+pooled embeddings of its batch, the top-k scores and ids of its queries) as .npy files for output-for-output comparisons
+of two builds: every input is generated from fixed seeds, so the same arguments give the same inputs.
 
-  python bench.py --gpus 1 --steps 10 --warmup 3
+  python bench.py --gpus 1 --steps 10 --warmup 3 [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
   python bench.py --impl reference ...      # the reference's CPU path (HF GPTNeoModel fp32 + pooling + cos_sim/topk)
 """
@@ -72,7 +75,8 @@ def peaks():
     if os.path.exists(p):
         z = json.load(open(p))
         return dict(hbm=z["hbm_gbs"], tf_burst=z["bf16_tflops"], tf_sustained=z["bf16_tflops_sustained"], src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sustained=1400.0, src="fallback")
+    # NVIDIA's H100 SXM data sheet (dense bf16, HBM3), not a measured figure
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sustained=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -223,7 +227,7 @@ def calibrate_reference(weights, enc_seconds, search_seconds):
 
 def run_reference(args, rank):
     """`--impl reference`: the reference's CPU path (HF GPTNeoModel fp32 on all host cores + Pooling / exact-search ports),
-    each step a bounded sample of the workload (~3 s), throughput in the same unit as the B200 arm."""
+    each step a bounded sample of the workload (~3 s), throughput in the same unit as the GPU arm."""
     if rank != 0:
         return
     w = synthetic_weights(0)
@@ -261,6 +265,15 @@ def measured_traffic():
             return json.load(f), os.path.relpath(files[-1], os.path.dirname(os.path.abspath(__file__)))
     except (OSError, ValueError):
         return {}, None
+
+
+def dump_outputs(out_dir, emb, scores, ids):
+    """What one timed step hands its caller, as float32 / float64 .npy files: the pooled embeddings of the encoded batch
+    [B, d] and the top-k scores [NQ, k] and document ids [NQ, k] of the searched queries (ids are exact in float64)."""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "embeddings.npy"), emb.detach().float().cpu().numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "topk_scores.npy"), scores.detach().float().cpu().numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "topk_ids.npy"), ids.detach().cpu().numpy().astype(np.float64))
 
 
 def workload_config(n):
@@ -555,8 +568,8 @@ def run_b200(args, rank, world, local_rank):
     barrier()
 
     # ---- device-timed loop (inputs resident in HBM) -------------------------------------------------------------
-    # The timed region is K steps repeated R times back to back (R chosen so that the region lasts >= ~1.2 s: 30 steps of
-    # 7 ms alone would be a 0.2 s measurement); every number below is divided by K*R.  Two passes over the SAME steps:
+    # The timed region is exactly K = --steps steps back to back (ask for enough of them that the region lasts a second or
+    # more); every number below is divided by K.  Two passes over the SAME steps:
     # pass 1 is the timed region of `value` (three CUDA events per step); pass 2 repeats K steps with the library's
     # per-launch CUDA events switched on (two event records around each of the ~140 launches of a step cost ~7 % of the
     # step, so they stay out of pass 1) and feeds `roofline` / `kernel_ms_per_step`.
@@ -566,6 +579,8 @@ def run_b200(args, rank, world, local_rank):
     tot_n1 = (ctypes.c_int64 * 8)()
     gclk_c, gclk_ns = ctypes.c_double(), ctypes.c_double()
 
+    last = {}
+
     def timed_pass(n_steps):
         ev = [[torch.cuda.Event(enable_timing=True) for _ in range(3)] for _ in range(n_steps)]
         barrier()
@@ -573,9 +588,9 @@ def run_b200(args, rank, world, local_rank):
         for k in range(n_steps):
             r = resident[k % len(resident)]
             ev[k][0].record()
-            enc.encode_packed(r[0], r[1], r[2], B, B * S, S)
+            last["emb"] = enc.encode_packed(r[0], r[1], r[2], B, B * S, S)
             ev[k][1].record()
-            search_step(queries)
+            last["search"] = search_step(queries)
             ev[k][2].record()
         barrier()
         t_w = time.perf_counter() - t_w0
@@ -584,17 +599,12 @@ def run_b200(args, rank, world, local_rank):
         return e_ms, s_ms, ev[0][0].elapsed_time(ev[-1][2]), t_w
 
     K = args.steps
-    _, _, probe_ms, _ = timed_pass(min(K, 5))
-    step_est = maxr(probe_ms / min(K, 5))
-    R = max(1, int(np.ceil(1200.0 / max(1e-3, step_est * K))))
-    if world > 1:
-        rt = torch.tensor([R], device=dev)
-        dist.all_reduce(rt, op=dist.ReduceOp.MAX)
-        R = int(rt.item())
-    KR = K * R
+    KR = K  # the timed region is exactly --steps steps
     lib.sgpt_profile_read(None, None, tot_n0)
     lib.sgpt_profile_gemm_clock(ctypes.byref(gclk_c), ctypes.byref(gclk_ns))  # reset
     enc_ms, sea_ms, tot_ms, t_wall = timed_pass(KR)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["emb"], *last["search"])
     lib.sgpt_profile_read(None, None, tot_n1)
     lib.sgpt_profile_gemm_clock(ctypes.byref(gclk_c), ctypes.byref(gclk_ns))
     launches = sum(int(tot_n1[c] - tot_n0[c]) for c in range(8))
@@ -661,11 +671,11 @@ def run_b200(args, rank, world, local_rank):
     e2e_enc_s, _, _ = e2e_pass(False, KR)  # encode-only variant (extra key)
 
     # the same search issued back to back (no encode in between): inside a step it starts in the clock / power state the
-    # encoder leaves behind (SM and L2 clocks ~1.6 of 1.96 GHz under the power cap), which slows an HBM-streaming kernel
-    # through the L2's per-clock throughput cap (profiles/r02_search_phases_clock_state_and_query_count.jsonl)
+    # encoder leaves behind (a power-capped card runs lower clocks under the encoder's load), which can slow an
+    # HBM-streaming kernel through the L2's per-clock throughput
     iso_ms = maxr(time_search(lambda: search_step(queries), 50))
     # a DRES-sized query batch (XS:54-60 encodes ALL queries before it scores): 1024 queries per call are scanned 256 at a
-    # time by CTA pairs (cta_group::2, M = 256), i.e. 4 passes over the shard instead of 8
+    # time (two CTAs per corpus tile), i.e. 4 passes over the shard instead of 8
     large = None
     if world == 1:
         try:
@@ -680,14 +690,14 @@ def run_b200(args, rank, world, local_rank):
 
     # ---- strong scaling of the exact search over ONE 10 M-doc corpus split across the ranks -----------------------------
     # (north_star: "linear top-k scaling to 8 GPUs on a 10M-doc synthetic corpus"; the main line above is weak scaling at
-    # 1 M docs per GPU.)  Two legs: D = 768 (the 125M model's embedding size) and D = 4096 (config 5: sgpt-bloom-7b1).  A
-    # failure is reported as an error string and cannot cost the main numbers.
+    # 1 M docs per GPU.)  Two legs: 10 M docs at D = 768 (the 125M model's embedding size) and 5 M docs at D = 4096 (config 5:
+    # sgpt-bloom-7b1; 10 M x 4096 bf16 would be 82 GB, more than one 80 GB H100 holds).  A failure is reported as an error
+    # string and cannot cost the main numbers.
     big = None
     if args.corpus_10m:
         big = {}
-        for Dbig in (768, 4096):
+        for Dbig, total in ((768, 10_000_000), (4096, 5_000_000)):
             try:
-                total = 10_000_000
                 lo, hi = shard_range(total, rank, world)
                 gb = torch.Generator(device=dev).manual_seed(555 + rank)
                 qb_ = torch.randn(NQ, Dbig, generator=gq, device=dev)
@@ -756,7 +766,7 @@ def run_b200(args, rank, world, local_rank):
         "metric": METRIC, "value": emb_per_s, "unit": "embeddings/s", "n_gpus": world, "steps": K, "warmup": args.warmup,
         "ms_per_step": tot_ms / KR, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16",
         "data": "synthetic", "config": workload_config(world),
-        "timed_region": {"repeats_of_the_K_steps": R, "steps_timed": KR, "device_seconds": tot_ms / 1e3,
+        "timed_region": {"steps_timed": KR, "device_seconds": tot_ms / 1e3,
                          "note": "every per-step figure is the region's total divided by steps_timed"},
         "encode_ms_per_step": enc_ms / KR, "search_ms_per_step": sea_ms / KR,
         "search": {"value": qps, "unit": "queries/s", "corpus_docs": NDOCS * world, "top_k": TOPK,
@@ -768,7 +778,7 @@ def run_b200(args, rank, world, local_rank):
                                             "measured right after the encoder (power-capped clocks)"},
                    "large_query_batch": large},
         "encoder_model_tflops": (lin_flops + att_flops) * B * world * KR / (enc_ms / 1e3) / 1e12,
-        "roofline": {"kernel": "gemm_bf16_tn_kernel (tcgen05 linear layers)", "bound": "tensor", "achieved": gemm_tflops,
+        "roofline": {"kernel": "gemm_bf16_tn_kernel (wgmma linear layers)", "bound": "tensor", "achieved": gemm_tflops,
                      "peak": pk["tf_sustained"], "unit": "TFLOP/s",
                      "frac": (gemm_tflops / pk["tf_sustained"]) if gemm_tflops else None, "traffic": gemm_traffic,
                      "traffic_unit": "DRAM bytes per launch (ncu, read+write, mean over the layer shapes)",
@@ -838,8 +848,10 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's outputs (embeddings, top-k scores and ids) as .npy")
     ap.add_argument("--no-corpus-10m", dest="corpus_10m", action="store_false",
-                    help="skip the extra legs that time the exact search over one 10M-doc corpus (D = 768 and 4096) split "
+                    help="skip the extra legs that time the exact search over one large corpus (10M x 768, 5M x 4096) split "
                          "across the ranks (strong scaling; reported as search_10m_strong_scaling)")
     ap.add_argument("--no-other-configs", dest="other_configs", action="store_false",
                     help="skip the N=1 legs for BASELINE configs 3-5 (1.3B / 5.8B / bloom-7b1 encoders, their shard shapes) "

@@ -1,5 +1,5 @@
 /*
- * sgpt_b200 — C ABI of the B200-native SGPT bi-encoder hot path.
+ * sgpt_b200 — C ABI of the H100-native (sm_90a) SGPT bi-encoder hot path.
  *
  * The reference (Muennighoff/sgpt @ 37c8bf09) is pure Python and has no FFI layer; its plug-in boundary is the pair
  * of duck-typed protocols in biencoder/beir/custommodels/exact_search.py:22-32 (embedder: encode_queries /
@@ -55,7 +55,7 @@ int sgpt_layernorm(const float* x, const float* gamma, const float* beta, void* 
  *     epilogue: SGPT_EPI_BF16       out bf16[M,N]  = acc + bias
  *               SGPT_EPI_GELU_BF16  out bf16[M,N]  = gelu_new(acc + bias)       (HF activations.py NewGELUActivation)
  *               SGPT_EPI_RESID_F32  out fp32[M,N]  = resid + acc + bias         (resid fp32[M,N], may alias out)
- *     Runs on the tcgen05 tensor cores (TMA-staged tiles, TMEM accumulators). */
+ *     Runs on the wgmma tensor cores (TMA-staged tiles, register accumulators). */
 #define SGPT_EPI_BF16 0
 #define SGPT_EPI_GELU_BF16 1
 #define SGPT_EPI_RESID_F32 2
@@ -87,7 +87,7 @@ int sgpt_linear_qkv_rotary(const void* x, int64_t ldx, const void* w_qkv, void* 
  *     window: 0 = plain causal; w > 0 = GPT-Neo local attention (key j visible to query i iff i-w < j <= i, :63-66).
  *     alibi_slopes: fp32[H] or NULL; adds slope_h * (key position in its sequence) to the scaled scores (BLOOM ALiBi,
  *                   HF:bloom/modeling_bloom.py:43-86; the bias depends on the key only).
- *     impl: 0 = tcgen05 tensor-core kernel, 1 = SIMT cross-check kernel (test infrastructure). */
+ *     impl: 0 = tensor-core (mma.sync) kernel, 1 = SIMT cross-check kernel (test infrastructure). */
 int sgpt_attention(const void* qkv, void* out, const int32_t* cu_seqlens, int B, int T, int H, int hd, float scale,
                    int window, int max_seqlen, const float* alibi_slopes, int impl, sgpt_stream_t stream);
 
@@ -252,7 +252,7 @@ int sgpt_f32_to_bf16(const float* x, void* y, int64_t count, sgpt_stream_t strea
 
 /* S1. scores[q,j] = fixnan( <Q[q,:], C[j,:]> * q_scale[q] * c_scale[j] )      ST/util.py:24-63, XS:96-99
  *     Q bf16[nq,D], C bf16[n,D], q_scale fp32[nq]|NULL, c_scale fp32[n]|NULL (NULL = 1: dot_score),
- *     scores fp32[nq, lds]; NaN -> -1 as XS:99.  tcgen05 GEMM, corpus streamed once from HBM. */
+ *     scores fp32[nq, lds]; NaN -> -1 as XS:99.  wgmma GEMM, corpus streamed once from HBM. */
 int sgpt_scores(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* scores, int64_t lds,
                 int nq, int64_t n, int D, sgpt_stream_t stream);
 
@@ -369,7 +369,7 @@ int sgpt_pool_partials(const float* x, const int32_t* pos, const int32_t* cu_seq
 #define SGPT_NUM_LAUNCH_CATEGORIES 8
 int sgpt_profile_enable(int on);
 int sgpt_profile_read(double* ms_by_cat, int64_t* timed_launches_by_cat, int64_t* total_launches_by_cat);
-/* SM clock the tcgen05 GEMM kernels actually ran at: every GEMM launch has one thread read %clock64 and %globaltimer
+/* SM clock the GEMM kernels actually ran at: every GEMM launch has one thread read %clock64 and %globaltimer
  * at its start and end and accumulate both deltas on the device.  Returns the accumulated SM cycles and nanoseconds
  * since the previous call (cycles / ns = GHz under load, which nvidia-smi sampling cannot resolve) and resets them.
  * Synchronises the device. */

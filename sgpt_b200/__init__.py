@@ -1,4 +1,4 @@
-"""sgpt_b200 — B200-native SGPT bi-encoder hot path (GPT forward -> weighted-mean pool -> cosine/dot top-k).
+"""sgpt_b200 — H100-native (sm_90a) SGPT bi-encoder hot path (GPT forward -> weighted-mean pool -> cosine/dot top-k).
 
 Public surface mirrors the reference's plug-in protocols (biencoder/beir/beir_dense_retriever.py,
 biencoder/beir/custommodels/exact_search.py):
@@ -7,7 +7,7 @@ biencoder/beir/custommodels/exact_search.py):
     model = DenseRetrievalExactSearch(CustomEmbedder(model_name, method="weightedmean", specb=True), batch_size=128)
     results = model.search(corpus, queries, top_k=1000, score_function="cos_sim")
 
-All arithmetic runs in the in-tree CUDA library (libsgpt_b200.so, sm_100a); importing the package does not load it,
+All arithmetic runs in the in-tree CUDA library (libsgpt_b200.so, sm_90a: H100); importing the package does not load it,
 using it without the library raises.
 """
 from .config import ModelConfig, preset  # noqa: F401

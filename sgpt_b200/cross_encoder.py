@@ -1,4 +1,4 @@
-"""Continuation log-likelihood scoring with the B200 encoder — the SGPT cross-encoder path (SURVEY.md §8f row 4).
+"""Continuation log-likelihood scoring with the CUDA encoder — the SGPT cross-encoder path (SURVEY.md §8f row 4).
 
 ``LogLikelihoodScorer.loglikelihood_tokens`` has the contract of ``_loglikelihood_tokens``
 (crossencoder/beir/sgptce.py:150-262): requests ``(cache_key, context_enc, continuation_enc)`` in, one float per request
@@ -6,7 +6,7 @@ out — the sum of ``log p(continuation token | everything before it)``.  What c
 
 * the batch is packed ragged (no right padding with token 0 as at :201-204; with causal attention the padding never
   influenced the real positions anyway), one ``sgpt_forward`` call per batch;
-* only the rows that predict continuation tokens go through ln_f + the LM head (``sgpt_lm_logprobs``: tcgen05 GEMM
+* only the rows that predict continuation tokens go through ln_f + the LM head (``sgpt_lm_logprobs``: wgmma GEMM
   against the tied/untied LM-head matrix, fused log-softmax-gather kernel); the ``[batch, seq, vocab]`` fp32
   log-softmax tensor of :221 and its ``.cpu()`` copy never exist;
 * per-request sums are taken on the device (``sgpt_segment_sum``), one small D2H per batch.

@@ -1,17 +1,17 @@
 // F4: causal (optionally sliding-window) self-attention over a ragged batch, HF:gpt_neo/modeling_gpt_neo.py:105-130.
 //
-// tcgen05 kernel (impl 0).  One CTA = one (sequence, head, 128-query tile); 128 threads, thread r owns query row r
-// (TMEM lane r), so the softmax needs no cross-thread reduction.
-//   smem : Q[128,hd] K[128,hd] V[128,hd] (TMA, SWIZZLE_128B, 64-column sub-tiles) + P[128,128] bf16
-//   TMEM : S = Q K^T (128 fp32 columns) | O (hd fp32 columns)
-//   loop over 128-key tiles j (only tiles the causal/window mask can reach):
-//       S  = Q K_j^T                    tcgen05.mma, A = Q (K-major), B = K_j (K-major)
-//       online softmax in fp32 (exp2, running max m and sum l per row), P -> bf16 -> swizzled smem
-//       O  = alpha * O                  tcgen05.ld / tcgen05.st  (skipped on the first tile)
-//       O += P V_j                      tcgen05.mma, A = P (K-major), B = V_j (MN-major: V is [key, hd] row-major)
+// Tensor-core kernel (impl 0): FlashAttention-2 style with mma.sync.m16n8k16 (bf16 operands, fp32 accumulate).  One CTA =
+// one (head, sequence, 64-query tile), 4 warps; warp w owns query rows 16 w .. 16 w + 15, and each thread holds two rows
+// (g, g + 8 of its warp's 16) of the score and output fragments, so a row reduction is two shuffles inside a quad.
+//   smem : Q [64 x hd] | two stages of { K_j [KT x hd], V_j [KT x hd] } (KT = 64 keys, 32 at hd = 256), rows padded by
+//          16 bytes so that every ldmatrix phase hits 8 distinct bank groups; filled by cp.async, positions beyond the
+//          sequence zero-filled
+//   loop over the key tiles j the causal / window mask can reach (K_{j+1}, V_{j+1} load while tile j computes):
+//       S  = Q K_j^T                    mma.sync, A = Q (ldmatrix), B = K_j (ldmatrix: [key, hd] rows are K-major)
+//       online softmax in fp32 in the exp2 domain (running max m and per-thread partial sum l per row)
+//       O  = alpha * O + P V_j          P re-packed from the S accumulators into bf16 A fragments (no smem round trip),
+//                                       B = V_j (ldmatrix.trans: V is [key, hd] row-major)
 //   epilogue: O / l -> bf16 -> out[token, head*hd : (head+1)*hd]
-// K_{j+1} is fetched by TMA while tile j's softmax runs; V_{j+1} while tile j+1's QK^T and softmax run.
-// hd=64 uses 81 KB smem and 256 TMEM columns so two CTAs share an SM and overlap each other's MMA/softmax phases.
 //
 // SIMT kernel (impl 1): one warp per (token, head), fp32 everywhere — test cross-check only.
 #include <math.h>
@@ -23,782 +23,233 @@
 
 namespace sgpt {
 
-constexpr int kAttnTile = 128;
-constexpr int kSubBytes = kAttnTile * 128;  // one [128 rows x 64 bf16] sub-tile
+constexpr int kAttnQ = 64;  // query rows per CTA (4 warps x 16)
+constexpr int kAttnThreads = 128;
 
-// Visibility of the 128 query rows of a tile.  vis_*: this THREAD's row (causal / window / ragged length bounds on the
-// key position); w_*: bounds over the 32 rows of its WARP — a 32-key chunk entirely inside [w_lo_max, w_hi_min] needs no
-// per-element mask, a chunk entirely outside [w_lo_min, w_hi_max] contributes nothing (causal: half of the diagonal tile
-// on average).
-struct RowVis {
-  int vis_hi, vis_lo, w_hi_min, w_hi_max, w_lo_max, w_lo_min;
-};
-__device__ __forceinline__ RowVis make_row_vis(int qp0, int tid, int len, int window) {
-  RowVis r;
-  const int qpos = qp0 + tid;
-  r.vis_hi = min(qpos, len - 1);
-  r.vis_lo = (window > 0) ? (qpos - window + 1) : 0;
-  const int wq0 = qp0 + (tid >> 5) * 32;
-  r.w_hi_min = min(wq0, len - 1);
-  r.w_hi_max = min(wq0 + 31, len - 1);
-  r.w_lo_max = (window > 0) ? (wq0 + 31 - window + 1) : 0;
-  r.w_lo_min = (window > 0) ? (wq0 - window + 1) : 0;
-  return r;
-}
-
-// Softmax pass 1 over one 128-key tile whose scores sit in TMEM (thread = query row): the row maximum in the exp2
-// domain, i.e. of s * sl2 (+ slope2 * key_pos with ALiBi), -inf when no key of the tile is visible.
-__device__ __forceinline__ float softmax_tile_max(uint32_t tS_row, int kv0, const RowVis& rv, float sl2, float slope2) {
-  const int vis_hi = rv.vis_hi, vis_lo = rv.vis_lo, w_hi_min = rv.w_hi_min, w_hi_max = rv.w_hi_max,
-            w_lo_max = rv.w_lo_max, w_lo_min = rv.w_lo_min;
-  float mx = -INFINITY, mxa = -INFINITY;  // raw-score maximum (no ALiBi) / scaled+biased maximum (ALiBi)
-#pragma unroll 1
-  for (int c = 0; c < 4; ++c) {
-    const int c_lo = kv0 + c * 32, c_hi = c_lo + 31;
-    if (c_lo > w_hi_max || c_hi < w_lo_min) continue;  // nothing visible for any row of this warp (warp-uniform)
-    uint32_t v[32];
-    tmem_ld_32x32(tS_row + c * 32, v);
-    tmem_ld_wait();
-    const bool unmasked = (c_hi <= w_hi_min && c_lo >= w_lo_max);  // warp-uniform
-    if (slope2 == 0.f) {
-      // no ALiBi: the maximum is taken over the raw scores, the (positive) scale is applied once after the reduction
-      if (unmasked) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) mx = fmaxf(mx, __uint_as_float(v[i]));
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const int kp = c_lo + i;
-          if (kp <= vis_hi && kp >= vis_lo) mx = fmaxf(mx, __uint_as_float(v[i]));
-        }
-      }
-    } else {
-      // ALiBi: maximum of the scaled, biased scores s * sl2 + slope2 * key_pos (two FMAs per element)
-      const float ab = slope2 * static_cast<float>(c_lo);
-      if (unmasked) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i)
-          mxa = fmaxf(mxa, fmaf(__uint_as_float(v[i]), sl2, fmaf(slope2, static_cast<float>(i), ab)));
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const int kp = c_lo + i;
-          const float t = fmaf(__uint_as_float(v[i]), sl2, fmaf(slope2, static_cast<float>(i), ab));
-          if (kp <= vis_hi && kp >= vis_lo) mxa = fmaxf(mxa, t);
-        }
-      }
-    }
-  }
-  return (slope2 == 0.f) ? mx * sl2 : mxa;  // sl2 > 0
-}
-
-// Softmax pass 2: p = exp2(s * sl2 (+ ALiBi) - m_use) for the same tile, P -> bf16 -> the thread's row of the swizzled
-// [128 x 128] smem operand (two 64-key sub-tiles); returns the row sum of p.
-__device__ __forceinline__ float softmax_tile_exp(uint32_t tS_row, int kv0, const RowVis& rv, float sl2, float slope2,
-                                                  float m_use, uint32_t sP_addr, int tid) {
-  const int vis_hi = rv.vis_hi, vis_lo = rv.vis_lo, w_hi_min = rv.w_hi_min, w_hi_max = rv.w_hi_max,
-            w_lo_max = rv.w_lo_max, w_lo_min = rv.w_lo_min;
-  float lsum = 0.f;
-#pragma unroll 1
-  for (int c = 0; c < 4; ++c) {
-    const int c_lo = kv0 + c * 32, c_hi = c_lo + 31;
-    uint32_t pk[16];
-    if (c_lo > w_hi_max || c_hi < w_lo_min) {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) pk[i] = 0u;
-    } else {
-      uint32_t v[32];
-      tmem_ld_32x32(tS_row + c * 32, v);
-      tmem_ld_wait();
-      const bool unmasked = (c_hi <= w_hi_min && c_lo >= w_lo_max);  // warp-uniform
-      if (slope2 == 0.f) {
-        if (unmasked) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float p0 = exp2f(fmaf(__uint_as_float(v[2 * i]), sl2, -m_use));
-            const float p1 = exp2f(fmaf(__uint_as_float(v[2 * i + 1]), sl2, -m_use));
-            lsum += p0 + p1;
-            pk[i] = pack_bf16(p0, p1);
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const int kp = c_lo + 2 * i;
-            float p0 = exp2f(fmaf(__uint_as_float(v[2 * i]), sl2, -m_use));
-            float p1 = exp2f(fmaf(__uint_as_float(v[2 * i + 1]), sl2, -m_use));
-            if (!(kp <= vis_hi && kp >= vis_lo)) p0 = 0.f;
-            if (!(kp + 1 <= vis_hi && kp + 1 >= vis_lo)) p1 = 0.f;
-            lsum += p0 + p1;
-            pk[i] = pack_bf16(p0, p1);
-          }
-        }
-      } else {
-        const float ab = fmaf(slope2, static_cast<float>(c_lo), -m_use);  // slope2 * key_pos - m, position part
-        if (unmasked) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float p0 = exp2f(fmaf(__uint_as_float(v[2 * i]), sl2, fmaf(slope2, static_cast<float>(2 * i), ab)));
-            const float p1 =
-                exp2f(fmaf(__uint_as_float(v[2 * i + 1]), sl2, fmaf(slope2, static_cast<float>(2 * i + 1), ab)));
-            lsum += p0 + p1;
-            pk[i] = pack_bf16(p0, p1);
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const int kp = c_lo + 2 * i;
-            float p0 = exp2f(fmaf(__uint_as_float(v[2 * i]), sl2, fmaf(slope2, static_cast<float>(2 * i), ab)));
-            float p1 =
-                exp2f(fmaf(__uint_as_float(v[2 * i + 1]), sl2, fmaf(slope2, static_cast<float>(2 * i + 1), ab)));
-            if (!(kp <= vis_hi && kp >= vis_lo)) p0 = 0.f;
-            if (!(kp + 1 <= vis_hi && kp + 1 >= vis_lo)) p1 = 0.f;
-            lsum += p0 + p1;
-            pk[i] = pack_bf16(p0, p1);
-          }
-        }
-      }
-    }
-    // P[row, kv 32c .. 32c+31] -> sub-tile (c >> 1), 16-B chunks 4*(c&1) .. +3, XOR-swizzled with (row & 7)
-    const uint32_t prow = sP_addr + (c >> 1) * kSubBytes + tid * 128;
-#pragma unroll
-    for (int q4 = 0; q4 < 4; ++q4) {
-      const int chunk = ((c & 1) * 4 + q4) ^ (tid & 7);
-      sts_v4(prow + chunk * 16, pk[4 * q4], pk[4 * q4 + 1], pk[4 * q4 + 2], pk[4 * q4 + 3]);
-    }
-  }
-  return lsum;
-}
-
-// kSingle: every sequence of the batch fits one 128-key tile (max_seqlen <= 128 — all of the reference's NLI models
-// and BASELINE configs 1-2).  Then Q and K are dead once S = Q K^T has been read, so P reuses their smem, and O
-// reuses S's TMEM columns: 48 KB smem / 128 TMEM columns per CTA at hd = 64, i.e. FOUR co-resident CTAs per SM whose
-// load / MMA / softmax / store phases overlap each other (the general variant keeps separate buffers: 2 CTAs per SM).
-template <int HD, bool kSingle>
+template <int HD>
 struct AttnCfg {
-  static constexpr int kSub = HD / 64;
-  static constexpr int kQBytes = kSub * kSubBytes;
-  static constexpr int kPBytes = 2 * kSubBytes;
-  static constexpr int kSmemBytes = 1024 + 3 * kQBytes + (kSingle ? 0 : kPBytes) + 64;
-  static constexpr int kTmemNeed = kSingle ? (HD > 128 ? HD : 128) : 128 + HD;
-  static constexpr int kTmemCols = kTmemNeed <= 128 ? 128 : (kTmemNeed <= 256 ? 256 : 512);
-  static_assert(!kSingle || 2 * kQBytes >= kPBytes, "P must fit into the Q|K region");
+  static constexpr int KT = HD == 256 ? 32 : 64;  // keys per tile (hd 256: the 128 output accumulators need the registers)
+  static constexpr int kPitch = HD + 8;            // bf16 per smem row
+  static constexpr int kQElems = kAttnQ * kPitch;
+  static constexpr int kKVElems = KT * kPitch;
+  static constexpr int kSmemBytes = (kQElems + 4 * kKVElems) * 2;
 };
 
-template <int HD, bool kSingle>
-__global__ void __launch_bounds__(128) attention_tc_kernel(const __grid_constant__ CUtensorMap tma_qkv,
-                                                           __nv_bfloat16* __restrict__ out,
-                                                           const int32_t* __restrict__ cu, int H, float sl2,
-                                                           int window, const float* __restrict__ alibi,
-                                                           int head_major, int prefetch_ahead) {
-  using Cfg = AttnCfg<HD, kSingle>;
-  // Heads vary fastest over the grid (x = head, y = sequence, z = query tile; head_major == 0 is the round-1 order with
-  // heads slowest): the CTAs resident at the same time then read ALL heads' 128-byte q / k / v pieces of the same token
-  // rows — whole 3 d-element rows of the qkv matrix — instead of one piece out of every row of the whole batch.
-  const int qt = head_major ? blockIdx.z : blockIdx.x, b = blockIdx.y, h = head_major ? blockIdx.x : blockIdx.z;
+__device__ __forceinline__ void cp_async_16(uint32_t dst, const void* src, bool valid) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
+// c[16 x 8] += a[16 x 16] * b[16 x 8]   (bf16 operands, fp32 accumulators)
+__device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+// `rows` rows of HD bf16 (sequence positions p0 .. p0 + rows - 1, columns col .. col + HD - 1 of the qkv matrix) ->
+// smem rows of kPitch; positions at or beyond the sequence length are zero-filled
+template <int HD>
+__device__ __forceinline__ void attn_load_rows(uint32_t sdst, const __nv_bfloat16* __restrict__ qkv, size_t ld, int seq0,
+                                               int p0, int rows, int len, int col, int tid) {
+  constexpr int C = HD / 8;  // 16-byte chunks per row
+  for (int i = tid; i < rows * C; i += kAttnThreads) {
+    const int r = i / C, c = i - r * C;
+    const int p = p0 + r;
+    const bool ok = p < len;
+    cp_async_16(sdst + (r * AttnCfg<HD>::kPitch + c * 8) * 2, qkv + static_cast<size_t>(seq0 + (ok ? p : 0)) * ld + col + c * 8,
+                ok);
+  }
+}
+
+template <int HD>
+__global__ void __launch_bounds__(kAttnThreads) attention_mma_kernel(const __nv_bfloat16* __restrict__ qkv,
+                                                                     __nv_bfloat16* __restrict__ out,
+                                                                     const int32_t* __restrict__ cu, int H, float sl2,
+                                                                     int window, const float* __restrict__ alibi) {
+  using Cfg = AttnCfg<HD>;
+  constexpr int KT = Cfg::KT, P = Cfg::kPitch;
+  // heads vary fastest over the grid: the CTAs resident at the same time read all heads' q / k / v pieces of the same
+  // token rows, i.e. whole rows of the qkv matrix
+  const int h = blockIdx.x, b = blockIdx.y, qt = blockIdx.z;
+  pdl_sync();  // programmatic dependent launch: see common.cuh
   const int seq0 = __ldg(cu + b);
   const int len = __ldg(cu + b + 1) - seq0;
-  const int qp0 = qt * kAttnTile;
-  if (qp0 >= len) return;  // whole CTA exits together, before any barrier/TMEM state exists
+  const int qp0 = qt * kAttnQ;
+  if (qp0 >= len) return;
 
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;
-  uint8_t* sK = sQ + Cfg::kQBytes;
-  uint8_t* sV = sK + Cfg::kQBytes;
-  uint8_t* sP = kSingle ? sQ : sV + Cfg::kQBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + Cfg::kQBytes + (kSingle ? 0 : Cfg::kPBytes));
-  uint64_t* bar_q = bars + 0;
-  uint64_t* bar_k = bars + 1;
-  uint64_t* bar_v = bars + 2;
-  uint64_t* bar_s = bars + 3;
-  uint64_t* bar_o = bars + 4;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 5);
-
-  const int tid = threadIdx.x;
-  const int warp = tid >> 5;
+  extern __shared__ __align__(16) uint8_t attn_smem[];
+  const uint32_t sQ = smem_u32(attn_smem);
+  const uint32_t sKV = sQ + Cfg::kQElems * 2;  // stage s: K at sKV + 2 s kKVElems * 2, V right behind it
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int d = H * HD;
+  const size_t ld = 3 * static_cast<size_t>(d);
 
   const int lo_pos = (window > 0) ? max(0, qp0 - window + 1) : 0;
-  const int j_lo = kSingle ? 0 : lo_pos / kAttnTile;
-  const int j_hi = kSingle ? 0 : qt;  // len > qp0, so the diagonal tile always exists
+  const int j_lo = lo_pos / KT;
+  const int j_hi = min(qp0 + kAttnQ - 1, len - 1) / KT;
 
-  if (tid == 0) {
-    tma_prefetch_desc(&tma_qkv);
-    mbar_init(bar_q, 1);
-    mbar_init(bar_k, 1);
-    mbar_init(bar_v, 1);
-    mbar_init(bar_s, 1);
-    mbar_init(bar_o, 1);
-    fence_mbar_init();
-    // The first loads leave before the TMEM allocation and the CTA-wide barrier below: only this thread arms and issues
-    // them, everybody else meets them through the mbarriers after the __syncthreads.  (Barrier init overlapped the previous
-    // kernel's tail; cu_seqlens is written by a copy, never by a kernel, so reading it earlier is safe; qkv is touched only
-    // after the programmatic-dependency wait.)
-    pdl_sync();
-    mbar_expect_tx(bar_q, Cfg::kQBytes);
-    for (int s = 0; s < Cfg::kSub; ++s) tma_load_2d(sQ + s * kSubBytes, &tma_qkv, bar_q, h * HD + 64 * s, seq0 + qp0);
-    mbar_expect_tx(bar_k, Cfg::kQBytes);
-    for (int s = 0; s < Cfg::kSub; ++s)
-      tma_load_2d(sK + s * kSubBytes, &tma_qkv, bar_k, d + h * HD + 64 * s, seq0 + j_lo * kAttnTile);
-    mbar_expect_tx(bar_v, Cfg::kQBytes);
-    for (int s = 0; s < Cfg::kSub; ++s)
-      tma_load_2d(sV + s * kSubBytes, &tma_qkv, bar_v, 2 * d + h * HD + 64 * s, seq0 + j_lo * kAttnTile);
-  }
-  if (warp == 1) {
-    tmem_alloc(tmem_holder, Cfg::kTmemCols);
-    tmem_relinquish();
-  }
-  if (prefetch_ahead > 0 && head_major && tid == 64) {
-    // L2 prefetch of the first Q / K / V tiles of the unit `prefetch_ahead` CTAs further down the launch order (= the CTA
-    // that will take this one's place on some SM): its own loads then meet the L2 instead of the DRAM.  A CTA lives for a
-    // handful of microseconds, two thirds of which used to be this first wait (ncu: 38 % of the warp samples).
-    const long long lin = static_cast<long long>(blockIdx.x) +
-                          static_cast<long long>(gridDim.x) * (blockIdx.y + static_cast<long long>(gridDim.y) * blockIdx.z) +
-                          prefetch_ahead;
-    const int h2 = static_cast<int>(lin % gridDim.x);
-    const long long r2 = lin / gridDim.x;
-    const int b2 = static_cast<int>(r2 % gridDim.y);
-    const int qt2 = static_cast<int>(r2 / gridDim.y);
-    if (qt2 < static_cast<int>(gridDim.z)) {
-      const int s2 = __ldg(cu + b2);
-      const int len2 = __ldg(cu + b2 + 1) - s2;
-      const int qp2 = qt2 * kAttnTile;
-      if (qp2 < len2) {
-        const int lo2 = (window > 0) ? max(0, qp2 - window + 1) : 0;
-        const int j2 = kSingle ? 0 : lo2 / kAttnTile;
-        pdl_sync();
-        for (int s = 0; s < Cfg::kSub; ++s) {
-          tma_prefetch_l2_2d(&tma_qkv, h2 * HD + 64 * s, s2 + qp2);
-          tma_prefetch_l2_2d(&tma_qkv, d + h2 * HD + 64 * s, s2 + j2 * kAttnTile);
-          tma_prefetch_l2_2d(&tma_qkv, 2 * d + h2 * HD + 64 * s, s2 + j2 * kAttnTile);
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
-  const uint32_t tS = tmem_base;
-  const uint32_t tO = kSingle ? tmem_base : tmem_base + 128;
-  const uint32_t lane_off = static_cast<uint32_t>(warp * 32) << 16;
-  pdl_sync();
-
-  constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, false);
-  constexpr uint32_t idesc_o = make_idesc_bf16(128, HD, true);
+  attn_load_rows<HD>(sQ, qkv, ld, seq0, qp0, kAttnQ, len, h * HD, tid);
+  attn_load_rows<HD>(sKV, qkv, ld, seq0, j_lo * KT, KT, len, d + h * HD, tid);
+  attn_load_rows<HD>(sKV + Cfg::kKVElems * 2, qkv, ld, seq0, j_lo * KT, KT, len, 2 * d + h * HD, tid);
+  cp_async_commit();
 
   // BLOOM ALiBi (HF:bloom/modeling_bloom.py:84-86): + slope_h * (key position) before the softmax, here pre-multiplied
   // by log2(e) because the softmax runs in the exp2 domain
   const float slope2 = (alibi != nullptr) ? __ldg(alibi + h) * 1.4426950408889634f : 0.f;
-  const int qpos = qp0 + tid;
-  const RowVis rv = make_row_vis(qp0, tid, len, window);
-  float m_run = -INFINITY, l_run = 0.f;
+  const int g = lane >> 2, t4 = lane & 3;
+  int vis_hi[2], vis_lo[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int qpos = qp0 + warp * 16 + g + 8 * r;
+    vis_hi[r] = min(qpos, len - 1);
+    vis_lo[r] = (window > 0) ? (qpos - window + 1) : 0;
+  }
+  float o[HD / 8][4];
+#pragma unroll
+  for (int n = 0; n < HD / 8; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
 
   for (int j = j_lo; j <= j_hi; ++j) {
-    const uint32_t ph = static_cast<uint32_t>(j - j_lo) & 1u;
+    const int s = (j - j_lo) & 1;
+    if (j < j_hi) {  // the other stage was released by the __syncthreads at the end of the previous tile
+      const uint32_t nk = sKV + (s ^ 1) * 2 * Cfg::kKVElems * 2;
+      attn_load_rows<HD>(nk, qkv, ld, seq0, (j + 1) * KT, KT, len, d + h * HD, tid);
+      attn_load_rows<HD>(nk + Cfg::kKVElems * 2, qkv, ld, seq0, (j + 1) * KT, KT, len, 2 * d + h * HD, tid);
+    }
+    cp_async_commit();
+    cp_async_wait<1>();  // everything but the prefetch just issued has landed
+    __syncthreads();
+    const uint32_t sK = sKV + s * 2 * Cfg::kKVElems * 2, sV = sK + Cfg::kKVElems * 2;
+
     // ---- S = Q K_j^T ----
-    if (tid == 0) {
-      if (j == j_lo) mbar_wait(bar_q, 0);
-      mbar_wait(bar_k, ph);
-      tc_fence_after();
-      const uint32_t aq = smem_u32(sQ), ak = smem_u32(sK);
+    float sc[KT / 8][4];
 #pragma unroll
-      for (int kk = 0; kk < HD / 16; ++kk) {
-        const uint32_t off = (kk >> 2) * kSubBytes + (kk & 3) * 32;
-        umma_bf16_ss(tS, make_smem_desc_sw128(aq + off, 16, 1024), make_smem_desc_sw128(ak + off, 16, 1024), idesc_s,
-                     kk != 0);
-      }
-      umma_commit(bar_s);
-    }
-    __syncwarp();
-    mbar_wait(bar_s, ph);
-    tc_fence_after();
-    // K buffer is free again: prefetch K_{j+1} under the softmax
-    if (!kSingle && tid == 0 && j < j_hi) {
-      mbar_expect_tx(bar_k, Cfg::kQBytes);
-      for (int s = 0; s < Cfg::kSub; ++s)
-        tma_load_2d(sK + s * kSubBytes, &tma_qkv, bar_k, d + h * HD + 64 * s, seq0 + (j + 1) * kAttnTile);
-    }
-    __syncwarp();
-
-    // ---- online softmax over this row's 128 scores (pass 1: row maximum) ----
-    const int kv0 = j * kAttnTile;
-    const float m_new = fmaxf(m_run, softmax_tile_max(tS + lane_off, kv0, rv, sl2, slope2));
-    const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
-    const float alpha = exp2f(m_run - m_use);
-    // The P buffer (and O) still belong to the previous tile's P V MMA until it has completed.
-    if (j > j_lo) {
-      mbar_wait(bar_o, ph ^ 1u);
-      tc_fence_after();
-      __syncwarp();
-    }
-    // ---- pass 2: p = exp2(s * sl2 (+ alibi) - m), P -> bf16 -> swizzled smem ----
-    const float lsum = softmax_tile_exp(tS + lane_off, kv0, rv, sl2, slope2, m_use, smem_u32(sP), tid);
-    l_run = l_run * alpha + lsum;
-    m_run = m_new;
-
-    // ---- O = alpha * O (the previous P V MMA has landed: waited for above) ----
-    if (j > j_lo) {
-#pragma unroll 1
-      for (int c = 0; c < HD / 32; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(tO + lane_off + c * 32, v);
-        tmem_ld_wait();
+    for (int n = 0; n < KT / 8; ++n) sc[n][0] = sc[n][1] = sc[n][2] = sc[n][3] = 0.f;
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * alpha);
-        tmem_st_32x32(tO + lane_off + c * 32, v);
+    for (int kk = 0; kk < HD / 16; ++kk) {
+      uint32_t a[4];
+      ldmatrix_x4(sQ + ((warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * P + kk * 16 + (lane >> 4) * 8) * 2, a);
+#pragma unroll
+      for (int nb = 0; nb < KT / 16; ++nb) {
+        uint32_t kb[4];
+        ldmatrix_x4(sK + ((nb * 16 + (lane & 7) + (lane >> 4) * 8) * P + kk * 16 + ((lane >> 3) & 1) * 8) * 2, kb);
+        mma_bf16_16816(sc[2 * nb], a, kb[0], kb[1]);
+        mma_bf16_16816(sc[2 * nb + 1], a, kb[2], kb[3]);
       }
-      tmem_st_wait();
     }
-    fence_proxy_async_smem();  // P (generic-proxy stores) -> visible to the tensor core
-    tc_fence_before();
-    __syncthreads();           // all S reads and P writes of the CTA are done (kSingle: S columns become O)
+
+    // ---- online softmax (exp2 domain); element e of sc[n] is row g + 8 (e / 2), key kv0 + 8 n + 2 t4 + e % 2 ----
+    const int kv0 = j * KT;
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int n = 0; n < KT / 8; ++n) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int r = e >> 1;
+        const int kp = kv0 + 8 * n + 2 * t4 + (e & 1);
+        const float x = fmaf(sc[n][e], sl2, slope2 * static_cast<float>(kp));
+        sc[n][e] = (kp <= vis_hi[r] && kp >= vis_lo[r]) ? x : -INFINITY;
+        mx[r] = fmaxf(mx[r], sc[n][e]);
+      }
+    }
+    float alpha[2], m_use[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      const float m_new = fmaxf(m_run[r], mx[r]);
+      m_use[r] = (m_new == -INFINITY) ? 0.f : m_new;
+      alpha[r] = exp2f(m_run[r] - m_use[r]);
+      m_run[r] = m_new;
+    }
+    float lsum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int n = 0; n < KT / 8; ++n) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        sc[n][e] = exp2f(sc[n][e] - m_use[e >> 1]);
+        lsum[e >> 1] += sc[n][e];
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) l_run[r] = l_run[r] * alpha[r] + lsum[r];
+#pragma unroll
+    for (int n = 0; n < HD / 8; ++n) {
+      o[n][0] *= alpha[0];
+      o[n][1] *= alpha[0];
+      o[n][2] *= alpha[1];
+      o[n][3] *= alpha[1];
+    }
+
     // ---- O += P V_j ----
-    if (tid == 0) {
-      tc_fence_after();
-      mbar_wait(bar_v, ph);
-      tc_fence_after();
-      const uint32_t ap = smem_u32(sP), av = smem_u32(sV);
 #pragma unroll
-      for (int kk = 0; kk < kAttnTile / 16; ++kk) {
-        const uint64_t da = make_smem_desc_sw128(ap + (kk >> 2) * kSubBytes + (kk & 3) * 32, 16, 1024);
-        const uint64_t db = make_smem_desc_sw128(av + kk * 2048, kSubBytes, 1024);
-        umma_bf16_ss(tO, da, db, idesc_o, (j > j_lo) || (kk != 0));
-      }
-      umma_commit(bar_o);
-      if (!kSingle && j < j_hi) {
-        // V buffer is reusable once this P V completes; wait for it, then prefetch V_{j+1} (lands during the next
-        // tile's QK^T + softmax)
-        mbar_wait(bar_o, ph);
-        mbar_expect_tx(bar_v, Cfg::kQBytes);
-        for (int s = 0; s < Cfg::kSub; ++s)
-          tma_load_2d(sV + s * kSubBytes, &tma_qkv, bar_v, 2 * d + h * HD + 64 * s, seq0 + (j + 1) * kAttnTile);
+    for (int kk = 0; kk < KT / 16; ++kk) {
+      uint32_t a[4];
+      a[0] = pack_bf16(sc[2 * kk][0], sc[2 * kk][1]);
+      a[1] = pack_bf16(sc[2 * kk][2], sc[2 * kk][3]);
+      a[2] = pack_bf16(sc[2 * kk + 1][0], sc[2 * kk + 1][1]);
+      a[3] = pack_bf16(sc[2 * kk + 1][2], sc[2 * kk + 1][3]);
+#pragma unroll
+      for (int nd = 0; nd < HD / 16; ++nd) {
+        uint32_t vb[4];
+        ldmatrix_x4_trans(sV + ((kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * P + nd * 16 + (lane >> 4) * 8) * 2, vb);
+        mma_bf16_16816(o[2 * nd], a, vb[0], vb[1]);
+        mma_bf16_16816(o[2 * nd + 1], a, vb[2], vb[3]);
       }
     }
-    __syncwarp();
+    __syncthreads();  // stage s may be refilled by the next iteration's prefetch
   }
 
-  // ---- epilogue ----
-  {
-    const uint32_t ph = static_cast<uint32_t>(j_hi - j_lo) & 1u;
-    mbar_wait(bar_o, ph);
-    tc_fence_after();
-    __syncwarp();
-    const float inv_l = (l_run > 0.f) ? 1.0f / l_run : 0.f;
-    const bool row_ok = qpos < len;
-    __nv_bfloat16* dst = out + static_cast<size_t>(seq0 + qpos) * d + h * HD;
-#pragma unroll 1
-    for (int c = 0; c < HD / 32; ++c) {
-      uint32_t v[32];
-      tmem_ld_32x32(tO + lane_off + c * 32, v);
-      tmem_ld_wait();
-      if (row_ok) {
-        uint4* d4 = reinterpret_cast<uint4*>(dst + c * 32);
+  // ---- epilogue: O / l -> bf16 ----
 #pragma unroll
-        for (int q4 = 0; q4 < 4; ++q4) {
-          uint32_t o[4];
+  for (int r = 0; r < 2; ++r) {
+    float l = l_run[r];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv_l = (l > 0.f) ? 1.0f / l : 0.f;
+    const int qpos = qp0 + warp * 16 + g + 8 * r;
+    if (qpos < len) {
+      __nv_bfloat16* dst = out + static_cast<size_t>(seq0 + qpos) * d + h * HD + 2 * t4;
 #pragma unroll
-          for (int i = 0; i < 4; ++i)
-            o[i] = pack_bf16(__uint_as_float(v[8 * q4 + 2 * i]) * inv_l, __uint_as_float(v[8 * q4 + 2 * i + 1]) * inv_l);
-          d4[q4] = make_uint4(o[0], o[1], o[2], o[3]);
-        }
-      }
+      for (int n = 0; n < HD / 8; ++n)
+        *reinterpret_cast<uint32_t*>(dst + 8 * n) = pack_bf16(o[n][2 * r] * inv_l, o[n][2 * r + 1] * inv_l);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Warp-specialised, persistent variant (impl 0 for head_dim 64 / 128).
-//
-// One CTA per SM, 320 threads, TWO independent work slots per CTA.  A work unit = (sequence, head, 128-query tile); slot s
-// of CTA c walks units (2c + s), (2c + s) + 2 G, ... (heaviest q-tiles first).  Roles:
-//   warps 0-3   softmax / correction / epilogue warpgroup of slot 0   (thread = query row = TMEM lane)
-//   warps 4-7   the same for slot 1
-//   warp  8     TMA producer (one lane): Q tile of each unit, K/V tiles of its key loop, for both slots
-//   warp  9     tcgen05.mma issuer (one lane) for both slots + TMEM allocation
-// Per slot: smem Q [128 x hd] | NKV stages of { K_j [128 x hd] (re-used for P_j: K_j is dead once S_j = Q K_j^T has
-// completed) | V_j [128 x hd] }; TMEM S (128 fp32 columns) | O (hd columns).  Per key tile j of a unit:
-//       producer : K_j, V_j -> stage (after the P V MMA that last read the stage has completed)
-//       mma      : S = Q K_j^T                       -> s_full
-//       softmax  : row max, p = exp2(...), P -> bf16 -> smem (over K_j), O *= alpha (after o_full of tile j-1) -> p_full
-//       mma      : O += P V_j                        -> kv_empty (stage), o_full
-// The two slots are independent units, so the tensor core runs slot 1's MMAs while slot 0's warpgroup is in its softmax
-// and vice versa, and the producer runs ahead of both (NKV = 2 stages at hd 64); the single in-order issue thread and the
-// single producer thread serve both slots with non-blocking mbarrier polls (whichever slot is ready goes first), so
-// units of different lengths do not stall each other.  The old one-CTA-per-unit kernel serialised load -> MMA ->
-// softmax -> MMA inside a CTA and relied on 2-4 co-resident CTAs for overlap.
-// ---------------------------------------------------------------------------------------------------------------
-// kSingle: every sequence fits one 128-key tile (max_seqlen <= 128: configs 1-2 and all NLI models).  Then a unit is ONE
-// key tile: Q and K are dead once S = Q K^T has completed, so P re-uses Q|K and O re-uses S's TMEM columns — 48 KB of smem
-// and 128 TMEM columns per slot at hd 64, i.e. FOUR slots per CTA (four softmax warpgroups): with ~2 us of load latency
-// per unit and only ~2 us of work, four units in flight per SM are what keeps the HBM stream busy.
-template <int HD, bool kSingle>
-struct AttnWsCfg {
-  static constexpr int kSub = HD / 64;
-  static constexpr int kQBytes = kSub * kSubBytes;            // Q / K / V tile bytes
-  static constexpr int kKPBytes = 2 * kSubBytes;              // multi-tile: the K region also hosts P [128 x 128] bf16
-  static constexpr int kStageBytes = kKPBytes + kQBytes;      // multi-tile stage { K|P , V }
-  static constexpr int kNKV = kSingle ? 1 : ((HD == 64) ? 2 : 1);
-  static constexpr int kSlots = (kSingle && HD == 64) ? 4 : 2;
-  static constexpr int kSlotBytes = kSingle ? 3 * kQBytes : kQBytes + kNKV * kStageBytes;
-  static constexpr int kBarBytes = 1024;
-  static constexpr int kSmemBytes = 1024 + kSlots * kSlotBytes + kBarBytes;
-  static constexpr int kTmemCols = 512;
-  static constexpr int kTmemSlot = kSingle ? 128 : 256;       // columns per slot: S at +0, O at +128 (single: O over S)
-  static constexpr int kThreads = 32 * (4 * kSlots + 2);
-  static_assert(kSmemBytes <= 232448, "attention: exceeds the 227 KB per-CTA shared memory limit");
-  static_assert(HD == 64 || HD == 128, "warp-specialised attention: head_dim 64 or 128");
-  static_assert(!kSingle || 2 * kQBytes >= 2 * kSubBytes, "P must fit into Q|K");
-};
-
-struct AttnUnit {
-  int b, h, qt;     // sequence, head, query tile
-  int seq0, len;    // first token row / length of the sequence
-  int j_lo, j_hi;   // key tiles visited
-};
-
-// unit number -> work description; false when the unit does not exist (query tile beyond the sequence's length)
-__device__ __forceinline__ bool attn_unit(int u, int B, int H, int QT, int window, const int32_t* __restrict__ cu,
-                                          AttnUnit& w) {
-  const int bh = B * H;
-  w.qt = QT - 1 - u / bh;  // heaviest query tiles (most key tiles) first
-  const int r = u % bh;
-  w.b = r / H;
-  w.h = r % H;
-  w.seq0 = __ldg(cu + w.b);
-  w.len = __ldg(cu + w.b + 1) - w.seq0;
-  const int qp0 = w.qt * kAttnTile;
-  if (qp0 >= w.len) return false;
-  const int lo_pos = (window > 0) ? max(0, qp0 - window + 1) : 0;
-  w.j_lo = lo_pos / kAttnTile;
-  w.j_hi = w.qt;
-  return true;
-}
-
-template <int HD, bool kSingle>
-__global__ void __launch_bounds__(AttnWsCfg<HD, kSingle>::kThreads, 1)
-attention_ws_kernel(const __grid_constant__ CUtensorMap tma_qkv, __nv_bfloat16* __restrict__ out,
-                    const int32_t* __restrict__ cu, int B, int H, int QT, float sl2, int window,
-                    const float* __restrict__ alibi) {
-  using Cfg = AttnWsCfg<HD, kSingle>;
-  constexpr int NKV = Cfg::kNKV, NS = Cfg::kSlots;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  // barriers, per slot: q_full q_empty s_full p_full o_full o_empty | k_full[NKV] v_full[NKV] kv_empty[NKV]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + NS * Cfg::kSlotBytes);
-  constexpr int kBarsPerSlot = 6 + 3 * NKV;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + NS * kBarsPerSlot);
-  auto bar = [&](int s, int i) { return bars + s * kBarsPerSlot + i; };
-  enum { Q_FULL = 0, Q_EMPTY = 1, S_FULL = 2, P_FULL = 3, O_FULL = 4, O_EMPTY = 5, K_FULL = 6, V_FULL = 6 + NKV,
-         KV_EMPTY = 6 + 2 * NKV };
-  // smem: single  [Q | K | V] per slot, P over Q|K;   multi  [Q | NKV x {K (P) | V}]
-  auto slot_q = [&](int s) { return smem + s * Cfg::kSlotBytes; };
-  auto slot_k = [&](int s, int st) {
-    return kSingle ? smem + s * Cfg::kSlotBytes + Cfg::kQBytes
-                   : smem + s * Cfg::kSlotBytes + Cfg::kQBytes + st * Cfg::kStageBytes;
-  };
-  auto slot_v = [&](int s, int st) { return kSingle ? smem + s * Cfg::kSlotBytes + 2 * Cfg::kQBytes : slot_k(s, st) + Cfg::kKPBytes; };
-  auto slot_p = [&](int s, int st) { return kSingle ? slot_q(s) : slot_k(s, st); };
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  constexpr int kWarpProducer = 4 * NS, kWarpMma = 4 * NS + 1;
-  const int d = H * HD;
-  const int n_units = QT * B * H;
-  const int stride = NS * static_cast<int>(gridDim.x);
-
-  if (warp == kWarpProducer && lane == 0) {
-    tma_prefetch_desc(&tma_qkv);
-    for (int s = 0; s < NS; ++s) {
-      mbar_init(bar(s, Q_FULL), 1);
-      mbar_init(bar(s, Q_EMPTY), 1);
-      mbar_init(bar(s, S_FULL), 1);
-      mbar_init(bar(s, P_FULL), 128);
-      mbar_init(bar(s, O_FULL), 1);
-      mbar_init(bar(s, O_EMPTY), 128);
-      for (int i = 0; i < NKV; ++i) {
-        mbar_init(bar(s, K_FULL + i), 1);
-        mbar_init(bar(s, V_FULL + i), 1);
-        mbar_init(bar(s, KV_EMPTY + i), 1);
-      }
-    }
-    fence_mbar_init();
-  }
-  if (warp == kWarpMma) {
-    tmem_alloc(tmem_holder, Cfg::kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
-  pdl_sync();  // cu_seqlens is written by a copy, qkv by the previous kernel: nothing global is read above this line
-
-  if (warp == kWarpProducer) {
-    // ===================== TMA producer (all slots, non-blocking round robin) =====================
-    if (lane == 0) {
-      int u[NS], j[NS];
-      bool have[NS], q_sent[NS], done[NS];
-      AttnUnit w[NS];
-      uint32_t nq[NS], nkv[NS];  // Q tiles / KV tiles issued so far per slot
-      int n_done = 0;
-#pragma unroll
-      for (int s = 0; s < NS; ++s) {
-        u[s] = NS * static_cast<int>(blockIdx.x) + s;
-        j[s] = 0; have[s] = false; q_sent[s] = false; done[s] = false; nq[s] = 0; nkv[s] = 0;
-      }
-      uint32_t idle = 0;  // consecutive polls without progress: a protocol bug traps instead of hanging the GPU
-      while (n_done < NS) {
-        if (++idle > (1u << 26)) {
-          printf("sgpt: attention producer stalled (block %d)\n", blockIdx.x);
-          __trap();
-        }
-#pragma unroll
-        for (int s = 0; s < NS; ++s) {
-          if (done[s]) continue;
-          if (!have[s]) {
-            while (u[s] < n_units && !attn_unit(u[s], B, H, QT, window, cu, w[s])) u[s] += stride;
-            if (u[s] >= n_units) { done[s] = true; ++n_done; continue; }
-            have[s] = true;
-            q_sent[s] = false;
-            j[s] = w[s].j_lo;
-          }
-          const int st = static_cast<int>(nkv[s] % NKV);
-          if (kSingle) {
-            // one stage holds Q, K and V of the unit; it is free once the previous unit's P V (which read P over Q|K, and V)
-            // has completed
-            if (!mbar_test_wait(bar(s, KV_EMPTY), (nkv[s] & 1u) ^ 1u)) continue;
-          } else if (!q_sent[s]) {
-            // the Q buffer is free once every S MMA of the previous unit has completed
-            if (!mbar_test_wait(bar(s, Q_EMPTY), (nq[s] & 1u) ^ 1u)) continue;
-          }
-          if (!q_sent[s]) {
-            mbar_expect_tx(bar(s, Q_FULL), Cfg::kQBytes);
-            for (int x = 0; x < Cfg::kSub; ++x)
-              tma_load_2d(slot_q(s) + x * kSubBytes, &tma_qkv, bar(s, Q_FULL), w[s].h * HD + 64 * x,
-                          w[s].seq0 + w[s].qt * kAttnTile);
-            ++nq[s];
-            q_sent[s] = true;
-          }
-          if (!kSingle && !mbar_test_wait(bar(s, KV_EMPTY + st), ((nkv[s] / NKV) & 1u) ^ 1u)) continue;
-          mbar_expect_tx(bar(s, K_FULL + st), Cfg::kQBytes);
-          for (int x = 0; x < Cfg::kSub; ++x)
-            tma_load_2d(slot_k(s, st) + x * kSubBytes, &tma_qkv, bar(s, K_FULL + st), d + w[s].h * HD + 64 * x,
-                        w[s].seq0 + j[s] * kAttnTile);
-          mbar_expect_tx(bar(s, V_FULL + st), Cfg::kQBytes);
-          for (int x = 0; x < Cfg::kSub; ++x)
-            tma_load_2d(slot_v(s, st) + x * kSubBytes, &tma_qkv, bar(s, V_FULL + st), 2 * d + w[s].h * HD + 64 * x,
-                        w[s].seq0 + j[s] * kAttnTile);
-          ++nkv[s];
-          idle = 0;
-          if (++j[s] > w[s].j_hi) {
-            have[s] = false;
-            u[s] += stride;
-          }
-        }
-      }
-    }
-  } else if (warp == kWarpMma) {
-    // ===================== MMA issuer (all slots, non-blocking round robin) =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, false);
-      constexpr uint32_t idesc_o = make_idesc_bf16(128, HD, true);
-      int u[NS], j[NS];
-      bool have[NS], want_pv[NS], done[NS];
-      AttnUnit w[NS];
-      uint32_t nq[NS], nt[NS];  // units started / key tiles completed per slot
-      int n_done = 0;
-#pragma unroll
-      for (int s = 0; s < NS; ++s) {
-        u[s] = NS * static_cast<int>(blockIdx.x) + s;
-        j[s] = 0; have[s] = false; want_pv[s] = false; done[s] = false; nq[s] = 0; nt[s] = 0;
-      }
-      uint32_t idle = 0;
-      while (n_done < NS) {
-        if (++idle > (1u << 26)) {
-          printf("sgpt: attention MMA issuer stalled (block %d)\n", blockIdx.x);
-          __trap();
-        }
-#pragma unroll
-        for (int s = 0; s < NS; ++s) {
-          if (done[s]) continue;
-          if (!have[s]) {
-            while (u[s] < n_units && !attn_unit(u[s], B, H, QT, window, cu, w[s])) u[s] += stride;
-            if (u[s] >= n_units) { done[s] = true; ++n_done; continue; }
-            have[s] = true;
-            j[s] = w[s].j_lo;
-            want_pv[s] = false;
-          }
-          const int st = static_cast<int>(nt[s] % NKV);
-          const uint32_t st_par = (nt[s] / NKV) & 1u;
-          const uint32_t tS = tmem_base + s * Cfg::kTmemSlot, tO = kSingle ? tS : tS + 128;
-          if (!want_pv[s]) {
-            // ---- S = Q K_j^T ---- (multi: the S columns are free, this slot's previous P V waited for p_full of the previous
-            // tile; single: S shares its columns with O, which the epilogue of the previous unit must have read)
-            if (j[s] == w[s].j_lo && !mbar_test_wait(bar(s, Q_FULL), nq[s] & 1u)) continue;
-            if (!mbar_test_wait(bar(s, K_FULL + st), st_par)) continue;
-            if (kSingle && !mbar_test_wait(bar(s, O_EMPTY), (nq[s] & 1u) ^ 1u)) continue;
-            tc_fence_after();
-            const uint32_t aq = smem_u32(slot_q(s)), ak = smem_u32(slot_k(s, st));
-#pragma unroll
-            for (int kk = 0; kk < HD / 16; ++kk) {
-              const uint32_t off = (kk >> 2) * kSubBytes + (kk & 3) * 32;
-              umma_bf16_ss(tS, make_smem_desc_sw128(aq + off, 16, 1024), make_smem_desc_sw128(ak + off, 16, 1024),
-                           idesc_s, kk != 0);
-            }
-            umma_commit(bar(s, S_FULL));
-            idle = 0;
-            if (j[s] == w[s].j_hi) {  // last S of the unit: (multi) Q may be overwritten once these MMAs are done
-              if (!kSingle) umma_commit(bar(s, Q_EMPTY));
-              ++nq[s];
-            }
-            want_pv[s] = true;
-          } else {
-            // ---- O += P V_j ----
-            if (!mbar_test_wait(bar(s, P_FULL), nt[s] & 1u)) continue;
-            if (!mbar_test_wait(bar(s, V_FULL + st), st_par)) continue;
-            tc_fence_after();
-            const uint32_t ap = smem_u32(slot_p(s, st)), av = smem_u32(slot_v(s, st));
-#pragma unroll
-            for (int kk = 0; kk < kAttnTile / 16; ++kk) {
-              const uint64_t da = make_smem_desc_sw128(ap + (kk >> 2) * kSubBytes + (kk & 3) * 32, 16, 1024);
-              const uint64_t db = make_smem_desc_sw128(av + kk * 2048, kSubBytes, 1024);
-              umma_bf16_ss(tO, da, db, idesc_o, (j[s] > w[s].j_lo) || (kk != 0));
-            }
-            umma_commit(bar(s, KV_EMPTY + st));  // the stage (P, and V; single: Q|K too) may be refilled
-            umma_commit(bar(s, O_FULL));
-            idle = 0;
-            ++nt[s];
-            want_pv[s] = false;
-            if (++j[s] > w[s].j_hi) {
-              have[s] = false;
-              u[s] += stride;
-            }
-          }
-        }
-      }
-    }
-  } else {
-    // ===================== softmax / correction / epilogue warpgroups =====================
-    const int s = warp >> 2;            // slot
-    const int row = tid & 127;          // query row of the tile == TMEM lane
-    const uint32_t lane_off = static_cast<uint32_t>((warp & 3) * 32) << 16;
-    const uint32_t tS = tmem_base + s * Cfg::kTmemSlot + lane_off, tO = kSingle ? tS : tS + 128;
-    uint32_t nt = 0;                    // key tiles completed by this slot
-    AttnUnit w;
-    for (int u = NS * static_cast<int>(blockIdx.x) + s; u < n_units; u += stride) {
-      if (!attn_unit(u, B, H, QT, window, cu, w)) continue;
-      const int qp0 = w.qt * kAttnTile;
-      const float slope2 = (alibi != nullptr) ? __ldg(alibi + w.h) * 1.4426950408889634f : 0.f;
-      const RowVis rv = make_row_vis(qp0, row, w.len, window);
-      float m_run = -INFINITY, l_run = 0.f;
-      for (int j = w.j_lo; j <= w.j_hi; ++j, ++nt) {
-        const int st = static_cast<int>(nt % NKV);
-        const uint32_t sP = smem_u32(slot_p(s, st));
-        mbar_wait(bar(s, S_FULL), nt & 1u);
-        tc_fence_after();
-        const int kv0 = j * kAttnTile;
-        const float m_new = fmaxf(m_run, softmax_tile_max(tS, kv0, rv, sl2, slope2));
-        const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
-        const float alpha = exp2f(m_run - m_use);
-        // P over the K tile of this stage (single: over Q|K): the S MMAs that read them have completed (s_full)
-        const float lsum = softmax_tile_exp(tS, kv0, rv, sl2, slope2, m_use, sP, row);
-        l_run = l_run * alpha + lsum;
-        if (!kSingle && j > w.j_lo) {
-          // O = alpha * O once the previous tile's P V has landed; skipped by a warp whose rows all kept their maximum
-          // (alpha == 1 exactly): the usual case after the first key tiles
-          mbar_wait(bar(s, O_FULL), (nt - 1u) & 1u);
-          tc_fence_after();
-          if (__any_sync(0xffffffffu, m_new != m_run)) {
-#pragma unroll 1
-            for (int c = 0; c < HD / 32; ++c) {
-              uint32_t o[32];
-              tmem_ld_32x32(tO + c * 32, o);
-              tmem_ld_wait();
-#pragma unroll
-              for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-              tmem_st_32x32(tO + c * 32, o);
-            }
-            tmem_st_wait();
-          }
-        }
-        m_run = m_new;
-        fence_proxy_async_smem();  // P (generic-proxy stores) -> visible to the tensor core
-        tc_fence_before();
-        mbar_arrive(bar(s, P_FULL));
-      }
-      // ---- epilogue: O / l -> bf16 -> out[token, head] ----
-      mbar_wait(bar(s, O_FULL), (nt - 1u) & 1u);
-      tc_fence_after();
-      const float inv_l = (l_run > 0.f) ? 1.0f / l_run : 0.f;
-      const bool row_ok = qp0 + row < w.len;
-      __nv_bfloat16* dst = out + static_cast<size_t>(w.seq0 + qp0 + row) * d + w.h * HD;
-#pragma unroll 1
-      for (int c = 0; c < HD / 32; ++c) {
-        uint32_t o[32];
-        tmem_ld_32x32(tO + c * 32, o);
-        tmem_ld_wait();
-        if (row_ok) {
-          uint4* d4 = reinterpret_cast<uint4*>(dst + c * 32);
-#pragma unroll
-          for (int q4 = 0; q4 < 4; ++q4) {
-            uint32_t pk[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-              pk[i] = pack_bf16(__uint_as_float(o[8 * q4 + 2 * i]) * inv_l, __uint_as_float(o[8 * q4 + 2 * i + 1]) * inv_l);
-            d4[q4] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-          }
-        }
-      }
-      tc_fence_before();
-      // single: O shares its TMEM columns with the next unit's S — tell the MMA issuer they have been read.  (multi: the
-      // next unit's first P V (accumulate = 0) overwrites O only after this warpgroup's p_full arrivals, which follow
-      // these loads in program order.)
-      if (kSingle) mbar_arrive(bar(s, O_EMPTY));
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kWarpMma) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
-  }
-}
-
-template <int HD, bool kSingle>
-static int launch_attention_ws_impl(const CUtensorMap& map, void* out, const int32_t* cu, int B, int H, float scale,
-                                    int window, int max_seqlen, const float* alibi, cudaStream_t stream) {
-  using Cfg = AttnWsCfg<HD, kSingle>;
-  auto kern = attention_ws_kernel<HD, kSingle>;
-  static PerDeviceOnce attr_once;
-  if (attr_once.first())
-    SGPT_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-  const int QT = (max_seqlen + kAttnTile - 1) / kAttnTile;
-  const long long units = static_cast<long long>(QT) * B * H;
-  long long ctas = (units + Cfg::kSlots - 1) / Cfg::kSlots;
-  if (ctas > sm_count()) ctas = sm_count();
-  if (ctas < 1) ctas = 1;
-  const float sl2 = scale * 1.4426950408889634f;
-  LaunchScope _ls(kCatAttention, stream);
-  SGPT_CHECK_CUDA(launch_kernel(kern, dim3(static_cast<unsigned>(ctas)), dim3(Cfg::kThreads), Cfg::kSmemBytes, stream, map,
-                                static_cast<__nv_bfloat16*>(out), cu, B, H, QT, sl2, window, alibi));
-  return SGPT_OK;
 }
 
 template <int HD>
-static int launch_attention_ws(const void* qkv, void* out, const int32_t* cu, int B, int T, int H, float scale, int window,
-                               int max_seqlen, const float* alibi, cudaStream_t stream) {
-  CUtensorMap map;
-  int rc = make_tma_2d_bf16(&map, qkv, static_cast<uint64_t>(T), 3ull * H * HD, 3ull * H * HD, kAttnTile, 64);
-  if (rc != SGPT_OK) return rc;
-  if (max_seqlen <= kAttnTile)
-    return launch_attention_ws_impl<HD, true>(map, out, cu, B, H, scale, window, max_seqlen, alibi, stream);
-  return launch_attention_ws_impl<HD, false>(map, out, cu, B, H, scale, window, max_seqlen, alibi, stream);
+static int launch_attention_mma(const void* qkv, void* out, const int32_t* cu, int B, int H, float scale, int window,
+                                int max_seqlen, const float* alibi, cudaStream_t stream) {
+  using Cfg = AttnCfg<HD>;
+  auto kern = attention_mma_kernel<HD>;
+  static PerDeviceOnce attr_once;
+  if (attr_once.first())
+    SGPT_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+  const int QT = (max_seqlen + kAttnQ - 1) / kAttnQ;
+  const float sl2 = scale * 1.4426950408889634f;
+  LaunchScope _ls(kCatAttention, stream);
+  SGPT_CHECK_CUDA(launch_kernel(kern, dim3(H, B, QT), dim3(kAttnThreads), Cfg::kSmemBytes, stream,
+                                static_cast<const __nv_bfloat16*>(qkv), static_cast<__nv_bfloat16*>(out), cu, H, sl2, window,
+                                alibi));
+  return SGPT_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -852,52 +303,6 @@ __global__ void __launch_bounds__(256) attention_simt_kernel(const __nv_bfloat16
     out[static_cast<size_t>(t) * d + h * HD + lane * E + e] = __float2bfloat16_rn(o[e] / l);
 }
 
-template <int HD, bool kSingle>
-static int launch_attention_tc_impl(const CUtensorMap& map, void* out, const int32_t* cu, int B, int H, float scale,
-                                    int window, int max_seqlen, const float* alibi, cudaStream_t stream) {
-  using Cfg = AttnCfg<HD, kSingle>;
-  auto kern = attention_tc_kernel<HD, kSingle>;
-  static PerDeviceOnce attr_once;
-  if (attr_once.first()) {
-    SGPT_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-  }
-  // SGPT_ATTN_HEAD_MAJOR=0: round-1 grid order (query tile fastest, heads slowest)
-  static const int head_major = [] { const char* e = getenv("SGPT_ATTN_HEAD_MAJOR"); return (e != nullptr && e[0] == '0') ? 0 : 1; }();
-  const int QT = (max_seqlen + kAttnTile - 1) / kAttnTile;
-  dim3 grid = head_major ? dim3(H, B, QT) : dim3(QT, B, H);
-  const float sl2 = scale * 1.4426950408889634f;
-  LaunchScope _ls(kCatAttention, stream);
-  // SGPT_ATTN_PREFETCH=0 turns the L2 prefetch of the successor unit off; the distance is one full set of resident CTAs
-  static const bool prefetch_on = [] { const char* e = getenv("SGPT_ATTN_PREFETCH"); return !(e != nullptr && e[0] == '0'); }();
-  static PerDeviceOnce occ_once;
-  static int resident_per_sm = 1;
-  if (occ_once.first()) {
-    int n = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, 128, Cfg::kSmemBytes) == cudaSuccess && n > 0) {
-      // (TMEM: 512 columns per SM bound the co-resident CTAs as well)
-      const int by_tmem = 512 / Cfg::kTmemCols;
-      resident_per_sm = n < by_tmem ? n : by_tmem;
-    } else {
-      cudaGetLastError();
-    }
-  }
-  const int prefetch_ahead = (prefetch_on && head_major) ? resident_per_sm * sm_count() : 0;
-  SGPT_CHECK_CUDA(launch_kernel(kern, grid, dim3(128), Cfg::kSmemBytes, stream, map, static_cast<__nv_bfloat16*>(out), cu,
-                                H, sl2, window, alibi, head_major, prefetch_ahead));
-  return SGPT_OK;
-}
-
-template <int HD>
-static int launch_attention_tc(const void* qkv, void* out, const int32_t* cu, int B, int T, int H, float scale,
-                               int window, int max_seqlen, const float* alibi, cudaStream_t stream) {
-  CUtensorMap map;
-  int rc = make_tma_2d_bf16(&map, qkv, static_cast<uint64_t>(T), 3ull * H * HD, 3ull * H * HD, kAttnTile, 64);
-  if (rc != SGPT_OK) return rc;
-  if (max_seqlen <= kAttnTile)  // one key tile per sequence: compact variant, up to 4 CTAs per SM
-    return launch_attention_tc_impl<HD, true>(map, out, cu, B, H, scale, window, max_seqlen, alibi, stream);
-  return launch_attention_tc_impl<HD, false>(map, out, cu, B, H, scale, window, max_seqlen, alibi, stream);
-}
-
 template <int HD>
 static int launch_attention_simt(const void* qkv, void* out, const int32_t* cu, int B, int T, int H, float scale,
                                  int window, const float* alibi, cudaStream_t stream) {
@@ -908,28 +313,9 @@ static int launch_attention_simt(const void* qkv, void* out, const int32_t* cu, 
                                 scale, window, alibi));
   return SGPT_OK;
 }
-
 }  // namespace sgpt
 
 using namespace sgpt;
-
-// SGPT_ATTN_IMPL=legacy routes impl 0 to the one-CTA-per-unit kernel (A/B measurements)
-static bool attention_legacy_forced() {
-  static const bool v = [] {
-    const char* e = getenv("SGPT_ATTN_IMPL");
-    return e != nullptr && e[0] == 'l';
-  }();
-  return v;
-}
-
-// SGPT_ATTN_WS_SINGLE=1 routes batches whose sequences all fit one key tile to the persistent 4-slot variant (A/B)
-static bool attention_ws_single() {
-  static const bool v = [] {
-    const char* e = getenv("SGPT_ATTN_WS_SINGLE");
-    return e != nullptr && e[0] == '1';
-  }();
-  return v;
-}
 
 extern "C" int sgpt_attention(const void* qkv, void* out, const int32_t* cu_seqlens, int B, int T, int H, int hd,
                               float scale, int window, int max_seqlen, const float* alibi_slopes, int impl,
@@ -941,23 +327,13 @@ extern "C" int sgpt_attention(const void* qkv, void* out, const int32_t* cu_seql
   SGPT_REQUIRE(window >= 0, "sgpt_attention: window must be >= 0");
   SGPT_REQUIRE(max_seqlen > 0 || T == 0, "sgpt_attention: max_seqlen must be positive");
   if (B == 0 || T == 0) return SGPT_OK;
-  if (impl == 0 && hd != 256 && (max_seqlen > 128 || attention_ws_single()) && !attention_legacy_forced()) {
-    // Warp-specialised persistent kernel (two work slots per CTA) for sequences of more than one key tile: measured
-    // 1.5-1.7x the one-CTA-per-unit kernel (SGPT-1.3B 64 x 256: 3.76 -> 2.18 ms per batch, bloom-7b1 32 x 300: 8.74 ->
-    // 5.83 ms; a variant with 64-key tiles double-buffered at hd 128 and a 4-slot single-tile variant both measured slower
-    // and were dropped, DESIGN.md §7).  head_dim 256 (GPT-J: one slot would fill the SM's smem) and batches whose sequences all fit ONE key tile
-    // (there four co-resident single-tile CTAs per SM beat two slots: 0.745 vs 0.886 ms per 125M step) keep the
-    // one-CTA-per-unit kernel.
-    SGPT_REQUIRE(static_cast<long long>(B) * H * ((max_seqlen + 127) / 128) < (1ll << 30), "sgpt_attention: too many work units");
-    if (hd == 64) return launch_attention_ws<64>(qkv, out, cu_seqlens, B, T, H, scale, window, max_seqlen, alibi_slopes, stream);
-    return launch_attention_ws<128>(qkv, out, cu_seqlens, B, T, H, scale, window, max_seqlen, alibi_slopes, stream);
-  }
   if (impl == 0 || impl == 2) {
-    SGPT_REQUIRE(H <= 65535 && B <= 65535, "sgpt_attention: grid limits exceeded (B=%d H=%d)", B, H);
+    SGPT_REQUIRE(H <= 65535 && B <= 65535 && (max_seqlen + kAttnQ - 1) / kAttnQ <= 65535,
+                 "sgpt_attention: grid limits exceeded (B=%d H=%d max_seqlen=%d)", B, H, max_seqlen);
     switch (hd) {
-      case 64: return launch_attention_tc<64>(qkv, out, cu_seqlens, B, T, H, scale, window, max_seqlen, alibi_slopes, stream);
-      case 128: return launch_attention_tc<128>(qkv, out, cu_seqlens, B, T, H, scale, window, max_seqlen, alibi_slopes, stream);
-      default: return launch_attention_tc<256>(qkv, out, cu_seqlens, B, T, H, scale, window, max_seqlen, alibi_slopes, stream);
+      case 64: return launch_attention_mma<64>(qkv, out, cu_seqlens, B, H, scale, window, max_seqlen, alibi_slopes, stream);
+      case 128: return launch_attention_mma<128>(qkv, out, cu_seqlens, B, H, scale, window, max_seqlen, alibi_slopes, stream);
+      default: return launch_attention_mma<256>(qkv, out, cu_seqlens, B, H, scale, window, max_seqlen, alibi_slopes, stream);
     }
   } else if (impl == 1) {
     switch (hd) {

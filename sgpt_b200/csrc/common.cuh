@@ -1,8 +1,8 @@
-// sm_100a building blocks shared by every kernel in this library: mbarrier, TMA, tcgen05 (UMMA / TMEM)
-// PTX wrappers, UMMA descriptor encoders, and small numeric helpers.
+// sm_90a building blocks shared by every kernel in this library: mbarrier, TMA and wgmma PTX wrappers, the wgmma
+// shared-memory descriptor encoder, and small numeric helpers.
 //
-// Everything here is hand-written inline PTX for sm_100a (no CUTLASS/CuTe).  Descriptor bit layouts follow the
-// PTX ISA "tcgen05 matrix descriptor" / "instruction descriptor" tables.
+// Everything here is hand-written inline PTX for sm_90a (no CUTLASS/CuTe).  Descriptor bit layouts follow the PTX ISA
+// "warpgroup-level matrix shared memory layout" / "matrix descriptor" tables.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -52,7 +52,7 @@ __device__ __forceinline__ float bf16_hi(uint32_t v) { return __uint_as_float(v 
 // cudaLaunchAttributeProgrammaticStreamSerialization (host_utils.h: launch_kernel): its CTAs may become resident while the
 // previous kernel of the stream is still draining.  pdl_wait() blocks until every prerequisite grid has completed and
 // its memory is visible — it must precede the FIRST global-memory access of the kernel; what sits before it (barrier
-// init, TMEM allocation, descriptor prefetch, index arithmetic) overlaps the predecessor's tail.
+// init, descriptor prefetch, index arithmetic) overlaps the predecessor's tail.
 // pdl_launch_dependents() lets the NEXT kernel of the stream start the same way once all CTAs of this grid have
 // executed it (or exited).  Both are no-ops when the launch carried no such attribute.
 // ---------------------------------------------------------------------------------------------------------------
@@ -104,19 +104,17 @@ __device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Spin with a bounded poll count: a protocol bug traps (launch error) instead of hanging the GPU.
+// Spin with a bounded poll count: a protocol bug traps (launch error) instead of hanging the GPU.  No printf on the
+// timeout path: a function call anywhere between a wgmma and its wait makes ptxas serialise every wgmma of the kernel
+// (C7510), and the GEMM's consumers wait here while their previous k-block's wgmma group is still in flight.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t polls = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++polls > (1u << 24)) {
-      printf("sgpt: mbarrier wait timed out (block %d thread %d bar %p parity %u)\n", blockIdx.x, threadIdx.x,
-             (void*)bar, parity);
-      __trap();
-    }
+    if (++polls > (1u << 24)) __trap();
   }
 }
 
-// generic-proxy writes to smem -> visible to the async proxy (TMA / tcgen05 operand reads)
+// generic-proxy writes to smem -> visible to the async proxy (TMA stores / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -156,35 +154,12 @@ __device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* desc, int 
                : "memory");
 }
 
-// Multicast tile load: the tile lands at the same smem offset in every CTA of the cluster whose bit is set in
-// cta_mask, and each destination CTA's mbarrier (same offset) receives the complete_tx.  One L2 read feeds all of them.
-__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* desc, uint64_t* bar, int c0,
-                                                      int c1, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%3, %4}], [%2], %5;"
-      :
-      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
-        "h"(cta_mask)
-      : "memory");
-}
-
 // 1-D bulk copy global -> shared (contiguous bytes; size and both addresses multiples of 16), completion on an mbarrier
 __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
                    smem_u32(smem_dst)),
                "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
-}
-
-// thread-block cluster helpers
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
 // smem tile -> global (bulk async-group completion).  Coordinates as for loads; out-of-range rows/columns are clipped.
@@ -233,184 +208,89 @@ __device__ __forceinline__ float2 lds_v2(uint32_t addr) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, load
+// wgmma (warpgroup MMA, sm_90a): shared-memory matrix descriptors, ordering fences, bf16 m64nNk16 with fp32 accumulators
+// held in the registers of the issuing warpgroup
 // ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_holder, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// Same, arriving on the barrier at this smem offset in every CTA of the cluster selected by cta_mask.
-__device__ __forceinline__ void umma_commit_multicast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 inputs, fp32 accumulate.
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      :
-      : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// A operand read from TMEM (packed bf16 pairs per 32-bit column), B from smem.
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n"
-      :
-      : "r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// ---- CTA-pair (cta_group::2) variants: the two CTAs of a 2-CTA cluster (one TPC) execute ONE M=256 MMA.  Each CTA holds
-// its own 128 rows of A, HALF of the B tile (N/2 rows) and its own 128 accumulator rows in TMEM; the leader CTA (rank 0)
-// issues the MMAs for both.  Compared with two independent M=128 MMAs the per-SM smem footprint, TMA write traffic and
-// operand read traffic of B halve, which is what leaves smem bandwidth for the epilogue.
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_holder, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_bf16_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                  uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      :
-      : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive (once all previously issued pair MMAs completed) on the barrier at this smem offset in the CTAs of cta_mask.
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-// shared::cluster address of `local` (a shared::cta address of this CTA) in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t local, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local), "r"(rank));
-  return r;
-}
-// arrive on an mbarrier that may live in another CTA of the cluster (address from mapa_shared)
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// Tile load into THIS CTA's smem whose complete_tx is delivered to a barrier in the pair's leader CTA
-// (bar_cluster_addr from mapa_shared(.., 0)); .cta_group::2 is what permits the barrier to live in the peer.
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const CUtensorMap* desc, uint32_t bar_cluster_addr,
-                                                 int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      :
-      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(desc)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-
-// The same, MULTICAST: the tile lands at this smem offset in every CTA of `cta_mask`; each destination CTA's complete_tx is
-// delivered to the mbarrier at `bar_addr`'s CTA-relative offset in the LEADER (even-ranked CTA) of the destination's own
-// pair — bar_addr is the shared::cluster address of the barrier in the ISSUING CTA's pair leader (mapa).  Used by the
-// 4-CTA cluster GEMM: two CTA pairs share every weight tile, fetched from L2 once.
-__device__ __forceinline__ void tma_load_2d_pair_multicast(void* smem_dst, const CUtensorMap* desc, uint32_t bar_addr,
-                                                           int c0, int c1, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%3, %4}], [%2], %5;"
-      :
-      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(desc)), "r"(bar_addr), "r"(c0), "r"(c1), "h"(cta_mask)
-      : "memory");
-}
-
-// Instruction descriptor for kind::f16 with bf16 A/B and fp32 D.
-//   [4,6) D format (1 = f32)   [7,10) A format (1 = bf16)   [10,13) B format (1 = bf16)
-//   [15] A major (0 = K)       [16] B major (0 = K, 1 = MN) [17,23) N >> 3            [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int m, int n, bool b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (0u << 15) | ((b_mn_major ? 1u : 0u) << 16) |
-         (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor, SWIZZLE_128B, for tiles written by TMA with a 128-byte inner box.
-//   [0,14) start >> 4   [16,30) LBO >> 4   [32,46) SBO >> 4   [46,48) version = 1   [61,64) layout (2 = SW128)
-// K-major operand (rows of 64 bf16 = 128 B, 8-row swizzle atoms): SBO = 1024 B, LBO unused (encoded 1).
-// MN-major operand (each K index is one 128-B row of 64 MN elements): SBO = 1024 B (8 K rows),
-//   LBO = byte distance between consecutive 64-element MN groups.
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                         uint32_t sbo_bytes) {
+// Shared-memory matrix descriptor of a K-major operand written by TMA with SWIZZLE_128B (rows of 64 bf16 = 128 B, 8-row
+// swizzle atoms of 1024 B; the tile base is 1024-byte aligned).
+//   [0,14) start >> 4   [16,30) LBO >> 4 (unused for swizzled K-major: 1)   [32,46) SBO >> 4 = 1024 B   [62,64) 1 = SW128
+// Advancing 16 bf16 (32 B) along K inside the swizzle row adds 2 to the start field.
+__device__ __forceinline__ uint64_t make_wgmma_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= 1ull << 46;
-  d |= 2ull << 61;
+  d |= static_cast<uint64_t>(1u) << 16;
+  d |= static_cast<uint64_t>(1024u >> 4) << 32;
+  d |= 1ull << 62;
   return d;
 }
-
-// TMEM -> registers: 32 lanes x 32 consecutive fp32 columns (thread i of the warp receives lane base+i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// wait until at most N committed wgmma groups of this warpgroup are still pending
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// registers -> TMEM (same shape as tmem_ld_32x32)
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, both operands K-major in shared memory; scale_d == 0 overwrites D.
+// Register i of thread t holds row 16 (t / 32) + (t % 32) / 4 + 8 ((i % 4) / 2), column 8 (i / 4) + 2 (t % 4) + i % 2.
+__device__ __forceinline__ void wgmma_bf16_m64n128(float (&d)[64], uint64_t desc_a, uint64_t desc_b, int scale_d) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      :
-      : "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]),
-        "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]),
-        "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_bf16_m64n256(float (&d)[128], uint64_t desc_a, uint64_t desc_b, int scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, %128, %129, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(desc_a), "l"(desc_b), "r"(scale_d));
+}
+
+// named barrier over `count` threads (a multiple of 32) of the CTA
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 // ---------------------------------------------------------------------------------------------------------------
 // numerics

@@ -140,8 +140,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const void* x, const flo
 }
 
 // bf16 residual stream -> bf16 normalised row with 16-byte accesses (8 elements per load / store; the generic kernel above
-// would read a bf16 row with 8-byte loads and write with 8-byte stores: measured 1.2x SLOWER than its fp32-input form
-// although it moves a third fewer bytes).  May run in place (a thread rewrites only the chunks it read).
+// would read a bf16 row with 8-byte loads and write with 8-byte stores).  May run in place (a thread rewrites only the chunks it read).
 template <int TPR, int V8, int MINB = 1>
 __global__ void __launch_bounds__(256, MINB) layernorm_bf16_kernel(const uint4* x, const float4* __restrict__ g,
                                                              const float4* __restrict__ b, uint4* y, int T, int d8,
@@ -196,12 +195,10 @@ __global__ void __launch_bounds__(256, MINB) layernorm_bf16_kernel(const uint4* 
   }
 }
 
-// Persistent form of the kernel above (the default for d <= 768 and 1024 < d <= 4096).  tools/ln_bench.cu measured what
-// the one-row-per-group kernel spends its time on: with the gamma / beta loads removed it runs at the speed of a plain copy
-// (d 768: 18.6 us against 26.7 us per 32768-row pass; d 2048: 25.5 / 39.0; d 4096: 28.9 / 45.1) — every row re-reads
-// 8 bytes of gamma / beta per element through the L1 against 2 bytes of x.  Here a thread group keeps its gamma / beta
+// Persistent form of the kernel above (the default for d <= 768 and 1024 < d <= 4096).  In the one-row-per-group kernel every
+// row re-reads 8 bytes of gamma / beta per element through the L1 against 2 bytes of x (tools/ln_bench.cu times both).  Here a thread group keeps its gamma / beta
 // chunks in registers and walks over rows (grid = MINB CTAs per SM), with the next row's loads issued as soon as the
-// current row is unpacked: 22.4 / 28.6 / 32.8 us.  May run in place (a group rewrites only rows it has already read, and
+// current row is unpacked.  May run in place (a group rewrites only rows it has already read, and
 // the row it prefetches is a different one).
 template <int TPR, bool kWholeCta>
 __device__ __forceinline__ float group_sum_once(float v, float* scratch /* [ROWS][TPR/32] of one parity */, int row_in_cta,
@@ -889,8 +886,7 @@ extern "C" int sgpt_layernorm_ex(const void* x, int x_bf16, const float* gamma, 
     const uint4* xi = static_cast<const uint4*>(x);
     const float4 *gi = reinterpret_cast<const float4*>(gamma), *bi = reinterpret_cast<const float4*>(beta);
     uint4* yo = static_cast<uint4*>(y);
-    // SGPT_LN_BULK=1: rows staged through shared memory by bulk async copies — measured SLOWER (0.98 vs 0.79 ms per 125M
-    // step in the same call; 1.3B 2.4 -> 2.4, bloom 3.4 -> 4.2 ms), off by default
+    // SGPT_LN_BULK=1: rows staged through shared memory by bulk async copies, off by default
     static const bool bulk = [] { const char* e = getenv("SGPT_LN_BULK"); return e != nullptr && e[0] == '1'; }();
     if (bulk) {
       // stages of 8 rows; as many per CTA as ~48 KB hold (d 768: 4, d 2048: 1, d 4096: 1)

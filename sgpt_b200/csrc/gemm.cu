@@ -1,10 +1,9 @@
-// Host launchers for the tcgen05 GEMM (gemm.cuh): nn.Linear with fused epilogues (F3/F5/F6), the query x corpus
+// Host launchers for the wgmma GEMM (gemm.cuh): nn.Linear with fused epilogues (F3/F5/F6), the query x corpus
 // similarity (S1) and its threshold-filter variant used by the fused search (search.cu).
 #include "gemm.cuh"
 
 #include <stdlib.h>
 
-#include <type_traits>
 
 #include "../../include/sgpt_b200.h"
 #include "gemm_api.h"
@@ -16,14 +15,12 @@ template <int BN, class Epi, int CL = 1>
 static int launch_gemm(const void* a, int64_t lda, const void* b, int64_t ldb, int M, int N, int K,
                        const typename Epi::Params& ep, cudaStream_t stream, int cat = kCatGemm,
                        TileMap tmap = TileMap()) {
-  using Cfg = GemmCfg<BN, CL, EpiStaging<Epi>::value>;
+  using Cfg = GemmCfg<BN, EpiStaging<Epi>::value>;
   CUtensorMap ta, tb;
   int rc = make_tma_2d_bf16(&ta, a, static_cast<uint64_t>(M), static_cast<uint64_t>(K), static_cast<uint64_t>(lda),
                             kGemmBM, kGemmBK);
   if (rc != SGPT_OK) return rc;
-  // in a CTA pair each CTA holds half of the B tile; with two pairs per cluster (CL = 4) it fetches a quarter and
-  // receives the other quarter of its half by multicast from the CTA of its parity in the other pair
-  rc = make_tma_2d_bf16(&tb, b, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldb), BN / CL,
+  rc = make_tma_2d_bf16(&tb, b, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldb), BN,
                         kGemmBK);
   if (rc != SGPT_OK) return rc;
   auto kern = gemm_bf16_tn_kernel<BN, Epi, CL>;
@@ -33,149 +30,52 @@ static int launch_gemm(const void* a, int64_t lda, const void* b, int64_t ldb, i
   }
   const int m_tiles = ((M + kGemmBM - 1) / kGemmBM + CL - 1) / CL;
   const int n_tiles = tmap.count((N + BN - 1) / BN);
-  // work units (one per cluster iteration): tile groups x K slices
+  // work units (CL CTAs each): tile groups x K slices
   const long long tiles = static_cast<long long>(m_tiles) * n_tiles * tmap.ksplit;
   if (tiles == 0) return SGPT_OK;
-  long long clusters = sm_count() / CL;
-  cudaLaunchConfig_t cfg = {};
-  cfg.blockDim = dim3(128 + 32 * Epi::kEpiWarps);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  int na = 0;
-  if (CL == 4) {
-    // 4-CTA clusters cannot use every SM (GPCs whose SM count is not a multiple of 4): ask how many fit at once
-    static int max_clusters[64] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev >= 0 && dev < 64 && max_clusters[dev] == 0) {
-      cudaLaunchConfig_t q = cfg;
-      q.gridDim = dim3(static_cast<unsigned>(clusters * CL));
-      cudaLaunchAttribute qa[1];
-      qa[0].id = cudaLaunchAttributeClusterDimension;
-      qa[0].val.clusterDim.x = CL;
-      qa[0].val.clusterDim.y = 1;
-      qa[0].val.clusterDim.z = 1;
-      q.attrs = qa;
-      q.numAttrs = 1;
-      int n = 0;
-      if (cudaOccupancyMaxActiveClusters(&n, kern, &q) != cudaSuccess || n <= 0) {
-        cudaGetLastError();
-        n = static_cast<int>(clusters);
-      }
-      max_clusters[dev] = n;
-    }
-    if (dev >= 0 && dev < 64 && max_clusters[dev] > 0 && max_clusters[dev] < clusters) clusters = max_clusters[dev];
-  }
-  if (tiles < clusters) clusters = tiles;
-  cfg.gridDim = dim3(static_cast<unsigned>(clusters * CL));
-  if (CL > 1) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = CL;
-    attr[na].val.clusterDim.y = 1;
-    attr[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  if (pdl_enabled()) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = na;
+  long long units = sm_count() / CL;
+  if (tiles < units) units = tiles;
   LaunchScope _ls(cat, stream);
-  SGPT_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, M, N, K, ep, tmap));
+  SGPT_CHECK_CUDA(launch_kernel(kern, dim3(static_cast<unsigned>(units * CL)), dim3(kGemmThreads), Cfg::kSmemBytes, stream,
+                                ta, tb, M, N, K, ep, tmap));
   return SGPT_OK;
 }
 
-// SGPT_GEMM_CL4=1 enables the 4-CTA (two pairs, multicast weights) clusters.  Measured on B200 (profiles/
-// r02_gemm_epilogues_cl4_vs_cl2.jsonl): correct, but 3-8 % SLOWER than plain pairs on every encoder shape — the mainloop
-// is not bound by the L2 -> SM stream the multicast relieves but by the per-SM shared-memory fill, which is unchanged —
-// so it stays off by default.
-static bool cl4_enabled() {
-  static const bool v = [] {
-    const char* e = getenv("SGPT_GEMM_CL4");
-    return e != nullptr && e[0] == '1';
-  }();
-  return v;
-}
-
-// nn.Linear dispatch: tile width by wave efficiency; CTA pairs (cta_group::2, M = 256) whenever there are at least two
-// M-tiles — a third less L2->SM and smem traffic per FLOP than independent CTAs; two pairs per cluster sharing the weight
-// tile by multicast (another quarter less L2->SM traffic) when there are at least four M-tiles and 256-wide tiles.
-// Tile rasterisation (gemm.cuh TileMap::band): banded M-fastest order once the weight matrix no longer fits in the L2
-// next to the activations.  SGPT_GEMM_BAND=<g> forces a band height (0 = N fastest) for A/B measurements; read per call.
+// nn.Linear dispatch: 128 x 128 tiles (the 128 x 128 fp32 accumulator the epilogue reads back from shared memory leaves room
+// for four operand stages; 256-wide tiles would leave one).  Tile rasterisation (gemm.cuh TileMap::band): banded M-fastest
+// order once the weight matrix no longer fits in the H100's 50 MB L2 next to the activations.  SGPT_GEMM_BAND=<g> forces a
+// band height (0 = N fastest) for A/B measurements; read per call.
 static int pick_band(int M, int N, int K) {
   if (const char* e = getenv("SGPT_GEMM_BAND")) return atoi(e);
   const long long w_bytes = 2ll * N * K;
-  const int m_groups = (M + 2 * kGemmBM - 1) / (2 * kGemmBM);
-  return (w_bytes >= (64ll << 20) && m_groups >= 16) ? 8 : 0;
-}
-
-// The 16-warp early-release epilogue (gemm.cuh EpiTma16) for CTA pairs on 256-wide tiles: ON unless SGPT_GEMM_EPI16=0 (read
-// per call: the GPU tests compare both forms in one process).  Same box, alternating runs of bench.py: 38.70 k embeddings/s
-// with 8 epilogue warps, 39.73 / 39.76 k with 16 (GEMM time per step 5.50 -> 5.22 / 5.35 ms).
-static bool epi16_enabled() {
-  const char* e = getenv("SGPT_GEMM_EPI16");
-  return !(e != nullptr && e[0] == '0');
+  const int m_tiles = (M + kGemmBM - 1) / kGemmBM;
+  return (w_bytes >= (32ll << 20) && m_tiles >= 16) ? 8 : 0;
 }
 
 template <class Epi>
 static int launch_linear(const void* x, int64_t ldx, const void* w, int64_t ldw, int M, int N, int K,
-                         const typename Epi::Params& p, int bn, cudaStream_t stream, int ksplit = 1) {
-  const bool pair = M > kGemmBM;
+                         const typename Epi::Params& p, cudaStream_t stream, int ksplit = 1) {
   TileMap tm;
   tm.ksplit = ksplit;
   tm.band = pick_band(M, N, K);
-  using Epi16 = typename Epi16Of<Epi>::type;
-  if constexpr (!std::is_same<Epi16, Epi>::value) {
-    // (the opt-in 4-CTA-cluster experiment keeps its own 8-warp form)
-    if (bn == 256 && pair && epi16_enabled() && !cl4_enabled())
-      return launch_gemm<256, Epi16, 2>(x, ldx, w, ldw, M, N, K, p, stream, kCatGemm, tm);
-  }
-  if (bn == 256) {
-    if (M >= 4 * kGemmBM && cl4_enabled() && ksplit == 1)
-      return launch_gemm<256, Epi, 4>(x, ldx, w, ldw, M, N, K, p, stream);
-    return pair ? launch_gemm<256, Epi, 2>(x, ldx, w, ldw, M, N, K, p, stream, kCatGemm, tm)
-                : launch_gemm<256, Epi, 1>(x, ldx, w, ldw, M, N, K, p, stream, kCatGemm, tm);
-  }
-  return pair ? launch_gemm<128, Epi, 2>(x, ldx, w, ldw, M, N, K, p, stream, kCatGemm, tm)
-              : launch_gemm<128, Epi, 1>(x, ldx, w, ldw, M, N, K, p, stream, kCatGemm, tm);
+  return launch_gemm<128, Epi, 1>(x, ldx, w, ldw, M, N, K, p, stream, kCatGemm, tm);
 }
 
 // Split-K for the reduce-add (residual) epilogues: OFF unless SGPT_GEMM_SPLITK=2/3/4 asks for it (experiments, tests).
-// The idea: these GEMMs have few, long tiles (N = d_model) — 384 tile groups on 74 CTA pairs (125M c_proj) run as 6 rounds
-// of which the last is 19 % full — and S K-slices per tile give S x as many units of 1/S the length, so the tail shrinks
-// to a fraction of a slice.  Measured on B200 (tools/bench_splitk.py, isolated launches, us, unsplit / 2 / 3 / 4 slices):
-// 125M c_proj 117 / 115 / 121 / 117, 1.3B c_proj 328 / 339 / 379 / 403, 5.8B c_proj 874 / 907 / 953 / 1175 — the second
-// reduce-add per output element costs what the shorter tail saves.  And it is not free semantically: with S > 1 the order
-// in which the slices' partial sums reach the bf16 residual stream varies from run to run, so the encoder is no longer
-// bit-reproducible (tests/test_gpu_full_depth.py caught it).  A slice is at least 16 k-blocks (1024 of K).
-static int pick_ksplit(int M, int N, int K, int bn) {
+// S K-slices per tile give S x as many work units of 1/S the length, so the tail of the last wave shrinks, at the price
+// of a second reduce-add per output element.  It is not free semantically: with S > 1 the order in which the slices'
+// partial sums reach the bf16 residual stream varies from run to run, so the encoder is no longer bit-reproducible
+// (tests/test_gpu_full_depth.py).  A slice is at least 16 k-blocks (1024 of K).
+static int pick_ksplit(int K) {
   const char* env = getenv("SGPT_GEMM_SPLITK");  // read per call: the GPU tests flip it in-process
   const int forced = env != nullptr ? atoi(env) : -1;
   const int num_kb = (K + kGemmBK - 1) / kGemmBK;
   if (forced >= 2) return (forced <= 4 && num_kb / forced >= 16) ? forced : 1;
-  (void)M; (void)N; (void)bn;
   return 1;
 }
 
-// Tile-width heuristic: BN=256 halves the smem bytes the tensor core must read per FLOP, but with few tiles the
-// last wave is emptier; take the width with the better wave efficiency, preferring 256 on ties.
-static int pick_bn(int M, int N) {
-  if (N <= 128) return 128;
-  const int sms = sm_count();
-  auto eff = [&](int bn) {
-    const long long tiles = static_cast<long long>((M + kGemmBM - 1) / kGemmBM) * ((N + bn - 1) / bn);
-    const long long waves = (tiles + sms - 1) / sms;
-    const double useful = static_cast<double>(M) * N;
-    return useful / (static_cast<double>(waves) * sms * kGemmBM * bn);
-  };
-  return (eff(256) * 1.25 >= eff(128)) ? 256 : 128;
-}
-
 FilterGeometry filter_geometry(long long tiles, int nq) {
-  // queries above one M-tile are scanned by CTA pairs (M = 256): one group per (pair, column half)
+  // queries above one M-tile are scanned by two CTAs per work unit (256 rows): one group per (unit slot, column half)
   const long long units = nq > kGemmBM ? sm_count() / 2 : sm_count();
   const long long ctas = tiles < units ? (tiles > 0 ? tiles : 1) : units;
   const long long per_cta = (tiles + ctas - 1) / ctas;
@@ -185,9 +85,8 @@ FilterGeometry filter_geometry(long long tiles, int nq) {
   return g;
 }
 
-// nq <= 128: independent CTAs (M = 128).  128 < nq <= 256: CTA pairs running tcgen05.mma.cta_group::2 with M = 256 — each CTA
-// holds 128 of the queries and HALF of every corpus tile, so a scan moves half the corpus bytes per query through each SM
-// and the kernel turns from HBM-bound into tensor-bound (2 x the queries per pass over the shard).
+// nq <= 128: one CTA per work unit (M = 128).  128 < nq <= 256: two CTAs per work unit, each with 128 of the queries and
+// the same corpus tile — the second read of the tile is an L2 hit, so one pass over the shard from HBM serves 256 queries.
 template <class P>
 static int launch_filter_gemm(const void* Q, const void* C, int nq, int n, int D, const P& p, cudaStream_t stream, TileMap tm) {
   if (nq > kGemmBM) return launch_gemm<kSimBN, EpiFilterRows, 2>(Q, D, C, D, nq, n, D, p, stream, kCatScores, tm);
@@ -247,11 +146,6 @@ extern "C" int sgpt_linear(const void* x, int64_t ldx, const void* w, int64_t ld
   SGPT_REQUIRE(K % 8 == 0 && ldx % 8 == 0 && ldw % 8 == 0, "sgpt_linear: K, ldx, ldw must be multiples of 8");
   SGPT_REQUIRE(ldx >= K && ldw >= K && ldo >= N, "sgpt_linear: row pitch smaller than the row");
   if (M == 0) return SGPT_OK;
-  int bn = pick_bn(M, N);
-  if (const char* e = getenv("SGPT_GEMM_BN")) {  // experiments: force the tile width (128 / 256)
-    const int v = atoi(e);
-    if (v == 128 || (v == 256 && N > 128)) bn = v;
-  }
   switch (epilogue) {
     case SGPT_EPI_BF16:
     case SGPT_EPI_GELU_BF16: {
@@ -263,10 +157,10 @@ extern "C" int sgpt_linear(const void* x, int64_t ldx, const void* w, int64_t ld
       if (rc != SGPT_OK) return rc;
       if (epilogue == SGPT_EPI_BF16) {
         EpiBiasActBF16<false>::Params p{om, bias, out, static_cast<int>(ldo)};
-        return launch_linear<EpiBiasActBF16<false>>(x, ldx, w, ldw, M, N, K, p, bn, stream);
+        return launch_linear<EpiBiasActBF16<false>>(x, ldx, w, ldw, M, N, K, p, stream);
       }
       EpiBiasActBF16<true>::Params p{om, bias, out, static_cast<int>(ldo)};
-      return launch_linear<EpiBiasActBF16<true>>(x, ldx, w, ldw, M, N, K, p, bn, stream);
+      return launch_linear<EpiBiasActBF16<true>>(x, ldx, w, ldw, M, N, K, p, stream);
     }
     case SGPT_EPI_RESID_F32: {
       SGPT_REQUIRE(resid != nullptr, "sgpt_linear: SGPT_EPI_RESID_F32 needs resid");
@@ -282,7 +176,7 @@ extern "C" int sgpt_linear(const void* x, int64_t ldx, const void* w, int64_t ld
                                static_cast<uint64_t>(ldo), 32, 32);
       if (rc != SGPT_OK) return rc;
       EpiResidualF32::Params p{om, bias, out, static_cast<int>(ldo)};
-      return launch_linear<EpiResidualF32>(x, ldx, w, ldw, M, N, K, p, bn, stream, pick_ksplit(M, N, K, bn));
+      return launch_linear<EpiResidualF32>(x, ldx, w, ldw, M, N, K, p, stream, pick_ksplit(K));
     }
     case SGPT_EPI_RESID_BF16: {
       SGPT_REQUIRE(resid != nullptr && static_cast<const void*>(resid) == out,
@@ -293,7 +187,7 @@ extern "C" int sgpt_linear(const void* x, int64_t ldx, const void* w, int64_t ld
                                 static_cast<uint64_t>(ldo), 32, 64);
       if (rc != SGPT_OK) return rc;
       EpiResidualBF16::Params p{om, bias, out, static_cast<int>(ldo)};
-      return launch_linear<EpiResidualBF16>(x, ldx, w, ldw, M, N, K, p, bn, stream, pick_ksplit(M, N, K, bn));
+      return launch_linear<EpiResidualBF16>(x, ldx, w, ldw, M, N, K, p, stream, pick_ksplit(K));
     }
     case 102:
     case 103:
@@ -304,18 +198,18 @@ extern "C" int sgpt_linear(const void* x, int64_t ldx, const void* w, int64_t ld
                                 static_cast<uint64_t>(ldo), 32, 64);
       if (rc != SGPT_OK) return rc;
       OpTmaBiasActBF16<false>::Params p{om, bias, out, static_cast<int>(ldo)};
-      if (epilogue == 102) return launch_linear<EpiTma<OpTmaBiasActBF16<false>, 1>>(x, ldx, w, ldw, M, N, K, p, bn, stream);
-      if (epilogue == 105) return launch_linear<EpiTma<OpTmaBiasActBF16<false>, 4>>(x, ldx, w, ldw, M, N, K, p, bn, stream);
-      if (epilogue == 104) return launch_linear<EpiTma<OpTmaBiasActBF16<false>, 3>>(x, ldx, w, ldw, M, N, K, p, bn, stream);
-      return launch_linear<EpiTma<OpTmaBiasActBF16<false>, 2>>(x, ldx, w, ldw, M, N, K, p, bn, stream);
+      if (epilogue == 102) return launch_linear<EpiTma<OpTmaBiasActBF16<false>, 1>>(x, ldx, w, ldw, M, N, K, p, stream);
+      if (epilogue == 105) return launch_linear<EpiTma<OpTmaBiasActBF16<false>, 4>>(x, ldx, w, ldw, M, N, K, p, stream);
+      if (epilogue == 104) return launch_linear<EpiTma<OpTmaBiasActBF16<false>, 3>>(x, ldx, w, ldw, M, N, K, p, stream);
+      return launch_linear<EpiTma<OpTmaBiasActBF16<false>, 2>>(x, ldx, w, ldw, M, N, K, p, stream);
     }
     case 100: {  // profiling aid: mainloop only
       EpiDebugNull<false>::Params p{0};
-      return launch_linear<EpiDebugNull<false>>(x, ldx, w, ldw, M, N, K, p, bn, stream);
+      return launch_linear<EpiDebugNull<false>>(x, ldx, w, ldw, M, N, K, p, stream);
     }
-    case 101: {  // profiling aid: mainloop + TMEM loads
+    case 101: {  // profiling aid: mainloop + accumulator loads
       EpiDebugNull<true>::Params p{0};
-      return launch_linear<EpiDebugNull<true>>(x, ldx, w, ldw, M, N, K, p, bn, stream);
+      return launch_linear<EpiDebugNull<true>>(x, ldx, w, ldw, M, N, K, p, stream);
     }
     default:
       set_error("sgpt_linear: unknown epilogue %d", epilogue);
@@ -342,7 +236,7 @@ extern "C" int sgpt_linear_qkv_rotary(const void* x, int64_t ldx, const void* w_
   if (rc != SGPT_OK) return rc;
   EpiRotaryBF16::Params p{om, pos, reinterpret_cast<const float2*>(cos_sin), M, d_model, head_dim, rotary_dim, max_pos,
                           qkv, N};
-  return launch_linear<EpiRotaryBF16>(x, ldx, w_qkv, d_model, M, N, d_model, p, pick_bn(M, N), stream);
+  return launch_linear<EpiRotaryBF16>(x, ldx, w_qkv, d_model, M, N, d_model, p, stream);
 }
 
 // F2+F3 / F2+F6 with the LayerNorm folded into the GEMM (gemm.cuh OpTmaLnBiasActBF16): x_bf16 is the bf16 copy of the
@@ -362,16 +256,15 @@ extern "C" int sgpt_linear_lnfold(const void* x_bf16, int64_t ldx, const void* w
   CUtensorMap om;
   int rc = make_tma_2d_bf16(&om, out, static_cast<uint64_t>(M), static_cast<uint64_t>(N), static_cast<uint64_t>(ldo), 32, 64);
   if (rc != SGPT_OK) return rc;
-  const int bn = pick_bn(M, N);
   const float inv_d = 1.0f / static_cast<float>(K);
   if (gelu) {
     EpiLnBiasActBF16<true>::Params p{om, bias_folded, colsum, reinterpret_cast<const float2*>(row_stats), n_groups, inv_d, eps,
                                      out, static_cast<int>(ldo)};
-    return launch_linear<EpiLnBiasActBF16<true>>(x_bf16, ldx, w_folded, ldw, M, N, K, p, bn, stream);
+    return launch_linear<EpiLnBiasActBF16<true>>(x_bf16, ldx, w_folded, ldw, M, N, K, p, stream);
   }
   EpiLnBiasActBF16<false>::Params p{om, bias_folded, colsum, reinterpret_cast<const float2*>(row_stats), n_groups, inv_d, eps,
                                     out, static_cast<int>(ldo)};
-  return launch_linear<EpiLnBiasActBF16<false>>(x_bf16, ldx, w_folded, ldw, M, N, K, p, bn, stream);
+  return launch_linear<EpiLnBiasActBF16<false>>(x_bf16, ldx, w_folded, ldw, M, N, K, p, stream);
 }
 
 extern "C" int sgpt_linear_qkv_rotary_lnfold(const void* x_bf16, int64_t ldx, const void* w_folded,
@@ -397,7 +290,7 @@ extern "C" int sgpt_linear_qkv_rotary_lnfold(const void* x_bf16, int64_t ldx, co
   EpiLnRotaryBF16::Params p{{om, pos, reinterpret_cast<const float2*>(cos_sin), M, d_model, head_dim, rotary_dim, max_pos, qkv, N},
                             bias_folded, colsum, reinterpret_cast<const float2*>(row_stats), n_groups,
                             1.0f / static_cast<float>(d_model), eps, qkv, N};
-  return launch_linear<EpiLnRotaryBF16>(x_bf16, ldx, w_folded, d_model, M, N, d_model, p, pick_bn(M, N), stream);
+  return launch_linear<EpiLnRotaryBF16>(x_bf16, ldx, w_folded, d_model, M, N, d_model, p, stream);
 }
 
 // F5 / F6b with the statistics of the NEXT LayerNorm (gemm.cuh EpiResidLn): resid += x w^T + bias in place, plus the
@@ -423,10 +316,8 @@ extern "C" int sgpt_linear_resid_ln(const void* x, int64_t ldx, const void* w, i
     static const int l2pf = [] { const char* e = getenv("SGPT_RESID_L2_PREFETCH"); return (e != nullptr && e[0] == '0') ? 0 : 1; }();
     p.l2_prefetch = l2pf;
   }
-  // always 256-wide tiles: each epilogue warp then owns exactly one 128-column statistics group
-  if (M >= 4 * kGemmBM && cl4_enabled()) return launch_gemm<256, EpiResidLn, 4>(x, ldx, w, ldw, M, N, K, p, stream);
-  return M > kGemmBM ? launch_gemm<256, EpiResidLn, 2>(x, ldx, w, ldw, M, N, K, p, stream)
-                     : launch_gemm<256, EpiResidLn, 1>(x, ldx, w, ldw, M, N, K, p, stream);
+  // 128-wide tiles and four epilogue warps: each warp owns exactly one 128-column statistics group
+  return launch_gemm<128, EpiResidLn, 1>(x, ldx, w, ldw, M, N, K, p, stream);
 }
 
 extern "C" int sgpt_scores(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* scores,
@@ -439,5 +330,5 @@ extern "C" int sgpt_scores(const void* Q, const void* C, const float* q_scale, c
   if (nq == 0 || n == 0) return SGPT_OK;
   EpiScoresF32::Params p{scores, q_scale, c_scale, static_cast<long long>(lds)};
   // lanes = queries (A operand), columns = corpus rows (B operand, streamed once from HBM)
-  return launch_gemm<kSimBN, EpiScoresF32>(Q, D, C, D, nq, static_cast<int>(n), D, p, stream, kCatScores);
+  return launch_gemm<128, EpiScoresF32>(Q, D, C, D, nq, static_cast<int>(n), D, p, stream, kCatScores);
 }

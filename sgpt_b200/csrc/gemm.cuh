@@ -1,27 +1,27 @@
-// Persistent, warp-specialised tcgen05 GEMM for sm_100a:  C[M,N] = A[M,K] * B[N,K]^T  (bf16 in, fp32 accumulate).
+// Persistent, warp-specialised wgmma GEMM for sm_90a:  C[M,N] = A[M,K] * B[N,K]^T  (bf16 in, fp32 accumulate).
 //
-//   A : activations / queries, row-major [M,K]  -> K-major UMMA operand A (TMEM lane = row of A)
-//   B : nn.Linear weight [out,in] / corpus shard [n,D], row-major [N,K] -> K-major UMMA operand B
+//   A : activations / queries, row-major [M,K]  -> K-major wgmma operand A
+//   B : nn.Linear weight [out,in] / corpus shard [n,D], row-major [N,K] -> K-major wgmma operand B
 //
-// Roles (E epilogue warps + 4 control warps = 256 or 384 threads, 1 CTA per SM):
-//   warps 0..E-1  epilogue       (E = 8 for the TMA epilogues: two warps per TMEM lane quarter, each half the columns)
-//   warp  E       TMA producer   (one lane; kStages-deep smem ring of {A 128x64, B BNx64} bf16 tiles, SWIZZLE_128B)
-//   warp  E+1     MMA issuer     (one lane; tcgen05.mma M=128, N=BN, K=16; 2 TMEM accumulator stages)
-//   warp  E+2     TMEM allocator
+// Roles (9 warps = 288 threads, 1 CTA per SM):
+//   warps 0..7   two consumer warpgroups: warpgroup g runs wgmma m64nBNk16 for rows [64 g, 64 g + 64) of the 128 x BN
+//                tile with the fp32 accumulator in its registers, then the epilogue
+//   warp  8      TMA producer (one lane; kStages-deep smem ring of {A 128x64, B BNx64} bf16 tiles, SWIZZLE_128B)
 //
-// The accumulator is double-buffered in TMEM so tile i's epilogue overlaps tile i+1's MMAs; smem stages and TMEM
-// stages are handed over with mbarriers only (no __syncthreads in the main loop).
+// The producer runs ahead across tiles, so the next tile's operands stream in while the current tile's epilogue runs;
+// smem stages are handed over with mbarriers only.
 //
-// Epilogue data paths.  tcgen05.ld hands thread r of a warp row r of the tile (32 consecutive columns per load); a
-// direct global store from that layout would touch 32 different rows per instruction.  Two families:
+// Epilogue data paths.  The consumers park the accumulator in shared memory (fp32, 128 rows x BN, each 128-byte row
+// segment XOR-swizzled by (row & 7) so that both the fragment stores and the row reads are free of bank conflicts), and
+// the epilogue warps read it back with thread = row, 32 consecutive columns per read (acc_ld_32).  E = 4 or 8 epilogue
+// warps: warp w owns the 32-row slab (w % 4) and, with 8 warps, the column half (w / 4).  Two families:
 //   EpiTma<Op>    (nn.Linear outputs)  thread = row: bias/activation in registers, the 128-byte row segment is written
 //                 to a per-warp smem box in the SWIZZLE_128B layout and one elected lane hands the [32 x 128 B] box to
-//                 the TMA engine — a plain tensor store (bf16 outputs) or an fp32 reduce-add into the residual stream
-//                 (`resid += acc + bias`, performed by the L2; no residual load in the SM at all).  Two boxes per warp
-//                 are double-buffered with cp.async.bulk.wait_group.read; M/N tails are clipped by the tensor map.
-//   EpiStaged<Op> (similarity scores / threshold filter)  smem transpose so that lane = column pair and each warp
-//                 instruction touches one contiguous row segment; needed where the work is per-(query row) with
-//                 warp-wide ballots.
+//                 the TMA engine — a plain tensor store (bf16 outputs) or a reduce-add into the residual stream
+//                 (`resid += acc + bias`, performed by the L2; no residual load in the SM at all).  M/N tails are clipped
+//                 by the tensor map.
+//   EpiStaged<Op> (similarity scores)  smem transpose so that lane = column pair and each warp instruction touches one
+//                 contiguous row segment.
 #pragma once
 #include "common.cuh"
 
@@ -29,26 +29,24 @@ namespace sgpt {
 
 constexpr int kGemmBM = 128;
 constexpr int kGemmBK = 64;
-constexpr int kGemmThreads = 256;
-constexpr int kStageBytesPerWarp = 8192;  // per epilogue warp: 2 TMA boxes of 32 x 128 B, or one 32 x 64 fp32 slab
+constexpr int kGemmMmaWarps = 8;                        // two consumer warpgroups of 64 rows
+constexpr int kGemmThreads = 32 * (kGemmMmaWarps + 1);  // + the TMA producer warp
+constexpr int kStageBytesPerWarp = 4096;                // per epilogue warp (EpiTma): one TMA box of 32 x 128 B
 
-template <int BN, int CL = 1, int kStagingOverride = 0>
+template <int BN, int kStagingOverride = 0>
 struct GemmCfg {
   static constexpr int kABytes = kGemmBM * kGemmBK * 2;
-  static constexpr int kBBytes = (BN / (CL >= 2 ? 2 : 1)) * kGemmBK * 2;  // a CTA pair splits the B tile between its two CTAs
-  static constexpr int kStageBytes = kABytes + kBBytes;    // 48 / 32 KB (single CTA, BN 256 / 128); 32 / 24 KB (pair)
+  static constexpr int kBBytes = BN * kGemmBK * 2;
+  static constexpr int kStageBytes = kABytes + kBBytes;  // 32 KB (BN 128) / 48 KB (BN 256)
   static constexpr int kBarrierBytes = 512;
-  // epilogue staging: 4 KB boxes, one per epilogue warp behind the 48 KB stages, two (double-buffered) otherwise; an
-  // epilogue that needs more (EpiResidLn: residual load boxes) states its own total
-  static constexpr int kStagingBytes =
-      kStagingOverride > 0 ? kStagingOverride : ((kStageBytes == 49152) ? 4 * kStageBytesPerWarp : 8 * kStageBytesPerWarp);
-  static constexpr int kStagesFit = (232448 - 1024 - kStagingBytes - kBarrierBytes) / kStageBytes;
-  static constexpr int kStagesDefault = (kStageBytes == 49152) ? 4 : (kStageBytes == 32768) ? 5 : 6;
-  static constexpr int kStages = kStagesFit < kStagesDefault ? kStagesFit : kStagesDefault;
+  static constexpr int kAccBytes = kGemmBM * BN * 4;     // the fp32 accumulator handed to the epilogue
+  // epilogue staging: one 4 KB box per epilogue warp; an epilogue that needs another size states its own total
+  static constexpr int kStagingBytes = kStagingOverride > 0 ? kStagingOverride : kGemmMmaWarps * kStageBytesPerWarp;
+  static constexpr int kStagesFit = (232448 - 1024 - kAccBytes - kStagingBytes - kBarrierBytes) / kStageBytes;
+  static constexpr int kStages = kStagesFit < 4 ? kStagesFit : 4;
   static_assert(kStages >= 2, "not enough shared memory for a double-buffered mainloop");
-  static constexpr int kTmemCols = 2 * BN;  // 256 or 512 (power of two)
-  // smem: [<=1024 align slack][stages * (A|B)][epilogue staging][barriers + tmem holder (+ epilogue barriers)]
-  static constexpr int kSmemBytes = 1024 + kStages * kStageBytes + kStagingBytes + kBarrierBytes;
+  // smem: [<=1024 align slack][stages * (A|B)][accumulator][epilogue staging][barriers]
+  static constexpr int kSmemBytes = 1024 + kStages * kStageBytes + kAccBytes + kStagingBytes + kBarrierBytes;
   static_assert(kSmemBytes <= 232448, "exceeds the 227 KB per-CTA shared memory limit");
 };
 
@@ -62,13 +60,6 @@ template <class State, class = void>
 struct StateHasKs { static constexpr bool value = false; };
 template <class State>
 struct StateHasKs<State, decltype((void)State::ks)> { static constexpr bool value = true; };
-
-// Epilogues with a kEarlyRelease member split their tile work into load() — the warp's accumulator columns into registers
-// — and store(); the kernel hands the TMEM accumulator stage back to the MMA issuer between the two.
-template <class Epi, class = void>
-struct EpiEarlyRelease { static constexpr bool value = false; };
-template <class Epi>
-struct EpiEarlyRelease<Epi, decltype((void)Epi::kEarlyRelease)> { static constexpr bool value = true; };
 
 // Epilogues may state a total staging size (kStagingBytes member); 0 / absent = the default rule of GemmCfg.
 template <class Epi, class = void>
@@ -84,6 +75,35 @@ __device__ __forceinline__ uint64_t global_timer_ns() {
   return t;
 }
 
+// 32 consecutive accumulator columns of this thread's row from the swizzled smem accumulator; `addr` is the row's
+// address at a column that is a multiple of 32 (a 128-byte segment), chunk j of the segment sits at j ^ (row & 7)
+// (row & 7 == lane & 7: the epilogue warps own 32-row slabs).
+__device__ __forceinline__ void acc_ld_32(uint32_t addr, uint32_t (&v)[32]) {
+  const uint32_t sw = threadIdx.x & 7u;
+#pragma unroll
+  for (uint32_t j = 0; j < 8; ++j) {
+    const float4 x = lds_v4(addr + ((j ^ sw) << 4));
+    v[4 * j] = __float_as_uint(x.x);
+    v[4 * j + 1] = __float_as_uint(x.y);
+    v[4 * j + 2] = __float_as_uint(x.z);
+    v[4 * j + 3] = __float_as_uint(x.w);
+  }
+}
+
+// Pins the accumulator registers at this point of the instruction stream: the compiler sees each wgmma as a synchronous
+// read-modify-write of them, so without this it may copy or reorder accesses to registers an in-flight wgmma still writes.
+template <int N>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+template <int BN>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[BN / 2], uint64_t da, uint64_t db, int scale_d) {
+  if constexpr (BN == 128) wgmma_bf16_m64n128(d, da, db, scale_d);
+  else wgmma_bf16_m64n256(d, da, db, scale_d);
+}
+
 // Optional selection of N-tiles: the similarity search scans a strided sample of corpus tiles first (to establish
 // per-query thresholds) and the remaining tiles afterwards.
 //   mode 0: all tiles;  mode 1: tiles 0, s, 2s, ...;  mode 2: every tile that is NOT a multiple of s   (s >= 2)
@@ -95,10 +115,10 @@ struct TileMap {
   int ksplit = 1;
   // Rasterisation of the output tiles over the persistent CTAs.  band <= 1: N fastest (consecutive work units share the
   // activation rows and sweep the whole weight matrix: right while the weights stay in L2).  band = g: M-tile groups are
-  // taken in bands of g, and inside a band the M index runs fastest — the ~74 CTA pairs working at the same time then cover
-  // g M-groups x ~74/g N-tiles and fetch g + 74/g operand tiles instead of 1-2 + 64: for weight matrices larger than the
-  // L2 (GPT-J / BLOOM-7B c_fc: 134 MB streamed once per ~1.2 M-groups = 5 TB/s of HBM reads with N fastest) the operand
-  // traffic per wave drops ~4x.
+  // taken in bands of g, and inside a band the M index runs fastest — the 132 CTAs working at the same time then cover
+  // g M-tiles x ~132/g N-tiles and fetch g + 132/g operand tiles instead of 1-2 + 131: for weight matrices larger than the
+  // L2 (GPT-J / BLOOM-7B c_fc: 134 MB, streamed once per ~1 M-tile with N fastest) the operand traffic per wave drops
+  // several-fold.
   int band = 0;
   __host__ __device__ void coords(int tile, int m_tiles, int n_tiles, int& mg, int& nt) const {
     if (band <= 1) {
@@ -125,57 +145,37 @@ struct TileMap {
   }
 };
 
-// CL = 1: independent CTAs, tcgen05.mma.cta_group::1, one 128 x BN tile per CTA iteration.
-// CL = 2: CTA pairs (2-CTA clusters = the two SMs of a TPC) executing tcgen05.mma.cta_group::2 with M = 256: CTA r of
-//   the pair owns rows [128 r, 128 r + 128) of the 256 x BN tile (its A rows in its smem, its accumulator rows in its
-//   TMEM) and holds B rows [BN/2 r, BN/2 r + BN/2) — half of the weight tile — in its smem.  Only the leader (rank 0)
-//   issues MMAs; both CTAs run a TMA producer (signalling the LEADER's full barrier) and the epilogue of their rows.
-//   Per SM this removes a third of the smem writes (TMA) and operand reads (MMA) of the single-CTA kernel — measured:
-//   with cta_group::1 the mainloop alone ran at the tensor peak but every byte the epilogue moved through smem
-//   (st.shared + TMA-store reads) slowed it down (75 -> 103 us on the 32768 x 2304 x 768 QKV GEMM).
-//   Barrier protocol: full[s] (leader, 1 arrive + 2 x stage bytes) <- both producers' TMA; empty[s] (each CTA, count 1)
-//   <- leader's tcgen05.commit multicast; tmem_full[a] (each CTA) <- commit multicast; tmem_empty[a] (leader, count
-//   2 x epilogue warps) <- both CTAs' epilogue warps (remote arrive from the peer).
-// CL = 4: TWO CTA pairs (ranks {0,1} and {2,3}) on the same N-tile and adjacent 256-row M-groups.  At K = 768 the
-//   CL = 2 mainloop is bound by the L2 -> SM operand stream (64 B/clk/SM at the tensor peak against the ~43 B/clk/SM the
-//   L2 delivers: ncu l1tex__m_xbar2l1tex_read_bytes 12.9 TB/s), not by the tensor pipe.  Both pairs need the SAME weight
-//   tile, so every CTA fetches only a QUARTER of it (BN/4 rows) and multicasts it into its own smem and into the smem of
-//   the CTA of the same parity in the other pair: per k-block the four CTAs read 64 KB of A + 32 KB of B from L2 instead
-//   of 64 + 64 (-25 %).  Each pair still runs its own cta_group::2 MMA from its own leader; a smem stage is written by
-//   CTAs of BOTH pairs, so empty[s] counts one commit from each pair's leader (multicast to all four CTAs).
+// CL = 1: one 128 x BN tile per work unit.
+// CL = 2: two CTAs per work unit on the same N-tile and adjacent M-tiles (CTA r of the unit owns rows [128 r, 128 r + 128)
+//   of a 256 x BN tile group): the similarity search scans up to 256 queries per pass over the corpus this way, and both
+//   CTAs of a unit share the candidate-list group of the unit (EpiFilterRows).
 template <int BN, class Epi, int CL = 1>
-__global__ void __launch_bounds__(128 + 32 * Epi::kEpiWarps, 1)
+__global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, int M,
                     int N, int K, const __grid_constant__ typename Epi::Params ep, TileMap tmap) {
-  using Cfg = GemmCfg<BN, CL, EpiStaging<Epi>::value>;
+  using Cfg = GemmCfg<BN, EpiStaging<Epi>::value>;
   constexpr int kStages = Cfg::kStages;
-  static_assert(CL == 1 || CL == 2 || CL == 4, "cluster size");
-  constexpr bool kPair = CL >= 2;
+  static_assert(CL == 1 || CL == 2, "work unit size");
+  static_assert(Epi::kEpiWarps == 4 || Epi::kEpiWarps == 8, "4 or 8 epilogue warps");
+  static_assert(BN == 128 || BN == 256, "tile width");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_tiles = smem;
-  float* stage_base = reinterpret_cast<float*>(smem + kStages * Cfg::kStageBytes);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes + Cfg::kStagingBytes);
+  uint8_t* acc_smem = smem + kStages * Cfg::kStageBytes;
+  float* stage_base = reinterpret_cast<float*>(acc_smem + Cfg::kAccBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(acc_smem + Cfg::kAccBytes + Cfg::kStagingBytes);
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full_bar = empty_bar + kStages;
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-  uint64_t* epi_bars = tmem_empty_bar + 3;  // 2 mbarriers per epilogue warp (EpiResidLn's residual loads)
+  uint64_t* epi_bars = empty_bar + kStages;  // 2 mbarriers per epilogue warp (EpiResidLn's residual loads)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  // Warp roles.  The epilogue warps take the LOW warp ids and the TMA producer / MMA issuer the HIGH ones: the SM's
-  // issue arbiter favours higher warp ids among ready warps, and the two single-thread control warps must never be
-  // starved of issue slots by epilogue arithmetic sharing their scheduler (measured: with the control warps at ids
-  // 0/1 the epilogue's issue time added directly to the MMA time of every tile).
-  constexpr int kWarpProducer = Epi::kEpiWarps, kWarpMma = Epi::kEpiWarps + 1, kWarpTmem = Epi::kEpiWarps + 2;
+  constexpr int kWarpProducer = kGemmMmaWarps;
 
-  const uint32_t crank = kPair ? cluster_ctarank() : 0u;  // position inside the cluster = M-tile of the group
-  const uint32_t prank = crank & 1u;                       // rank inside the CTA pair; leader = crank & ~1
-  const int cid = blockIdx.x / CL, ncl = gridDim.x / CL;      // cluster index / number of clusters
-  const int m_tiles = ((M + kGemmBM - 1) / kGemmBM + CL - 1) / CL;  // M-tile groups (CL tiles each)
-  const int n_tiles = tmap.count((N + BN - 1) / BN);                // N-tiles this launch visits
+  const int crank = CL > 1 ? static_cast<int>(blockIdx.x % CL) : 0;  // M-tile of the unit's tile group
+  const int cid = blockIdx.x / CL, ncl = gridDim.x / CL;               // unit slot / number of unit slots
+  const int m_tiles = ((M + kGemmBM - 1) / kGemmBM + CL - 1) / CL;    // M-tile groups (CL tiles each)
+  const int n_tiles = tmap.count((N + BN - 1) / BN);                  // N-tiles this launch visits
   const int ksplit = tmap.ksplit;
   const int num_tiles = m_tiles * n_tiles * ksplit;  // work units
   const int num_kb = (K + kGemmBK - 1) / kGemmBK;
@@ -184,32 +184,13 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
   if (warp == kWarpProducer && lane == 0) {
     tma_prefetch_desc(&tma_a);
     tma_prefetch_desc(&tma_b);
-  }
-  if (warp == kWarpMma && lane == 0) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], CL == 4 ? 2 : 1);  // CL = 4: both pairs must have consumed the stage
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full_bar[i], 1);
-      mbar_init(&tmem_empty_bar[i], (kPair ? 2 : 1) * Epi::kEpiWarps);  // one arrive per epilogue warp (of both CTAs of a pair)
+      mbar_init(&empty_bar[i], kGemmMmaWarps);  // one arrive per consumer warp: each warp waits for its own wgmma part
     }
     fence_mbar_init();
   }
-  if (warp == kWarpTmem) {
-    if (kPair) {
-      tmem_alloc_pair(tmem_holder, Cfg::kTmemCols);
-      tmem_relinquish_pair();
-    } else {
-      tmem_alloc(tmem_holder, Cfg::kTmemCols);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
-  if (kPair) cluster_sync_all();  // peer barriers / TMEM must exist before any remote arrive, commit or pair MMA
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
+  __syncthreads();
   pdl_sync();  // everything above overlapped the previous kernel's tail; global memory is touched only below
   const bool clock_probe = (blockIdx.x == 0 && threadIdx.x == 0);
   const long long probe_c0 = clock_probe ? clock64() : 0;
@@ -224,155 +205,127 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
         const int tile = unit / ksplit, ks = unit - tile * ksplit;
         int mg, nt;
         tmap.coords(tile, m_tiles, n_tiles, mg, nt);
-        const int m0 = (mg * CL + static_cast<int>(crank)) * kGemmBM;
+        const int m0 = (mg * CL + crank) * kGemmBM;
         const int n0 = tmap.map(nt) * BN;
         const int kb_end = min(num_kb, (ks + 1) * kb_per);
         for (int kb = ks * kb_per; kb < kb_end; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem_tiles + stage * Cfg::kStageBytes;
           uint8_t* sb = sa + Cfg::kABytes;
-          if (kPair) {
-            // my A rows and my half of the B tile land in MY smem; the bytes are accounted on the pair leader's barrier
-            const uint32_t leader_full = mapa_shared(smem_u32(&full_bar[stage]), crank & ~1u);
-            if (prank == 0) mbar_expect_tx(&full_bar[stage], 2 * Cfg::kStageBytes);
-            tma_load_2d_pair(sa, &tma_a, leader_full, kb * kGemmBK, m0);
-            if (CL == 2) {
-              tma_load_2d_pair(sb, &tma_b, leader_full, kb * kGemmBK, n0 + static_cast<int>(prank) * (BN / 2));
-            } else {
-              // quarter (crank >> 1) of my pair-rank's half of the weight tile, multicast to the CTA of my parity in both
-              // pairs (same smem offset there); each destination accounts the bytes on ITS pair leader's full barrier
-              const int quarter = static_cast<int>(crank >> 1);
-              tma_load_2d_pair_multicast(sb + quarter * (BN / 4) * 128, &tma_b, leader_full,
-                                         kb * kGemmBK, n0 + static_cast<int>(prank) * (BN / 2) + quarter * (BN / 4),
-                                         static_cast<uint16_t>(0x5u << prank));
-            }
-          } else {
-            mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-            tma_load_2d(sa, &tma_a, &full_bar[stage], kb * kGemmBK, m0);
-            tma_load_2d(sb, &tma_b, &full_bar[stage], kb * kGemmBK, n0);
-          }
+          mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+          tma_load_2d(sa, &tma_a, &full_bar[stage], kb * kGemmBK, m0);
+          tma_load_2d(sb, &tma_b, &full_bar[stage], kb * kGemmBK, n0);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == kWarpMma) {
-    // ===================== MMA issuer =====================
-    if (lane == 0 && prank == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(kGemmBM * (kPair ? 2 : 1), BN, false);
-      // commit masks: my pair's two CTAs; the smem stages of a 4-CTA cluster are shared by both pairs
-      const uint16_t pair_mask = static_cast<uint16_t>(0x3u << (crank & ~1u));
-      const uint16_t stage_mask = (CL == 4) ? static_cast<uint16_t>(0xF) : pair_mask;
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int unit = cid; unit < num_tiles; unit += ncl) {
-        mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * BN;
-        const int ks = unit % ksplit;
-        const int kb_begin = ks * kb_per, kb_end = min(num_kb, kb_begin + kb_per);
-        for (int kb = kb_begin; kb < kb_end; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem_tiles + stage * Cfg::kStageBytes);
-          const uint32_t sb = sa + Cfg::kABytes;
-          const uint64_t da = make_smem_desc_sw128(sa, 16, 1024);
-          const uint64_t db = make_smem_desc_sw128(sb, 16, 1024);
-#pragma unroll
-          for (int k = 0; k < kGemmBK / 16; ++k) {
-            // advance 16 bf16 = 32 B along K inside the 128-B swizzle row: +2 in the (addr >> 4) field
-            if (kPair) umma_bf16_ss_pair(tmem_d, da + 2 * k, db + 2 * k, idesc, ((kb - kb_begin) | k) != 0);
-            else umma_bf16_ss(tmem_d, da + 2 * k, db + 2 * k, idesc, ((kb - kb_begin) | k) != 0);
-          }
-          // frees this smem stage (in both CTAs of a pair) once the MMAs above have read it
-          if (kPair) umma_commit_pair(&empty_bar[stage], stage_mask);
-          else umma_commit(&empty_bar[stage]);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-        // accumulator complete -> epilogue (of both CTAs)
-        if (kPair) umma_commit_pair(&tmem_full_bar[acc], pair_mask);
-        else umma_commit(&tmem_full_bar[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp < Epi::kEpiWarps) {
-    // ===================== epilogue =====================
-    // A warp may only touch TMEM lanes 32*(warp%4)..+31.  With 8 epilogue warps two warps share a lane quarter and
-    // split the tile's columns (half 0 / half 1): twice the warps to hide TMEM-load, bias-load and smem latencies.
-    const int ew = warp & 3;              // TMEM lane quarter (hardware: warp id % 4) == 32-row slab of the tile
-    const int half = warp >> 2;           // column half handled by this warp (always 0 with 4 epilogue warps)
+  } else {
+    // ===================== consumers: wgmma mainloop, then the epilogue =====================
+    const int wg = warp >> 2;              // consumer warpgroup = 64-row half of the tile
+    const int ew = warp & 3;               // 32-row slab of the tile this warp's epilogue owns
+    const int half = warp >> 2;            // column half handled by this warp's epilogue (always 0 with 4 epilogue warps)
+    const bool epi_warp = warp < Epi::kEpiWarps;
     constexpr int kColsPerWarp = BN / (Epi::kEpiWarps / 4);
     constexpr int kSlabBytes = Cfg::kStagingBytes / Epi::kEpiWarps;
-    float* stage_slab = stage_base + warp * (kSlabBytes / 4);
-    const uint32_t leader_tmem_empty0 = kPair ? mapa_shared(smem_u32(&tmem_empty_bar[0]), crank & ~1u) : 0u;
+    float* stage_slab = stage_base + (epi_warp ? warp : 0) * (kSlabBytes / 4);
+    const uint32_t acc_base = smem_u32(acc_smem);
     typename Epi::State st;
-    Epi::init(st, ep, ew * 32 + lane, epi_bars + 2 * warp);
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    if (epi_warp) Epi::init(st, ep, ew * 32 + lane, epi_bars + 2 * warp);
+    int stage = 0;
+    uint32_t phase = 0;
     for (int unit = cid; unit < num_tiles; unit += ncl) {
       const int tile = unit / ksplit;
-      if constexpr (StateHasKs<typename Epi::State>::value) st.ks = static_cast<uint32_t>(unit - tile * ksplit);
+      const int ks = unit - tile * ksplit;
+      if constexpr (StateHasKs<typename Epi::State>::value) st.ks = static_cast<uint32_t>(ks);
       int mg, ntile;
       tmap.coords(tile, m_tiles, n_tiles, mg, ntile);
-      const int m0 = (mg * CL + static_cast<int>(crank)) * kGemmBM + ew * 32;  // this warp's 32-row slab
+      const int m0 = (mg * CL + crank) * kGemmBM + ew * 32;  // this warp's 32-row slab
       const int n0 = tmap.map(ntile) * BN + half * kColsPerWarp;
-      // work that does not depend on the accumulator (EpiResidLn: the first residual loads, and an L2 prefetch of the
-      // residual boxes of the tile after this one) overlaps the mainloop
-      if constexpr (EpiHasPrefetch<Epi>::value) {
-        const int nt = (unit + ncl) / ksplit;  // (split-K is never combined with a prefetching epilogue)
-        if (unit + ncl < num_tiles) {
-          int mg2, nt2;
-          tmap.coords(nt, m_tiles, n_tiles, mg2, nt2);
-          Epi::prefetch_next(ep, (mg2 * CL + static_cast<int>(crank)) * kGemmBM + ew * 32,
-                             tmap.map(nt2) * BN + half * kColsPerWarp, lane, M, N);
+      if (epi_warp) {
+        // work that does not depend on the accumulator (EpiResidLn: the first residual loads, and an L2 prefetch of the
+        // residual boxes of the tile after this one; row constants) overlaps the mainloop
+        if constexpr (EpiHasPrefetch<Epi>::value) {
+          const int nt = (unit + ncl) / ksplit;  // (split-K is never combined with a prefetching epilogue)
+          if (unit + ncl < num_tiles) {
+            int mg2, nt2;
+            tmap.coords(nt, m_tiles, n_tiles, mg2, nt2);
+            Epi::prefetch_next(ep, (mg2 * CL + crank) * kGemmBM + ew * 32, tmap.map(nt2) * BN + half * kColsPerWarp, lane,
+                               M, N);
+          }
         }
+        Epi::template pre_tile<kColsPerWarp, kSlabBytes>(st, ep, m0, n0, lane, stage_slab, M, N);
       }
-      Epi::template pre_tile<kColsPerWarp, kSlabBytes>(st, ep, m0, n0, lane, stage_slab, M, N);
-      mbar_wait(&tmem_full_bar[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t trow = tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + acc * BN + half * kColsPerWarp;
-      if constexpr (EpiEarlyRelease<Epi>::value) {
-        // the accumulator stage goes back to the MMA issuer as soon as this warp's columns are in registers: the stage is
-        // held for one TMEM load, not for the arithmetic, the shared-memory stores, the proxy fence and the TMA hand-over
-        Epi::template load<kColsPerWarp, kSlabBytes>(st, trow);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if (kPair) mbar_arrive_cluster(leader_tmem_empty0 + acc * 8);
-          else mbar_arrive(&tmem_empty_bar[acc]);
-        }
-        Epi::template store<kColsPerWarp, kSlabBytes>(st, ep, m0, n0, lane, stage_slab, M, N);
-      } else {
-        Epi::template tile<kColsPerWarp, kSlabBytes>(st, ep, m0, n0, lane, trow, stage_slab, M, N);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if (kPair) mbar_arrive_cluster(leader_tmem_empty0 + acc * 8);
-          else mbar_arrive(&tmem_empty_bar[acc]);
-        }
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-    Epi::finish(st, ep, static_cast<int>(crank) * kGemmBM + ew * 32 + lane);  // row inside the CL x 128-row tile group
-    if (clock_probe) {
-      atomicAdd(&g_gemm_clock[0], static_cast<unsigned long long>(clock64() - probe_c0));
-      atomicAdd(&g_gemm_clock[1], static_cast<unsigned long long>(global_timer_ns() - probe_t0));
-    }
-  }
 
-  tc_fence_before();
-  if (kPair) cluster_sync_all();  // the peers may still multicast-arrive on this CTA's barriers until they are done too
-  else __syncthreads();
-  if (warp == kWarpTmem) {
-    tc_fence_after();
-    if (kPair) tmem_dealloc_pair(tmem_base, Cfg::kTmemCols);
-    else tmem_dealloc(tmem_base, Cfg::kTmemCols);
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      const int kb_begin = ks * kb_per, kb_end = min(num_kb, kb_begin + kb_per);
+      int prev_stage = -1;
+      for (int kb = kb_begin; kb < kb_end; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem_tiles + stage * Cfg::kStageBytes) + wg * (64 * 128);
+        const uint32_t sb = smem_u32(smem_tiles + stage * Cfg::kStageBytes) + Cfg::kABytes;
+        const uint64_t da = make_wgmma_desc_sw128(sa), db = make_wgmma_desc_sw128(sb);
+        wgmma_fence_acc(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kGemmBK / 16; ++k) wgmma_bf16<BN>(acc, da + 2 * k, db + 2 * k, (kb > kb_begin || k > 0) ? 1 : 0);
+        wgmma_commit();
+        wgmma_fence_acc(acc);
+        if constexpr (BN == 128) {
+          // one k-block stays in flight: the stage of the PREVIOUS k-block has been read once its group completed
+          wgmma_wait<1>();
+          if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+          prev_stage = stage;
+        } else {
+          // 128 accumulators per thread: keeping a group in flight across the next barrier wait spills them (the
+          // 288-thread CTA caps a thread at 168 registers), so this k-block completes before the next one is issued
+          wgmma_wait<0>();
+          if (lane == 0) mbar_arrive(&empty_bar[stage]);
+        }
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+      if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+
+      // accumulator -> smem (the previous tile's epilogue reads must be over), then the epilogue reads it back by rows
+      named_bar_sync(1, 32 * kGemmMmaWarps);
+      {
+        const int t = threadIdx.x & 127;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2) + 8 * h;
+          const uint32_t rbase = acc_base + static_cast<uint32_t>(row) * (BN * 4);
+          const uint32_t sw = static_cast<uint32_t>(row & 7);
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const uint32_t col = 8 * j + 2 * (t & 3);
+            const uint32_t chunk = col >> 2;
+            const uint32_t phys = (chunk & ~7u) | ((chunk & 7u) ^ sw);
+            sts_v2(rbase + phys * 16 + (col & 3u) * 4, __float_as_uint(acc[4 * j + 2 * h]),
+                   __float_as_uint(acc[4 * j + 2 * h + 1]));
+          }
+        }
+      }
+      named_bar_sync(1, 32 * kGemmMmaWarps);
+      if (epi_warp) {
+        const uint32_t trow = acc_base + static_cast<uint32_t>(ew * 32 + lane) * (BN * 4) + half * kColsPerWarp * 4;
+        Epi::template tile<kColsPerWarp, kSlabBytes>(st, ep, m0, n0, lane, trow, stage_slab, M, N);
+      }
+    }
+    if (epi_warp) {
+      Epi::finish(st, ep, crank * kGemmBM + ew * 32 + lane);  // row inside the CL x 128-row tile group
+      if (clock_probe) {
+        atomicAdd(&g_gemm_clock[0], static_cast<unsigned long long>(clock64() - probe_c0));
+        atomicAdd(&g_gemm_clock[1], static_cast<unsigned long long>(global_timer_ns() - probe_t0));
+      }
+    }
   }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// TMA epilogue driver: TMEM -> registers (thread = row) -> Op (bias / activation) -> swizzled smem box -> TMA
+// TMA epilogue driver: accumulator -> registers (thread = row) -> Op (bias / activation) -> swizzled smem box -> TMA
 // ---------------------------------------------------------------------------------------------------------------
 template <class Row>
 struct EpiTmaState {
@@ -393,7 +346,7 @@ template <class Op, int kDebug = 0>  // kDebug: 1 = skip the TMA store (timing e
 struct EpiTma {
   using Params = typename Op::Params;
   using State = EpiTmaState<typename Op::Row>;
-  static constexpr int kEpiWarps = 8;                 // 2 warps per TMEM lane quarter; each owns ONE 4 KB smem box
+  static constexpr int kEpiWarps = 8;                 // 2 warps per 32-row slab; each owns ONE 4 KB smem box
   static constexpr int kCols = 128 / Op::kElemBytes;  // columns per 128-byte row segment: 64 (bf16) or 32 (fp32)
   static __device__ __forceinline__ void init(State& st, const Params&, int, uint64_t*) { st.it = 0; st.ks = 0; }
   template <int BN, int kSlabBytes>
@@ -424,9 +377,8 @@ struct EpiTma {
         __syncwarp();
       }
       uint32_t v[kCols];
-      tmem_ld_32x32(trow + c, *reinterpret_cast<uint32_t(*)[32]>(&v[0]));
-      if (kCols == 64) tmem_ld_32x32(trow + c + 32, *reinterpret_cast<uint32_t(*)[32]>(&v[kCols - 32]));
-      tmem_ld_wait();
+      acc_ld_32(trow + 4 * c, *reinterpret_cast<uint32_t(*)[32]>(&v[0]));
+      if (kCols == 64) acc_ld_32(trow + 4 * (c + 32), *reinterpret_cast<uint32_t(*)[32]>(&v[kCols - 32]));
       // 8 chunks of 16 bytes; chunk j of row r lives at position j ^ (r & 7) of the row (SWIZZLE_128B)
       // All 8 chunks are computed before any of them is stored: the bias / rotary-table loads inside Op::chunk are then
       // independent ordinary loads the compiler batches up front (one exposed latency per box instead of one per chunk;
@@ -462,93 +414,6 @@ struct EpiTma {
     }
   }
 };
-
-// ---------------------------------------------------------------------------------------------------------------
-// Default for CTA pairs on 256-wide tiles since the end of round 2 (SGPT_GEMM_EPI16=0 restores 8 warps): 16 epilogue warps — four per TMEM lane quarter, 64 accumulator
-// columns (= one 128-byte bf16 box) each — that release the accumulator stage EARLY (kernel: load -> arrive -> store).
-// Why: with 8 warps a warp walks through four boxes per tile in series (smem box free -> tcgen05.ld -> arithmetic -> 8 x
-// st.shared -> fence.proxy.async -> TMA) and keeps the TMEM stage until the last one; at K = 768 that chain is about as
-// long as the 6144-clock mainloop of the next tile, so the MMA issuer waits for a free accumulator (ncu: tensor pipe 41-55 %
-// active, issue slots 15-35 % busy).  Here the stage is held for ONE TMEM load.  640 threads -> at most 96 registers per
-// thread: the 64 accumulator values stay in registers and the box is computed and stored in two halves of four chunks.
-// ---------------------------------------------------------------------------------------------------------------
-template <class Op>
-struct EpiTma16 {
-  using Params = typename Op::Params;
-  struct State {
-    uint32_t it;
-    uint32_t ks;
-    typename Op::Row row;
-    uint32_t v[64];  // this warp's accumulator columns of the current tile (thread = row)
-  };
-  static constexpr int kEpiWarps = 16;
-  static constexpr bool kEarlyRelease = true;
-  static constexpr int kCols = 128 / Op::kElemBytes;  // columns per 128-byte row segment: 64 (bf16) or 32 (fp32)
-  static __device__ __forceinline__ void init(State& st, const Params&, int, uint64_t*) { st.it = 0; st.ks = 0; }
-  template <int BN, int kSlabBytes>
-  static __device__ __forceinline__ void pre_tile(State& st, const Params& p, int m0, int, int lane, float*, int M, int) {
-    if (m0 < M) st.row = Op::row_init(p, m0 + lane, M);
-  }
-  static __device__ __forceinline__ void finish(State&, const Params&, int lane_row) {
-    if ((lane_row & 31) == 0) bulk_wait_group<0>();
-  }
-  template <int BN, int kSlabBytes>
-  static __device__ __forceinline__ void load(State& st, uint32_t trow) {
-    static_assert(BN == 64, "EpiTma16: 64 accumulator columns per warp (256-wide tiles)");
-    tmem_ld_32x32(trow, *reinterpret_cast<uint32_t(*)[32]>(&st.v[0]));
-    tmem_ld_32x32(trow + 32, *reinterpret_cast<uint32_t(*)[32]>(&st.v[32]));
-    tmem_ld_wait();
-  }
-  template <int BN, int kSlabBytes>
-  static __device__ __forceinline__ void store(State& st, const Params& p, int m0, int n0, int lane, float* slab, int M,
-                                               int N) {
-    static_assert(kSlabBytes == 4096, "EpiTma16: one 4 KB box per warp");
-    if (m0 >= M) return;  // whole 32-row slab out of range (warp-uniform)
-    const uint32_t box = smem_u32(slab);
-    const uint32_t row_addr = box + lane * 128u;
-    const typename Op::Row rc = st.row;
-#pragma unroll
-    for (int c = 0; c < BN; c += kCols) {  // one box (bf16 outputs) or two (fp32)
-      const int n = n0 + c;
-      if (n >= N) break;  // warp-uniform
-      if (st.it >= 1) {   // the TMA store of this warp's previous box must have finished READING the box
-        if (lane == 0) bulk_wait_group_read<0>();
-        __syncwarp();
-      }
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        uint32_t o[4][4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int jj = 4 * h + j;
-          if constexpr (OpSplitK<Op>::value)
-            Op::chunk(p, rc, &st.v[c + jj * (kCols / 8)], n + jj * (kCols / 8), N, m0 + lane, o[j], st.ks == 0);
-          else
-            Op::chunk(p, rc, &st.v[c + jj * (kCols / 8)], n + jj * (kCols / 8), N, m0 + lane, o[j]);
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int jj = 4 * h + j;
-          sts_v4(row_addr + ((jj ^ (lane & 7)) << 4), o[j][0], o[j][1], o[j][2], o[j][3]);
-        }
-      }
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) {
-        Op::issue(p, reinterpret_cast<const void*>(__cvta_shared_to_generic(box)), n, m0);
-        bulk_commit_group();
-      }
-      ++st.it;
-    }
-  }
-};
-
-// The 16-warp form of an epilogue, for the three ops it has been validated and measured with (bit-identical outputs,
-// tests/test_gpu_raster.py; whole-model parity; +2.7 % embeddings/s on SGPT-125M, profiles/r02_gemm_epilogue_16_warps_ab.jsonl):
-// bias (+ gelu_new) -> bf16 and the bf16 residual reduce-add.  Every other epilogue (GPT-J rotary, fp32 residual, the
-// LayerNorm-fold family, the search filter) maps to itself.  (The ops are declared below.)
-template <class Epi>
-struct Epi16Of { using type = Epi; };
 
 // bias index helper: columns beyond N are clipped by the tensor map, their bias is read from the last valid entry
 __device__ __forceinline__ float bias_at(const float* bias, int col, int N) {
@@ -794,9 +659,9 @@ struct OpTmaLnRotaryBF16 {
 //     xb_bf16[m, n] = bf16(new residual)                       (A operand of the next QKV / c_fc GEMM)
 //     stats[m, n / 128] = (sum, sum of squares) of the new residual over this warp's 128 columns
 // The old residual is fetched by TMA into a per-warp smem box (two boxes in flight: the first two loads of a tile are
-// issued BEFORE the accumulator is waited for, the rest chase the stores), updated in place by the row-owning threads
-// and written back with a TMA store; the bf16 copy leaves through a second box.  8 epilogue warps; BN = 256 only (each
-// warp then owns exactly one 128-column statistics group).  N % 64 == 0.
+// issued before the tile's mainloop, the rest chase the stores), updated in place by the row-owning threads and written
+// back with a TMA store; the bf16 copy leaves through a second box.  4 epilogue warps on 128-wide tiles (each warp then
+// owns exactly one 128-column statistics group).  N % 64 == 0.
 struct EpiResidLn {
   struct Params {
     CUtensorMap resid_map;  // fp32 [M, N], box 32 rows x 32 cols, SWIZZLE_128B (load and store)
@@ -810,8 +675,8 @@ struct EpiResidLn {
     uint32_t it;     // residual boxes processed so far by this warp (selects the load buffer and its barrier phase)
     uint64_t* bars;  // two mbarriers of this warp
   };
-  static constexpr int kEpiWarps = 8;
-  static constexpr int kStagingBytes = 8 * 12288;  // per warp: two fp32 load/store boxes + one bf16 store box
+  static constexpr int kEpiWarps = 4;
+  static constexpr int kStagingBytes = 4 * 12288;  // per warp: two fp32 load/store boxes + one bf16 store box
   static __device__ __forceinline__ void init(State& st, const Params&, int lane_row, uint64_t* bars) {
     st.it = 0;
     st.bars = bars;
@@ -873,9 +738,8 @@ struct EpiResidLn {
       const uint32_t fb = sbase + b * 4096u;
       const int n = n0 + 32 * c;
       uint32_t v[32];
-      tmem_ld_32x32(trow + 32 * c, v);
+      acc_ld_32(trow + 4 * 32 * c, v);
       mbar_wait(&st.bars[b], ph);  // old residual box has landed
-      tmem_ld_wait();
       const uint32_t row_addr = fb + lane * 128u;
       uint32_t h[16];
 #pragma unroll
@@ -916,7 +780,7 @@ struct EpiResidLn {
 };
 
 // ---------------------------------------------------------------------------------------------------------------
-// Staged epilogue driver: TMEM -> registers (thread = row) -> smem slab -> (lane = column pair) -> Op::rows()
+// Staged epilogue driver: accumulator -> registers (thread = row) -> smem slab -> (lane = column pair) -> Op::rows()
 // The slab is [32 rows][32 column pairs] of float2 without padding; pair p of row r is stored at p ^ (r & 15), which
 // makes both the row-wise writes and the column-wise reads bank-conflict free for 8-byte accesses.
 // ---------------------------------------------------------------------------------------------------------------
@@ -942,14 +806,13 @@ struct EpiStaged {
       const int n = n0 + c;
       if (n >= N) break;  // warp-uniform
       uint32_t v0[32], v1[32];
-      tmem_ld_32x32(trow + c, v0);
+      acc_ld_32(trow + 4 * c, v0);
       if (n + 32 < N) {
-        tmem_ld_32x32(trow + c + 32, v1);
+        acc_ld_32(trow + 4 * (c + 32), v1);
       } else {
 #pragma unroll
         for (int i = 0; i < 32; ++i) v1[i] = 0u;
       }
-      tmem_ld_wait();
       __syncwarp();  // the previous slab's readers are done
       const uint32_t wrow = slab + lane * 256u;
       const uint32_t sw = lane & 15;
@@ -1034,7 +897,7 @@ struct OpScoresF32 {
 // query with an atomicAdd per 32-document chunk: ~17 k same-address atomics per counter per search serialised in the
 // L2 and, not the HBM stream, set the kernel's duration.)  L is sized for the worst case (every score of every tile the
 // CTA visits admitted), so there is no overflow path; only the touched prefix of each list generates memory traffic.
-// 8 epilogue warps (two per TMEM lane quarter, half the tile's documents each); no shared memory.
+// 8 epilogue warps (two per 32-row slab, half the tile's documents each); no staging memory.
 //
 // Sample mode (Params::pool != nullptr; pass A of the search): nothing is filtered; the thread writes the MAXIMUM of
 // every 4 consecutive documents' scores (32 floats per query and tile half) to pool[q][group][Lp].  Each maximum is the
@@ -1058,7 +921,7 @@ struct EpiFilterRows {
     float* pool;             // sample mode: [M][groups][Lp] block maxima (cand / counts / tau unused)
     long long stride_p;      // floats between consecutive queries' blocks of `pool`
     int Lp;                  // floats per (query, group): 32 x tiles per CTA
-    int pair;                // 1: launched as CTA pairs (cta_group::2, M = 256 queries per scan)
+    int pair;                // 1: launched with two CTAs per work unit (CL = 2: 256 queries per scan)
   };
   struct State {
     int cnt;    // front entries (sample mode: maxima written)
@@ -1072,8 +935,9 @@ struct EpiFilterRows {
     float rs, tau, tau_hi;
   };
   static constexpr int kEpiWarps = 8;
-  // one group per (cluster, column half): with CTA pairs (Params::pair = 1: up to 256 queries per scan, rank r of the pair
-  // owns queries 128 r .. 128 r + 127 and all 256 documents of the tile) both CTAs of a pair write the SAME group's lists —
+  static constexpr int kStagingBytes = 1024;  // (none used)
+  // one group per (work-unit slot, column half): with two CTAs per unit (Params::pair = 1: up to 256 queries per scan, CTA r
+  // of the unit owns queries 128 r .. 128 r + 127 and all 256 documents of the tile) both CTAs write the SAME group's lists —
   // of different queries
   static __device__ __forceinline__ int group_of(const Params& p) {
     return p.group0 + static_cast<int>(blockIdx.x >> p.pair) * 2 + static_cast<int>(threadIdx.x >> 7);
@@ -1130,13 +994,12 @@ struct EpiFilterRows {
       const int n = n0 + c;
       if (n >= N) break;  // warp-uniform
       uint32_t v[32];
-      tmem_ld_32x32(trow + c, v);
+      acc_ld_32(trow + 4 * c, v);
       const bool full = (n + 32 <= N);
       // scale of column c + i: component i % 4 of lane (c + i) / 4 (all lanes take part: the loop is warp-uniform)
       float cs[32];
 #pragma unroll
       for (int i = 0; i < 32; ++i) cs[i] = __shfl_sync(0xffffffffu, csv[i & 3], (c >> 2) + (i >> 2));
-      tmem_ld_wait();
       // XS:99 maps a NaN score to -1.  While tau > -1 (always, except for degenerate corpora) a NaN fails `x >= tau` exactly
       // as its image -1 would, and in sample mode fmaxf drops it (a smaller maximum keeps tau a valid lower bound): the
       // explicit mapping (two instructions per score) is only executed when some row of the warp could admit a -1.
@@ -1198,11 +1061,6 @@ using EpiFilterCandidates = EpiFilterRows;
 
 
 template <bool kGelu>
-struct Epi16Of<EpiTma<OpTmaBiasActBF16<kGelu>, 0>> { using type = EpiTma16<OpTmaBiasActBF16<kGelu>>; };
-template <>
-struct Epi16Of<EpiTma<OpTmaResidAddBF16, 0>> { using type = EpiTma16<OpTmaResidAddBF16>; };
-
-template <bool kGelu>
 using EpiBiasActBF16 = EpiTma<OpTmaBiasActBF16<kGelu>>;
 using EpiResidualF32 = EpiTma<OpTmaResidAddF32>;
 using EpiResidualBF16 = EpiTma<OpTmaResidAddBF16>;
@@ -1211,7 +1069,7 @@ template <bool kGelu>
 using EpiLnBiasActBF16 = EpiTma<OpTmaLnBiasActBF16<kGelu>>;
 using EpiLnRotaryBF16 = EpiTma<OpTmaLnRotaryBF16>;
 
-// Bring-up / profiling aids (sgpt_linear epilogue codes 100, 101): no epilogue work at all, or TMEM loads only.
+// Bring-up / profiling aids (sgpt_linear epilogue codes 100, 101): no epilogue work at all, or accumulator loads only.
 template <bool kLoad>
 struct EpiDebugNull {
   struct Params { int dummy; };
@@ -1228,12 +1086,11 @@ struct EpiDebugNull {
 #pragma unroll 1
       for (int c = 0; c < BN; c += 32) {
         uint32_t v[32];
-        tmem_ld_32x32(trow + c, v);
-        tmem_ld_wait();
+        acc_ld_32(trow + 4 * c, v);
 #pragma unroll
         for (int i = 0; i < 32; ++i) acc ^= v[i];
       }
-      if (acc == 0x12345678u) printf("~");  // keep the loads alive
+      asm volatile("" ::"r"(acc));  // keep the loads alive (no call: it would serialise the wgmma pipeline)
     }
   }
 };

@@ -18,9 +18,8 @@
 //                   (sum x, sum x^2 per 128 columns); the GEMMs that consume LN(resid) (QKV, c_fc) run on xb with gamma folded
 //                   into their weight columns and apply  y = r (xb W'^T) - r mu c + b'  per row in the epilogue
 //                   (OpTmaLnBiasActBF16); ln_f is folded into the pooling kernel the same way.  Parity-tested like the
-//                   default, and measured SLOWER on every config (profiles/r02_gemm_epilogues_*.jsonl, DESIGN.md §7): the
-//                   step is power-capped, every instruction and every byte the GEMM epilogues move costs as much time as
-//                   the 30 us LayerNorm pass it replaces — the folded c_fc epilogue alone loses 36 us of 135.
+//                   default; opt-in (every instruction and byte the GEMM epilogues add can cost as much time as the
+//                   LayerNorm pass it replaces).
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>

@@ -1,6 +1,6 @@
 // S1+S2 for one corpus shard without materialising the [nq, n] score matrix.
 //
-// Two passes of the same tcgen05 similarity GEMM:
+// Two passes of the same wgmma similarity GEMM:
 //   pass A  scans a strided SAMPLE of the corpus tiles (every s-th 256-document tile, at most one tile per SM, so the pass
 //           is a single round) and keeps, per query, the maximum score of every 4 consecutive documents (gemm.cuh
 //           EpiFilterRows, sample mode).  tau[q] = the k-th largest of those maxima (tau_select_kernel: ten block-wide

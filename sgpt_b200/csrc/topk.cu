@@ -372,8 +372,7 @@ __global__ void __launch_bounds__(kTopkThreads, 1) topk_select_kernel(TopkSrc sr
   uint32_t sub_n = 0;
   bool use_sub = false;  // digits 2 and 3 run over the compacted survivors of digit 1 instead of all keys
   // ---- fast path (all keys cached in shared memory) ------------------------------------------------------------------
-  // Histogram passes cost ~3 shared-memory atomics / warp-matches per key (ncu r2_1: 7 k instructions per warp, 80 us per
-  // launch at 38 k keys).  Instead: (1) a 1024-key strided SAMPLE (one key per thread) gives, by a 32-round bitwise
+  // Histogram passes cost ~3 shared-memory atomics / warp-matches per key.  Instead: (1) a 1024-key strided SAMPLE (one key per thread) gives, by a 32-round bitwise
   // search with block-wide counts, a pivot `lo` that is below the k-th largest key with overwhelming probability but
   // keeps only a few k / n of the keys; (2) ONE pass compacts the keys >= lo (with their flat positions) into a short
   // list and counts them — the count proves the pivot valid, otherwise the histogram path below takes over; (3) the
@@ -799,10 +798,9 @@ int launch_front_select(const TopkSrc& src, int nq, int k, float* out_scores, in
       src.G > kMaxFlatLists || (src.stride_g & 1) != 0 || (src.stride_q & 1) != 0 || k <= 0 || k > kFrontCap ||
       need_generic == nullptr)
     return SGPT_OK;
-  // OFF by default: measured SLOWER than the generic kernel on B200 (profiles/r02_search_phases_call29_*.jsonl): sorting all
-  // 4096 slots is 78 compare-exchange stages over 4 slots per thread = 30 us, against 20 us for compaction + exact k-th key +
-  // placing + sorting only the 1024 winners; the denser load (3.3 vs 5.3 us) does not pay for it.  SGPT_FRONT_SELECT=1
-  // (read per call) keeps it testable.
+  // OFF by default: sorting all 4096 slots is 78 compare-exchange stages over 4 slots per thread, against compaction + exact
+  // k-th key + placing + sorting only the 1024 winners in the generic kernel.  SGPT_FRONT_SELECT=1 (read per call) keeps it
+  // testable.
   {
     const char* e = getenv("SGPT_FRONT_SELECT");
     if (!(e != nullptr && e[0] == '1')) return SGPT_OK;
@@ -966,8 +964,7 @@ static bool launch_merge_sorted(const TopkSrc& src, int nq, int k, float* out_sc
                                 int* rc) {
   constexpr size_t kDynMax = 200 * 1024;
   const size_t bytes = static_cast<size_t>(src.G) * static_cast<size_t>(src.L) * 8;
-  // Measured on B200 (profiles/r02_bench_line_final_{2,8}gpu.json): 2 lists 0.016 ms against 0.032 ms for selecting again,
-  // 8 lists 0.047 against 0.031 ms — every entry pays one binary search per OTHER list — so only few lists are rank-merged.
+  // Every entry pays one binary search per OTHER list, so the rank-merge beats selecting again only for a few lists.
   if (!src.lists_sorted || src.packed == nullptr || !src.packed_global || src.counts != nullptr || out_scores == nullptr ||
       out_ids == nullptr || bytes > kDynMax || src.G < 1 || src.G > 3)
     return false;

@@ -1,4 +1,4 @@
-"""Embedder plug-ins with the reference's call surface, running on the B200 encoder.
+"""Embedder plug-ins with the reference's call surface, running on the CUDA encoder.
 
 * ``CustomEmbedder``  — drop-in for biencoder/beir/beir_dense_retriever.py:106-348 (script / HF path): same constructor
   keywords, ``embed_batcher``, ``encode_queries(List[(qid, text)], ...)``, ``encode_corpus(List[(cid, {title,text})], ...)``.
@@ -250,7 +250,7 @@ class CustomEmbedder:
 
 class SentenceEncoder:
     """``SentenceTransformer.encode`` for a [Transformer -> Pooling | WeightedMeanPooling (-> Dense | Asym)* (-> Normalize)]
-    SGPT model on the B200 encoder (module pipeline of sentence_transformers/SentenceTransformer.py:98, run as one
+    SGPT model on the CUDA encoder (module pipeline of sentence_transformers/SentenceTransformer.py:98, run as one
     ``sgpt_encode`` call + ``sgpt_dense`` per head)."""
 
     def __init__(self, config: ModelConfig, state_dict: Dict[str, torch.Tensor], tokenizer, device: str = "cuda:0",

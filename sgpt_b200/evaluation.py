@@ -1,4 +1,4 @@
-"""``InformationRetrievalEvaluator`` on the B200 exact search (SURVEY.md §8f row 3).
+"""``InformationRetrievalEvaluator`` on the CUDA exact search (SURVEY.md §8f row 3).
 
 Same constructor, ``__call__`` / ``compute_metrices`` / ``compute_metrics`` contract and metric definitions as
 sentence_transformers/evaluation/InformationRetrievalEvaluator.py:15-299 (Accuracy@k, Precision/Recall@k, MRR@k, NDCG@k

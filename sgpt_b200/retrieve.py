@@ -1,4 +1,4 @@
-"""`python -m sgpt_b200.retrieve` — the retrieval run of biencoder/beir/beir_dense_retriever.py:352-498 on the B200 path.
+"""`python -m sgpt_b200.retrieve` — the retrieval run of biencoder/beir/beir_dense_retriever.py:352-498 on the CUDA path.
 
 Same flags (BDR:31-96), same flow (load BEIR split -> drop empty documents -> build the embedder + exact search ->
 retrieve top-1000 -> write ``results_<model>_<method>_<dataset>.json`` -> NDCG/MAP/Recall/P into

@@ -1,4 +1,4 @@
-"""Reads a saved sentence-transformers model directory of the reference's fork into what the B200 encoder needs.
+"""Reads a saved sentence-transformers model directory of the reference's fork into what the CUDA encoder needs.
 
 Mirrors ``SentenceTransformer._load_sbert_model`` (sentence_transformers/SentenceTransformer.py:903-936): ``modules.json``
 lists ``{idx, name, path, type}`` entries; each module directory is parsed the way that module's own ``load`` does —

@@ -495,7 +495,7 @@ int main(int argc, char** argv) {
     test_linear(32768, 3072, 768, SGPT_EPI_GELU_BF16, 4);
     test_linear(32768, 768, 3072, SGPT_EPI_RESID_F32, 4);
   }
-  if (!strcmp(only, "nullepi")) {  // timing only: mainloop without / with TMEM loads in the epilogue
+  if (!strcmp(only, "nullepi")) {  // timing only: mainloop without / with accumulator loads in the epilogue
     for (int epi = 100; epi <= 105; ++epi)
       for (int K : {768, 3072}) {
         const int M = 32768, N = 2304;

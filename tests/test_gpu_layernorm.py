@@ -16,8 +16,9 @@ def _lib():
 
 
 # widths: 768 (<32,3> persistent), 1024 (<32,4> one-row), 2048 / 1536 (<128,2> persistent), 2560 / 4096 (<256,2>
-# persistent), 5120 (<256,4> one-row), 64 (tiny); row counts straddle the grid-stride loop (148 SMs x MINB CTAs x rows)
-@pytest.mark.parametrize("T,d", [(1, 768), (7, 768), (2368, 768), (2369 + 8 * 296, 768), (33000, 768), (300, 1024),
+# persistent), 5120 (<256,4> one-row), 64 (tiny); row counts straddle the grid-stride loop (SMs x MINB CTAs x rows) of
+# the H100's 132 SMs (2112 / 2113) and of a 148-SM part
+@pytest.mark.parametrize("T,d", [(1, 768), (7, 768), (2112, 768), (2113, 768), (2368, 768), (2369 + 8 * 296, 768), (33000, 768), (300, 1024),
                                  (5, 2048), (1777, 2048), (9001, 1536), (3, 4096), (1333, 4096), (2000, 2560),
                                  (700, 5120), (19, 64)])
 @pytest.mark.parametrize("in_place", [False, True])

@@ -63,7 +63,7 @@ def _worker(rank, world, port, q):
 
 def test_two_rank_nccl_and_peer_gather_match_whole_corpus_oracle():
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp
 
     ctx = mp.get_context("spawn")

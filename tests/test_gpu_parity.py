@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: pytest -m gpu).  Everything goes through the C ABI (ctypes -> libsgpt_b200.so).
+"""GPU parity tests (run on an H100: pytest -m gpu).  Everything goes through the C ABI (ctypes -> libsgpt_b200.so).
 
 Bars (BASELINE.json north_star): pooled embeddings within 1e-3 cosine of the reference HF path on the same inputs and
 weights; identical top-k document ids vs the oracle evaluated on the same stored (bf16-rounded) vectors, ties at the
@@ -203,11 +203,11 @@ def _assert_same_topk(scores_dev, ids_dev, full, k, id_base=0):
 
 @pytest.mark.parametrize("nq,n,D,k,fn", [(128, 20000, 768, 1001, "cos_sim"), (16, 5003, 2048, 1001, "dot"),
                                          (1, 3000, 768, 1001, "cos_sim"), (7, 600, 64, 1001, "cos_sim"),
-                                         # >= 8 x 148 corpus tiles: the two-pass threshold-filter path; 130 queries =
+                                         # >= 8 x 132 corpus tiles: the two-pass threshold-filter path; 130 queries =
                                          # two query blocks; ragged last tile (n % 256 != 0)
                                          (130, 320001, 64, 1001, "cos_sim"), (5, 310000, 128, 10, "dot"),
-                                         # more than 128 queries: CTA pairs scan 256 queries per pass (M = 256); 300 =
-                                         # one pair block + a 44-query block on the single-CTA plan; 256 = a full pair
+                                         # more than 128 queries: two CTAs per tile scan 256 queries per pass; 300 =
+                                         # one 256-query block + a 44-query block on the single-CTA plan; 256 = a full one
                                          (300, 320001, 64, 100, "dot"), (256, 150001, 128, 1001, "cos_sim")])
 def test_search_identical_topk_ids(nq, n, D, k, fn):
     from sgpt_b200 import CorpusShard

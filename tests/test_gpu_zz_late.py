@@ -1,6 +1,6 @@
 """GPU tests added late in round 1 (GPT-J scorer, multi-row-tile scores GEMM, sharded DRES, IR evaluator).  They run last
 (pytest orders files alphabetically and the driver runs with -x) so that a failure here could not hide the parity tests
-above; all four are green on the B200 (profiles/r01_pytest_gpu_s2.log)."""
+above."""
 import os
 
 import numpy as np

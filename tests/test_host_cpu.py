@@ -38,7 +38,7 @@ def test_library_exports_every_declared_symbol():
 
 def test_search_workspace_plan_is_consistent_across_query_blocks():
     """Host logic of the fused search (csrc/search.cu make_plan / sgpt_search_workspace_bytes; no GPU needed — the SM count
-    falls back to 148): batches above 256 queries are processed in blocks that REUSE one workspace, whose last block may be
+    falls back to the H100's 132): batches above 256 queries are processed in blocks that REUSE one workspace, whose last block may be
     small enough for the single-CTA plan with its different list layout, so the size for nq queries must cover every block
     size that can occur; small shards take the dense path (nq x n fp32 scores)."""
     from sgpt_b200 import _lib
@@ -53,7 +53,7 @@ def test_search_workspace_plan_is_consistent_across_query_blocks():
     assert ws(128, n, k) >= ws(7, n, k) > 0
     # two-pass lists are worst-case sized: ~8 bytes per (query, document)
     assert 0.9 < ws(128, n, k) / (128 * n * 8) < 1.2
-    # below two corpus tiles per SM (75 776 documents at 148 SMs): dense scores, 4 bytes per (query, document)
+    # below two corpus tiles per SM (67 584 documents at 132 SMs): dense scores, 4 bytes per (query, document)
     assert ws(16, 50_000, k) == 16 * 50_000 * 4 + 256
     assert ws(16, 80_000, k) > 16 * 80_000 * 4 + 256
 

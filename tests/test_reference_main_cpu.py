@@ -1,21 +1,20 @@
-"""SURVEY.md §8f row 1 / VERDICT r01 item 9: the reference's own ``main`` (biencoder/beir/beir_dense_retriever.py:352-498)
-runs UNMODIFIED against the stand-in ``beir`` package and ``custommodels`` of sgpt_b200/compat.  This container has the
-reference but no GPU, so the two classes that launch CUDA kernels are replaced by CPU stand-ins that keep their
-interfaces (a toy embedder with CustomEmbedder's constructor keywords; the oracle's restatement of the search loop behind
-DenseRetrievalExactSearch's ``search``); everything else — argument parsing, GenericDataLoader, empty-text filtering,
-EvaluateRetrieval.retrieve/evaluate, the result and metric files — is the reference's code driving the stand-in
-package.  (On the GPU box the reference is absent; the same flow with the real classes is covered by
-tests/test_gpu_heads.py and `python -m sgpt_b200.compat.run_reference`.)"""
+"""SURVEY.md §8f row 1 / VERDICT r01 item 9: the flow of the reference's ``main`` (biencoder/beir/beir_dense_retriever.py:
+352-498) — GenericDataLoader, empty-text filtering, DenseRetrievalExactSearch behind EvaluateRetrieval(k_values=[1, 3, 5,
+10, 100, 1000]).retrieve/evaluate — on the stand-in ``beir`` package of sgpt_b200/compat must reproduce what the
+reference's own ``main`` wrote for the same toy BEIR set: its result file and its metrics, stored in
+tests/golden/reference_main_toyset.json by tests/golden/make_reference_main.py, which ran that ``main`` unmodified on the
+stand-in packages.  The classes that launch CUDA kernels are CPU stand-ins with the same interfaces (a toy embedder with
+CustomEmbedder's constructor keywords; the oracle's restatement of the search loop behind DenseRetrievalExactSearch's
+``search``).  The same flow with the real classes is covered by tests/test_gpu_heads.py and
+`python -m sgpt_b200.compat.run_reference`."""
 import json
 import os
-import sys
 import zlib
 
 import numpy as np
-import pytest
 import torch
 
-REF = "/root/reference/biencoder/beir/beir_dense_retriever.py"
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_main_toyset.json")
 
 
 class _ToyEmbedder:
@@ -65,54 +64,59 @@ class _CpuDRES:
         return self.results
 
 
-@pytest.mark.skipif(not os.path.exists(REF), reason="the reference tree is only present in the build container")
-def test_reference_main_runs_unmodified_on_the_stand_in_packages(tmp_path, monkeypatch):
-    from sgpt_b200 import compat
-    from sgpt_b200.compat.run_reference import load_reference_script
-
-    # toy BEIR directory: the relevant document of every query repeats the query's words
+def make_toy_beir(root):
+    """Toy BEIR directory <root>/datasets/toyset: the relevant document of every query repeats the query's words."""
     rs = np.random.RandomState(0)
     words = [f"w{i}" for i in range(200)]
-    root = tmp_path / "datasets" / "toyset"
-    os.makedirs(root / "qrels")
+    root = os.path.join(root, "datasets", "toyset")
+    os.makedirs(os.path.join(root, "qrels"))
     corpus = {f"d{i}": {"title": " ".join(rs.choice(words, 2)), "text": " ".join(rs.choice(words, rs.randint(3, 30)))}
               for i in range(60)}
-    corpus["d_empty"] = {"title": "t", "text": ""}  # removed by the script (BDR:382-388)
+    corpus["d_empty"] = {"title": "t", "text": ""}  # removed by main (BDR:382-388)
     queries = {f"q{i}": corpus[f"d{i}"]["text"] for i in range(8)}
-    with open(root / "corpus.jsonl", "w") as f:
+    with open(os.path.join(root, "corpus.jsonl"), "w") as f:
         for k, v in corpus.items():
             f.write(json.dumps({"_id": k, **v}) + "\n")
-    with open(root / "queries.jsonl", "w") as f:
+    with open(os.path.join(root, "queries.jsonl"), "w") as f:
         for k, v in queries.items():
             f.write(json.dumps({"_id": k, "text": v}) + "\n")
-    with open(root / "qrels" / "test.tsv", "w") as f:
+    with open(os.path.join(root, "qrels", "test.tsv"), "w") as f:
         f.write("query-id\tcorpus-id\tscore\n")
         for i in range(8):
             f.write(f"q{i}\td{i}\t1\n")
+    return root, queries
 
-    monkeypatch.chdir(tmp_path)  # the script writes its result files into the working directory
-    monkeypatch.setattr(sys, "path", list(sys.path))
-    mod = load_reference_script(REF, embedder_cls=_ToyEmbedder, module_name="ref_bdr_under_test")
+
+def test_stand_in_packages_reproduce_the_reference_main_on_a_toy_set(tmp_path, monkeypatch):
+    from sgpt_b200 import compat
+
+    monkeypatch.syspath_prepend(compat.COMPAT_DIR)
     import beir
-    import custommodels
+    from beir.datasets.data_loader import GenericDataLoader
+    from beir.retrieval.evaluation import EvaluateRetrieval
 
     assert os.path.dirname(os.path.dirname(beir.__file__)) == compat.COMPAT_DIR  # the stand-in, not an installed beir
-    monkeypatch.setattr(mod, "DenseRetrievalExactSearch", _CpuDRES)  # (bound at import: `from custommodels import ...`)
-    assert custommodels.DenseRetrievalExactSearch.__module__ == "sgpt_b200.exact_search"
-    monkeypatch.setattr(sys, "argv", ["beir_dense_retriever.py", "--dataset", "toyset", "--datapath", str(tmp_path / "datasets"),
-                                      "--modelname", "toy/model", "--method", "weightedmean", "--device", "cpu",
-                                      "--batchsize", "16", "--specb"])
-    args = mod.parse_args()
-    mod.main(args)
 
-    results = json.load(open(tmp_path / "results_toy_model_weightedmean_toyset.json"))
-    assert set(results) == set(queries)
+    data_path, queries = make_toy_beir(str(tmp_path))
+    corpus, qs, qrels = GenericDataLoader(data_path).load(split="test")
+    for k in [k for k, v in corpus.items() if not v["text"]]:
+        del corpus[k]
+    model = _CpuDRES(_ToyEmbedder(model_name="toy/model", method="weightedmean", device="cpu", batch_size=16, specb=True))
+    retriever = EvaluateRetrieval(model, k_values=[1, 3, 5, 10, 100, 1000])
+    results = retriever.retrieve(corpus, qs)
+    ndcg, _map, recall, precision = retriever.evaluate(qrels, results, retriever.k_values)
+
+    want = json.load(open(GOLDEN))
+    assert set(results) == set(queries) == set(want["results"])
+    for q, docs in want["results"].items():
+        assert set(results[q]) == set(docs), q
+        for d, v in docs.items():
+            assert abs(results[q][d] - v) <= 1e-5 * (1 + abs(v)), (q, d)
     for i in range(8):
         assert max(results[f"q{i}"], key=results[f"q{i}"].get) == f"d{i}"  # the planted document ranks first
         assert "d_empty" not in results[f"q{i}"]
-    nd = json.load(open(tmp_path / "beir_embeddings_ndcgs.json"))
-    assert nd["ndcgs"]["toy_model"]["toyset"]["NDCG@1"] == 1.0
-    assert nd["recalls"]["toy_model"]["toyset"]["Recall@10"] == 1.0
-    assert set(nd) >= {"ndcgs", "maps", "recalls", "precisions"}
-    # a second run finds the result file and skips (BDR:433-436)
-    mod.main(args)
+    for name, got in (("ndcgs", ndcg), ("maps", _map), ("recalls", recall), ("precisions", precision)):
+        ref = want["metrics"][name]["toy_model"]["toyset"]
+        assert set(got) == set(ref), name
+        for key, v in ref.items():
+            assert abs(got[key] - v) <= 1e-9, (name, key)

@@ -1,5 +1,5 @@
-// Stand-alone microbenchmark of bf16 -> bf16 LayerNorm kernel variants on B200 (tools/, not part of the library).
-//   build:  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -o tools/ln_bench tools/ln_bench.cu
+// Stand-alone microbenchmark of bf16 -> bf16 LayerNorm kernel variants (tools/, not part of the library).
+//   build:  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -o tools/ln_bench tools/ln_bench.cu
 //   run:    tools/ln_bench T d     (e.g. 32768 768, 16384 2048, 9600 4096)
 // Every variant is checked against a double-precision host LayerNorm of sampled rows (1 bf16 ulp), then timed with CUDA
 // events over 40 launches, L2-warm (the same 2 buffers) and L2-cold (rotating over buffer pairs > 126 MB in total).
