@@ -54,7 +54,8 @@ int sgpt_layernorm(const float* x, const float* gamma, const float* beta, void* 
  *     x bf16[M,K] (row pitch ldx), w bf16[N,K] (nn.Linear weight layout, row pitch ldw), bias fp32[N] or NULL.
  *     epilogue: SGPT_EPI_BF16       out bf16[M,N]  = acc + bias
  *               SGPT_EPI_GELU_BF16  out bf16[M,N]  = gelu_new(acc + bias)       (HF activations.py NewGELUActivation)
- *               SGPT_EPI_RESID_F32  out fp32[M,N]  = resid + acc + bias         (resid fp32[M,N], may alias out)
+ *               SGPT_EPI_RESID_F32  out fp32[M,N]  = resid + acc + bias         (resid fp32[M,N] with row pitch ldo,
+ *                                                                                may alias out; unchanged if it does not)
  *     Runs on the wgmma tensor cores (TMA-staged tiles, register accumulators). */
 #define SGPT_EPI_BF16 0
 #define SGPT_EPI_GELU_BF16 1

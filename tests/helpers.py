@@ -54,6 +54,67 @@ def min_row_cosine(a, b):
     return torch.nn.functional.cosine_similarity(a, b, dim=1).min().item()
 
 
+BF16_U = 2.0 ** -8  # unit roundoff of bf16 (8 significant bits, round to nearest): |bf16(x) - x| <= BF16_U |x|
+
+
+def tensor_core_sum_bound(abs_sum, K):
+    """Bound on the fp32 error of a K-term dot product accumulated by the GEMM on the tensor cores: at most K/16 + 16
+    roundings (one per k16 step into the accumulator, plus the sum of the 16 products inside one step), each at most 2^-23
+    (one ulp, so truncating adders are covered) of a partial sum, and every partial sum is at most
+    abs_sum = sum_k |x_k w_k|."""
+    return (K / 16 + 16) * 2.0 ** -23 * abs_sum
+
+
+def rotary_cos_sin(max_pos, rotary_dim):
+    """GPT-J's table in the layout of include/sgpt_b200.h: fp32[max_pos, rotary_dim/2, 2] = (cos, sin), from the oracle's
+    create_sinusoidal_positions (oracle/gptj.py rotary_tables)."""
+    from oracle.gptj import rotary_tables
+
+    sin, cos = rotary_tables(max_pos, rotary_dim)
+    return torch.stack([cos, sin], dim=-1).contiguous()
+
+
+def rotary_reference(y, pos, cos_sin, d, head_dim, rotary_dim):
+    """fp64 GPT-J rotary embedding of a fused projection y [M, 3d] = [q | k | v]: HF's rotate_every_two (oracle/gptj.py
+    apply_rotary) on the first rotary_dim dims of every q and k head, with the (cos, sin) values of the table at pos."""
+    from oracle.gptj import apply_rotary
+
+    M = y.shape[0]
+    cs = cos_sin.to(y.device).double()[pos.long()]  # [M, rd/2, 2]
+    qk = y[:, :2 * d].reshape(M, 2 * d // head_dim, head_dim).clone()
+    qk[..., :rotary_dim] = apply_rotary(qk[None, ..., :rotary_dim], cs[None, ..., 1], cs[None, ..., 0])[0]
+    return torch.cat([qk.view(M, 2 * d), y[:, 2 * d:]], dim=1)
+
+
+def rotary_abs_bound(e, pos, cos_sin, d, head_dim, rotary_dim):
+    """Propagates a per-element error bound e >= 0 of y through the rotation: the pair (e0, e1) becomes
+    (|c| e0 + |s| e1, |c| e1 + |s| e0) on the rotated dims; the other dims keep their bound."""
+    M = e.shape[0]
+    cs = cos_sin.to(e.device).double()[pos.long()].abs().repeat_interleave(2, dim=1)  # [M, rd, 2]
+    qk = e[:, :2 * d].reshape(M, 2 * d // head_dim, head_dim).clone()
+    r = qk[..., :rotary_dim]
+    swapped = r.reshape(M, -1, rotary_dim // 2, 2).flip(-1).reshape(r.shape)
+    qk[..., :rotary_dim] = r * cs[:, None, :, 0] + swapped * cs[:, None, :, 1]
+    return torch.cat([qk.view(M, 2 * d), e[:, 2 * d:]], dim=1)
+
+
+def left_padded_positions(M, max_pos, seed):
+    """Positions of M packed rows taken from a left-padded batch: up to three runs of consecutive positions, none starting
+    at 0, the last one ending at max_pos - 1 (int32)."""
+    g = torch.Generator().manual_seed(seed)
+    cuts = sorted(torch.randint(1, M, (2,), generator=g).tolist()) if M > 2 else []
+    runs, prev = [], 0
+    for c in cuts + [M]:
+        if c > prev:
+            runs.append(c - prev)
+        prev = c
+    pos = []
+    for i, n in enumerate(runs):
+        start = max_pos - n if i == len(runs) - 1 else int(torch.randint(1, max_pos - n + 1, (1,), generator=g))
+        pos.append(torch.arange(start, start + n))
+    return torch.cat(pos).to(torch.int32)
+
+
 class LazyF32Weights(dict):
     """bf16/fp32 CPU tensors that are widened to fp32 only while an oracle expression uses them: the functional oracles
     index the state dict once per use, so a 6-7 B-parameter model never exists in fp32 as a whole (12-14 GB of bf16 on

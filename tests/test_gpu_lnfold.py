@@ -107,6 +107,97 @@ def test_linear_resid_ln(M, K, N, with_bias):
     assert (rd.cpu().double() - want2).abs().max().item() < 4e-3 * max(1.0, want2.abs().max().item())
 
 
+def _lnfold_fp32_bound(x, wf, w, beta, eps):
+    """Bound on the fp32 error of act-free sgpt_linear_lnfold arithmetic, y = r acc - r mu c + b', against
+    LayerNorm(x) W^T + b in exact arithmetic, for inputs where the bf16 copy of x and the folded weights are exact (x is
+    bf16-representable, gamma a power of two).  Terms, each sum bounded by (number of roundings) * 2^-24 * (sum of |terms|):
+      - acc = xb W'^T on the tensor cores: tensor_core_sum_bound;
+      - column sums c and folded bias b' (one warp per row: K/32 terms per lane, then 5 shuffles): (K/32 + 5) 2^-24;
+      - row sums of x and x^2 (8-term trees and 4 shuffles per 128-column group, then P groups): (8 + P) 2^-24, which
+        moves mu by d_mu and var by d_var; 1/sqrt(var + eps) by rsqrtf (2 ulp) adds 2^-22, the products around it 2^-23;
+      - the two fmas of the epilogue: 2^-23 of the magnitudes they combine.
+    Returns the bound [M, N] (fp64) on the device of x."""
+    from tests.helpers import tensor_core_sum_bound
+
+    xx, wf, w, beta = x.double(), wf.double(), w.double(), beta.double()
+    K = xx.shape[1]
+    P = (K + 127) // 128
+    mu = xx.mean(1, keepdim=True)
+    ex2 = (xx * xx).mean(1, keepdim=True)
+    var = ex2 - mu * mu
+    r = 1.0 / torch.sqrt(var + eps)
+    n_st, n_fold = (8 + P) * 2.0 ** -24, (K / 32 + 5) * 2.0 ** -24
+    d_mu = n_st * xx.abs().mean(1, keepdim=True) + 2.0 ** -24 * mu.abs()
+    d_var = n_st * ex2 + 2 * mu.abs() * d_mu + 2.0 ** -22 * (ex2 + mu * mu)
+    rel_r = 0.5 * d_var / (var + eps) + 2.0 ** -22 + 2.0 ** -23
+    a1, c1, b1 = xx.abs() @ wf.abs().T, wf.abs().sum(1), beta.abs() @ w.abs().T
+    c = wf.sum(1)
+    dev_term = (xx @ wf.T - mu * c).abs()  # |acc - mu c| = |sum_k (x_k - mu) W'_k|
+    return (r * (tensor_core_sum_bound(a1, K) + mu.abs() * n_fold * c1 + c.abs() * d_mu) + n_fold * b1
+            + rel_r * r * dev_term + 2.0 ** -23 * (r * (a1 + mu.abs() * c1) + b1))
+
+
+@pytest.mark.parametrize("M", [1, 77, 129, 300])
+@pytest.mark.parametrize("d,hd,rd", [(4096, 256, 64), (1024, 256, 256), (512, 128, 8), (768, 64, 32)])
+def test_linear_qkv_rotary_lnfold_equals_layernorm_then_rotary_projection(d, hd, rd, M):
+    """GPT-J's q/k/v projection with ln_1 folded in (sgpt_fold_layernorm + sgpt_resid_stats +
+    sgpt_linear_qkv_rotary_lnfold) against fp64 LayerNorm(x) W^T followed by rotate_every_two on the first rotary_dim dims
+    of every q and k head (HF:gptj:400, :98-101, :55-67 + :196-207), positions of a left-padded batch up to max_pos - 1.
+    x is drawn in bf16 and gamma from {1/2, 1, 2}, so the bf16 copy of the residual and the folded weights are exact and
+    the kernel differs from the reference only by fp32 arithmetic (_lnfold_fp32_bound, mixed by the rotation) and the bf16
+    store (u = 2^-8).  v columns and non-rotary dims must equal sgpt_linear_lnfold's output bit for bit."""
+    from tests.helpers import (BF16_U, left_padded_positions, rotary_abs_bound, rotary_cos_sin, rotary_reference)
+
+    L, lib = _lib()
+    max_pos, eps, dev = 2048, 1e-5, "cuda"
+    N = 3 * d
+    g = torch.Generator().manual_seed(M * 13 + d + rd)
+    x = (torch.randn(M, d, generator=g) * 2.0 + 0.5).to(torch.bfloat16).float()  # residual stream rows, non-zero mean
+    w = (torch.randn(N, d, generator=g) * d ** -0.5).to(torch.bfloat16)
+    gamma = 2.0 ** torch.randint(-1, 2, (d,), generator=g).float()
+    beta = torch.randn(d, generator=g) * 0.05
+    pos = left_padded_positions(M, max_pos, seed=M + rd)
+    cos_sin = rotary_cos_sin(max_pos, rd)
+    wd, gd, bd, xd, pd, csd = w.to(dev), gamma.to(dev), beta.to(dev), x.to(dev), pos.to(dev), cos_sin.to(dev)
+    wf = torch.empty(N, d, dtype=torch.bfloat16, device=dev)
+    cs, bf = torch.empty(N, device=dev), torch.empty(N, device=dev)
+    L.check(lib.sgpt_fold_layernorm(wd.data_ptr(), gd.data_ptr(), bd.data_ptr(), None, wf.data_ptr(), cs.data_ptr(),
+                                    bf.data_ptr(), N, d, L.current_stream()), "sgpt_fold_layernorm")
+    P = (d + 127) // 128
+    xb = torch.empty(M, d, dtype=torch.bfloat16, device=dev)
+    st = torch.empty(M, P, 2, device=dev)
+    L.check(lib.sgpt_resid_stats(xd.data_ptr(), xb.data_ptr(), st.data_ptr(), M, d, L.current_stream()))
+    out = torch.full((M, N), float("nan"), dtype=torch.bfloat16, device=dev)
+    L.check(lib.sgpt_linear_qkv_rotary_lnfold(xb.data_ptr(), d, wf.data_ptr(), bf.data_ptr(), cs.data_ptr(), st.data_ptr(),
+                                              P, eps, out.data_ptr(), pd.data_ptr(), csd.data_ptr(), M, d, hd, rd, max_pos,
+                                              L.current_stream()), "sgpt_linear_qkv_rotary_lnfold")
+    plain = torch.full((M, N), float("nan"), dtype=torch.bfloat16, device=dev)
+    L.check(lib.sgpt_linear_lnfold(xb.data_ptr(), d, wf.data_ptr(), d, bf.data_ptr(), cs.data_ptr(), st.data_ptr(), P, eps,
+                                   plain.data_ptr(), N, M, N, d, 0, L.current_stream()), "sgpt_linear_lnfold")
+    torch.cuda.synchronize()
+    assert torch.equal(wf.cpu(), (w.float() * gamma).to(torch.bfloat16))  # exact fold: gamma is a power of two
+    got = out.cpu()
+    assert bool(torch.isfinite(got).all())
+    passthrough = torch.ones(N, dtype=torch.bool)
+    passthrough[:2 * d].view(-1, hd)[:, :rd] = False
+    assert torch.equal(got[:, passthrough].view(torch.int16), plain.cpu()[:, passthrough].view(torch.int16)), \
+        "v columns / non-rotary dims differ from the lnfold projection"
+
+    xx = xd.double()
+    ln = (xx - xx.mean(1, keepdim=True)) / torch.sqrt(xx.var(1, unbiased=False, keepdim=True) + eps) * gd.double() + bd.double()
+    want = rotary_reference(ln @ wd.double().T, pd, cos_sin, d, hd, rd).cpu()
+    e = _lnfold_fp32_bound(xd, wf, wd, bd, eps)
+    y_abs = (ln @ wd.double().T).abs()
+    e_rot = rotary_abs_bound(e + 2.0 ** -22 * y_abs, pd, cos_sin, d, hd, rd).cpu()
+    tol = BF16_U * want.abs() + (1 + BF16_U) * e_rot
+    err = (got.double() - want).abs()
+    if bool((err > tol).any()):
+        m, n = (err > tol).nonzero()[0].tolist()
+        raise AssertionError(f"{int((err > tol).sum())} elements out of tolerance; first qkv[{m},{n}] (head {n // hd}, dim "
+                             f"{n % hd}, pos {int(pos[m])}) = {float(got[m, n])}, want {float(want[m, n])} "
+                             f"(tol {float(tol[m, n])})")
+
+
 def test_ln_fold_block_flow_matches_reference_fixture(golden_dir, monkeypatch):
     """The opt-in block flow without LayerNorm passes (SGPT_LN_FOLD=1, csrc/model.cu) against the same HF fixture as the
     default flow: pooled embeddings within 1e-3 cosine, all-layer pooling modes, and the two flows agree with each other."""

@@ -58,6 +58,40 @@ def test_search_workspace_plan_is_consistent_across_query_blocks():
     assert ws(16, 80_000, k) > 16 * 80_000 * 4 + 256
 
 
+@pytest.mark.parametrize("change,message", [
+    (dict(hd=96), b"head_dim 96 not in {64,128,256}"),
+    (dict(hd=0), b"head_dim 0 not in {64,128,256}"),
+    (dict(window=-1), b"window must be >= 0"),
+    (dict(scale=0.0), b"scale must be positive"),
+    (dict(scale=-0.125), b"scale must be positive"),
+    (dict(scale=float("nan")), b"scale must be positive"),
+    (dict(impl=3), b"unknown impl 3"),
+    (dict(impl=-1), b"unknown impl -1"),
+    (dict(max_seqlen=0), b"max_seqlen must be positive"),
+    (dict(max_seqlen=-64), b"max_seqlen must be positive"),
+])
+def test_attention_rejects_bad_arguments(change, message):
+    """sgpt_attention validates its arguments before any CUDA call: SGPT_ERR_INVALID and a message naming the problem."""
+    from sgpt_b200 import _lib
+
+    lib = _lib.lib()
+    args = dict(B=1, T=4, H=2, hd=64, scale=0.125, window=0, max_seqlen=4, impl=0)
+    args.update(change)
+    rc = lib.sgpt_attention(None, None, None, args["B"], args["T"], args["H"], args["hd"], args["scale"], args["window"],
+                            args["max_seqlen"], None, args["impl"], None)
+    assert rc == 1  # SGPT_ERR_INVALID
+    assert message in lib.sgpt_last_error()
+
+
+def test_attention_empty_batch_is_a_no_op():
+    """T == 0 needs no max_seqlen and launches nothing (valid on a machine without a GPU)."""
+    from sgpt_b200 import _lib
+
+    lib = _lib.lib()
+    assert lib.sgpt_attention(None, None, None, 3, 0, 2, 64, 0.125, 0, 0, None, 0, None) == 0
+    assert lib.sgpt_attention(None, None, None, 0, 0, 2, 128, 1.0, 256, 0, None, 1, None) == 0
+
+
 def test_missing_library_fails_loudly(monkeypatch):
     from sgpt_b200 import _lib
 
