@@ -257,6 +257,12 @@ int sgpt_f32_to_bf16(const float* x, void* y, int64_t count, sgpt_stream_t strea
 int sgpt_scores(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* scores, int64_t lds,
                 int nq, int64_t n, int D, sgpt_stream_t stream);
 
+/* Order of every top-k result below (sgpt_topk, sgpt_topk_merge, sgpt_search, sgpt_search_packed,
+ * sgpt_topk_merge_packed, sgpt_search_gather): the k winners are the first k entries in (score descending, id ascending)
+ * order, returned in that order, so equal scores that straddle the cut keep the lowest ids and the result depends only on
+ * the input.  -0.0 and +0.0 are the same score.  Scores passed to sgpt_topk / sgpt_topk_merge must not be NaN (the
+ * library's own score producers map NaN to -1, XS:99).  1 <= k <= 4096. */
+
 /* S2. Row-wise exact top-k of a score matrix (torch.topk(..., largest=True, sorted=False), XS:102-108), with the
  *     winners returned in DESCENDING score order (ties: ascending id).  ids are offset by id_base (global doc ids of a
  *     shard).  scores fp32[nq, lds] (n valid columns); out_scores fp32[nq,k]; out_ids int64[nq,k].

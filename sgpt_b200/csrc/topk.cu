@@ -5,7 +5,8 @@
 //                         in shared memory.  Fast path: sample pivot -> one compaction pass -> exact k-th key by a radix-4
 //                         bitwise search on register-resident keys; fallback: MSD radix select (11 + 11 + 10 bits,
 //                         warp-aggregated histograms).  Then the k winners are placed, their ids fetched, and sorted
-//                         (score descending, id ascending).  Sources through `TopkSrc`:
+//                         (score descending, id ascending).  When equal scores straddle the cut, the ones with the
+//                         smallest ids win, so the k winners are the first k of that order.  Sources through `TopkSrc`:
 //                           - a dense score row           scores[q, 0..n)                    (ids = id_base + column)
 //                           - filtered candidate lists    packed (score, local idx) pairs with per-(list, query) counts,
 //                                                         optionally two-sided (front / back parts, topk.cuh)
@@ -24,8 +25,10 @@
 
 namespace sgpt {
 
+// -0.0 takes the key of +0.0: equal scores, so their order is decided by the ids like any other tie
 __device__ __forceinline__ uint32_t score_key(float x) {
-  const uint32_t u = __float_as_uint(x);
+  uint32_t u = __float_as_uint(x);
+  u = (u == 0x80000000u) ? 0u : u;
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 __device__ __forceinline__ float key_score(uint32_t k) {
@@ -82,6 +85,12 @@ __device__ __forceinline__ Elem load_elem(const TopkSrc& s, int q, int g, long l
   return load_elem_at(s, q, list_base(s, q, g, g >= s.G ? list_len(s, q, g) : 0) + i, i);
 }
 
+// Order of an element among equal scores (smaller = earlier), monotone in its id: explicit and global ids are >= 0 when
+// valid; a dense row or packed local entry is ordered by its index, i.e. id - id_base.
+__device__ __forceinline__ unsigned long long tie_order(const TopkSrc& s, long long id) {
+  return static_cast<unsigned long long>((s.ids != nullptr || s.packed_global) ? id : id - s.id_base);
+}
+
 constexpr int kTopkThreads = 1024;
 
 // Phase timeline of the selection kernel (sgpt_debug_topk_timeline): thread 0 of CTA 0 stamps %globaltimer at the phase
@@ -118,6 +127,19 @@ __device__ __forceinline__ uint2 block_sum2(uint32_t a, uint32_t b, uint2 (*buf)
   const uint2 t = buf[parity][lane];
   parity ^= 1u;
   return make_uint2(__reduce_add_sync(0xffffffffu, t.x), __reduce_add_sync(0xffffffffu, t.y));
+}
+// three sums at once (same single barrier)
+__device__ __forceinline__ uint4 block_sum3(uint32_t a, uint32_t b, uint32_t c, uint4 (*buf)[32], uint32_t& parity, int lane,
+                                            int warp) {
+  a = __reduce_add_sync(0xffffffffu, a);
+  b = __reduce_add_sync(0xffffffffu, b);
+  c = __reduce_add_sync(0xffffffffu, c);
+  if (lane == 0) buf[parity][warp] = make_uint4(a, b, c, 0u);
+  __syncthreads();
+  const uint4 t = buf[parity][lane];
+  parity ^= 1u;
+  return make_uint4(__reduce_add_sync(0xffffffffu, t.x), __reduce_add_sync(0xffffffffu, t.y),
+                    __reduce_add_sync(0xffffffffu, t.z), 0u);
 }
 
 // One radix-4 step of the bitwise search for the rank-th largest key: with `pv` fixed above bit b+1, the counts of keys
@@ -225,10 +247,11 @@ __global__ void __launch_bounds__(kTopkThreads, 1) topk_select_kernel(TopkSrc sr
   __shared__ uint32_t warp_tot[32];
   __shared__ uint32_t s_off[kMaxFlatLists + 1];  // padded list offsets in the flat index space
   __shared__ uint32_t s_len[kMaxFlatLists];
-  __shared__ uint32_t s_bin, s_need, s_cnt_gt, s_cnt_eq;
+  __shared__ uint32_t s_bin, s_bin_cnt, s_need, s_cnt_gt, s_cnt_eq, s_cnt_eq2;
   __shared__ uint32_t s_total;  // < 2^32 (checked by the launcher)
   __shared__ uint32_t s_red[2][32];
   __shared__ uint2 s_red2[2][32];
+  __shared__ uint4 s_red3[2][32];
 
   const int q = blockIdx.x;
   const int tid = threadIdx.x;
@@ -369,6 +392,7 @@ __global__ void __launch_bounds__(kTopkThreads, 1) topk_select_kernel(TopkSrc sr
   const uint32_t kk = total < static_cast<uint32_t>(k) ? total : static_cast<uint32_t>(k);
 
   uint32_t prefix = 0, mask = 0, need = kk;
+  uint32_t n_eq = 0;  // elements whose key equals the kk-th key (>= need)
   uint32_t sub_n = 0;
   bool use_sub = false;  // digits 2 and 3 run over the compacted survivors of digit 1 instead of all keys
   // ---- fast path (all keys cached in shared memory) ------------------------------------------------------------------
@@ -429,10 +453,15 @@ __global__ void __launch_bounds__(kTopkThreads, 1) topk_select_kernel(TopkSrc sr
 #pragma unroll 1
       for (int b = 30; b >= 0; b -= 2) pv = radix4_step<kSubPairs / kTopkThreads>(kr, pv, b, kk, s_red2, red_par, lane, warp);
       prefix = pv;
-      uint32_t cgt = 0;
+      uint32_t cgt = 0, ceq = 0;
 #pragma unroll
-      for (uint32_t i = 0; i < kSubPairs / kTopkThreads; ++i) cgt += (kr[i] > pv) ? 1u : 0u;
-      need = kk - block_sum(cgt, s_red, red_par, lane, warp);  // winners among the keys equal to the kk-th key
+      for (uint32_t i = 0; i < kSubPairs / kTopkThreads; ++i) {
+        cgt += (kr[i] > pv) ? 1u : 0u;
+        ceq += (kr[i] == pv) ? 1u : 0u;
+      }
+      const uint2 c = block_sum2(cgt, ceq, s_red2, red_par, lane, warp);
+      need = kk - c.x;  // winners among the keys equal to the kk-th key
+      n_eq = c.y;
       fast_done = true;
     }
   }
@@ -478,9 +507,11 @@ __global__ void __launch_bounds__(kTopkThreads, 1) topk_select_kernel(TopkSrc sr
         if (above + h1 >= need) {
           s_bin = 2 * tid + 1;
           s_need = need - above;
+          s_bin_cnt = h1;
         } else {
           s_bin = 2 * tid;
           s_need = need - above - h1;
+          s_bin_cnt = h0;
         }
       }
       __syncthreads();
@@ -504,10 +535,80 @@ __global__ void __launch_bounds__(kTopkThreads, 1) topk_select_kernel(TopkSrc sr
       }
       __syncthreads();
     }
+    n_eq = s_bin_cnt;  // count of the last digit's bin: the keys equal to the kk-th key
   }
   timeline_mark(7);
-  // prefix == key of the kk-th largest element; `need` of the elements equal to it are winners.
-  if (tid == 0) { s_cnt_gt = 0; s_cnt_eq = 0; }
+  // prefix == key of the kk-th largest element; `need` of the n_eq elements equal to it are winners.
+  auto list_of = [&](uint32_t j) {  // list of flat index j
+    int lo = 0, hi = nl;
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (s_off[mid] <= j) lo = mid; else hi = mid;
+    }
+    return lo;
+  };
+  // Ties at the cut (n_eq > need, rare on continuous scores): the `need` tied elements with the smallest ids win
+  // (tie_order), so the result depends on the input alone.  tie_T = the need-th smallest tie order among them, found by
+  // the bitwise counting search of radix4_step, ascending; tie_lt of them order below tie_T.  The normal case skips this.
+  const bool straddle = kk > 0 && n_eq > need;  // (block-uniform)
+  auto flat_tie_order = [&](uint32_t j) {  // tie order of flat index j
+    const int g = list_of(j);
+    return tie_order(src, load_elem(src, q, g, static_cast<long long>(j - s_off[g])).id);
+  };
+  unsigned long long tie_T = 0;
+  uint32_t tie_lt = 0;
+  if (straddle) {
+    auto for_each_tied = [&](auto&& f) {
+      if (fast_done) {
+        for (uint32_t e = tid; e < sub_n; e += kTopkThreads) {
+          const uint2 kj = sub_kj[e];
+          if (kj.x == prefix) f(flat_tie_order(kj.y));
+        }
+      } else if (cached) {
+        for (uint32_t j = tid; j < flat_total; j += kTopkThreads)
+          if (ckeys[j] == prefix) f(flat_tie_order(j));
+      } else {
+        for_each_elem<false>(src, nl, q, tid, s_off, s_len, [&](int g, long long i, bool) {
+          const Elem e = load_elem(src, q, g, i);
+          if (e.key == prefix) f(tie_order(src, e.id));
+        });
+      }
+    };
+    unsigned long long m = 0;  // OR of the tie orders: the search starts at its highest bit
+    for_each_tied([&](unsigned long long t) { m |= t; });
+    {
+      const uint32_t lo32 = __reduce_or_sync(0xffffffffu, static_cast<uint32_t>(m));
+      const uint32_t hi32 = __reduce_or_sync(0xffffffffu, static_cast<uint32_t>(m >> 32));
+      if (lane == 0) s_red2[red_par][warp] = make_uint2(lo32, hi32);
+      __syncthreads();
+      const uint2 t = s_red2[red_par][lane];
+      red_par ^= 1u;
+      m = (static_cast<unsigned long long>(__reduce_or_sync(0xffffffffu, t.y)) << 32) | __reduce_or_sync(0xffffffffu, t.x);
+    }
+    const int top = m ? 63 - __clzll(static_cast<long long>(m)) : -1;
+#pragma unroll 1
+    for (int b = top & ~1; b >= 0; b -= 2) {
+      const unsigned long long c1 = tie_T | (1ull << b), c2 = tie_T | (2ull << b), c3 = tie_T | (3ull << b);
+      uint32_t n1 = 0, n2 = 0, n3 = 0;
+      for_each_tied([&](unsigned long long t) {
+        n1 += (t < c1) ? 1u : 0u;
+        n2 += (t < c2) ? 1u : 0u;
+        n3 += (t < c3) ? 1u : 0u;
+      });
+      const uint4 c = block_sum3(n1, n2, n3, s_red3, red_par, lane, warp);
+      if (c.z < need) { tie_T = c3; tie_lt = c.z; }
+      else if (c.y < need) { tie_T = c2; tie_lt = c.y; }
+      else if (c.x < need) { tie_T = c1; tie_lt = c.x; }
+    }
+  }
+  // slot of a tied element among the `need` tied winners (>= need: not a winner); straddling ties only
+  auto tie_slot = [&](unsigned long long t) -> uint32_t {
+    if (t < tie_T) return atomicAdd(&s_cnt_eq, 1u);  // exactly tie_lt < need of them
+    if (t != tie_T) return need;
+    const uint32_t s = atomicAdd(&s_cnt_eq2, 1u);  // (copies of one (score, id) entry when a merge input repeats it)
+    return s < need - tie_lt ? tie_lt + s : need;
+  };
+  if (tid == 0) { s_cnt_gt = 0; s_cnt_eq = 0; s_cnt_eq2 = 0; }
   for (int i = tid; i < KP; i += kTopkThreads) { skey[i] = 0; sid[i] = -1; }
   __syncthreads();
   if (kk > 0) {
@@ -517,11 +618,18 @@ __global__ void __launch_bounds__(kTopkThreads, 1) topk_select_kernel(TopkSrc sr
         const uint32_t slot = atomicAdd(&s_cnt_gt, 1u);
         skey[slot] = key;
         sid[slot] = load_elem(src, q, g, i).id;
-      } else {
+      } else if (!straddle) {
         const uint32_t s = atomicAdd(&s_cnt_eq, 1u);
         if (s < need) {
           skey[n_gt + s] = key;
           sid[n_gt + s] = load_elem(src, q, g, i).id;
+        }
+      } else {
+        const long long id = load_elem(src, q, g, i).id;
+        const uint32_t s = tie_slot(tie_order(src, id));
+        if (s < need) {
+          skey[n_gt + s] = key;
+          sid[n_gt + s] = id;
         }
       }
     };
@@ -534,7 +642,7 @@ __global__ void __launch_bounds__(kTopkThreads, 1) topk_select_kernel(TopkSrc sr
           skey[slot] = kj.x;
           sid[slot] = static_cast<long long>(kj.y);  // flat position for now
         } else if (kj.x == prefix) {
-          const uint32_t e2 = atomicAdd(&s_cnt_eq, 1u);
+          const uint32_t e2 = straddle ? tie_slot(flat_tie_order(kj.y)) : atomicAdd(&s_cnt_eq, 1u);
           if (e2 < need) {
             skey[n_gt + e2] = kj.x;
             sid[n_gt + e2] = static_cast<long long>(kj.y);
@@ -544,23 +652,15 @@ __global__ void __launch_bounds__(kTopkThreads, 1) topk_select_kernel(TopkSrc sr
       __syncthreads();
       for (uint32_t t = tid; t < kk; t += kTopkThreads) {
         const uint32_t j = static_cast<uint32_t>(sid[t]);
-        int lo = 0, hi = nl;
-        while (hi - lo > 1) {
-          const int mid = (lo + hi) >> 1;
-          if (s_off[mid] <= j) lo = mid; else hi = mid;
-        }
-        sid[t] = load_elem(src, q, lo, static_cast<long long>(j - s_off[lo])).id;
+        const int g = list_of(j);
+        sid[t] = load_elem(src, q, g, static_cast<long long>(j - s_off[g])).id;
       }
     } else if (cached) {
       for (uint32_t j = tid; j < flat_total; j += kTopkThreads) {
         const uint32_t key = ckeys[j];
         if (key == 0 || key < prefix) continue;
-        int lo = 0, hi = nl;
-        while (hi - lo > 1) {
-          const int mid = (lo + hi) >> 1;
-          if (s_off[mid] <= j) lo = mid; else hi = mid;
-        }
-        place(key, lo, static_cast<long long>(j - s_off[lo]));
+        const int g = list_of(j);
+        place(key, g, static_cast<long long>(j - s_off[g]));
       }
     } else {
       for_each_elem<false>(src, nl, q, tid, s_off, s_len, [&](int g, long long i, bool) {

@@ -65,6 +65,26 @@ def tensor_core_sum_bound(abs_sum, K):
     return (K / 16 + 16) * 2.0 ** -23 * abs_sum
 
 
+def topk_reference(scores, ids, k, exclude=None):
+    """Exact top-k of candidate entries, the contract of include/sgpt_b200.h: per query the entries with id >= 0 and
+    id != exclude[q], ordered by score descending with ties by ascending id (-0.0 equal to +0.0), the first k, the tail
+    filled with (-inf, -1).  scores [nq, m] (any float dtype, values taken exactly), ids int64 [nq, m], exclude int64 [nq]
+    or None.  Returns (fp64 scores [nq, k], int64 ids [nq, k])."""
+    s = torch.as_tensor(scores).double().cpu().numpy()
+    i = torch.as_tensor(ids).cpu().numpy().astype(np.int64)
+    nq = s.shape[0]
+    out_s = np.full((nq, k), -np.inf)
+    out_i = np.full((nq, k), -1, dtype=np.int64)
+    for q in range(nq):
+        ok = i[q] >= 0
+        if exclude is not None:
+            ok &= i[q] != int(exclude[q])
+        sq, iq = s[q][ok] + 0.0, i[q][ok]  # (+ 0.0 turns -0.0 into +0.0)
+        order = np.lexsort((iq, -sq))[:k]  # last key primary: score descending, then id ascending
+        out_s[q, :len(order)], out_i[q, :len(order)] = sq[order], iq[order]
+    return torch.from_numpy(out_s), torch.from_numpy(out_i)
+
+
 def rotary_cos_sin(max_pos, rotary_dim):
     """GPT-J's table in the layout of include/sgpt_b200.h: fp32[max_pos, rotary_dim/2, 2] = (cos, sin), from the oracle's
     create_sinusoidal_positions (oracle/gptj.py rotary_tables)."""

@@ -514,6 +514,5 @@ def test_search_full_size_1m_docs_properties():
     sa, ia = a.search(q, k, "cos_sim")
     sb, ib = b.search(q, k, "cos_sim")
     sm, im = merge_topk(torch.stack([sa, sb]), torch.stack([ia, ib]))
-    assert (sm - s).abs().max().item() < 1e-6
-    agree = sum(len(set(x) & set(y)) for x, y in zip(im.tolist(), i.tolist())) / (nq * k)
-    assert agree > 0.999  # identical up to ties at the cut
+    # a document's score does not depend on its shard, and ties resolve to the lowest ids: identical bits
+    assert torch.equal(sm.view(torch.int32), s.view(torch.int32)) and torch.equal(im, i)

@@ -83,6 +83,58 @@ def test_attention_rejects_bad_arguments(change, message):
     assert message in lib.sgpt_last_error()
 
 
+def _topk_call(name, k=10, G=2, nq=1, id_base=0, n=100, D=64):
+    """One retrieval entry point with dummy (never dereferenced) host pointers: every rejection below happens before a
+    CUDA call."""
+    from sgpt_b200 import _lib
+
+    lib = _lib.lib()
+    dummy = np.zeros(64, dtype=np.int64)
+    p = dummy.ctypes.data
+    if name == "sgpt_topk":
+        return lib.sgpt_topk(p, n, nq, n, k, id_base, p, p, p, None)
+    if name == "sgpt_topk_merge":
+        return lib.sgpt_topk_merge(p, p, G, nq, k, p, p, None, p, None)
+    if name == "sgpt_topk_merge_packed":
+        return lib.sgpt_topk_merge_packed(p, G, nq, k, p, p, None, None)
+    if name == "sgpt_search":
+        return lib.sgpt_search(p, p, None, None, nq, n, D, k, id_base, p, p, p, 1 << 40, None)
+    if name == "sgpt_search_packed":
+        return lib.sgpt_search_packed(p, p, None, None, nq, n, D, k, id_base, p, p, 1 << 40, None)
+    raise ValueError(name)
+
+
+@pytest.mark.parametrize("name", ["sgpt_topk", "sgpt_topk_merge", "sgpt_topk_merge_packed"])
+@pytest.mark.parametrize("k", [0, 4097])
+def test_topk_entry_points_reject_k_outside_1_to_4096(name, k):
+    from sgpt_b200 import _lib
+
+    assert _topk_call(name, k=k) == 1  # SGPT_ERR_INVALID
+    assert f"k={k} outside [1, 4096]".encode() in _lib.lib().sgpt_last_error()
+
+
+@pytest.mark.parametrize("name,message", [("sgpt_topk_merge", b"bad sizes G=0"),
+                                          ("sgpt_topk_merge_packed", b"bad arguments G=0")])
+def test_merges_reject_zero_lists(name, message):
+    from sgpt_b200 import _lib
+
+    assert _topk_call(name, G=0) == 1
+    assert message in _lib.lib().sgpt_last_error()
+
+
+def test_search_rejects_ids_beyond_31_bits_and_ragged_dims():
+    """sgpt_search_packed stores int32 ids, so id_base + n must stay below 2^31; the GEMM needs D % 8 == 0."""
+    from sgpt_b200 import _lib
+
+    lib = _lib.lib()
+    n = 1000
+    assert _topk_call("sgpt_search_packed", id_base=(1 << 31) - n, n=n) == 1
+    assert b"global ids must fit 31 bits" in lib.sgpt_last_error()
+    for name in ("sgpt_search", "sgpt_search_packed"):
+        assert _topk_call(name, D=60) == 1
+        assert b"D=60 must be a positive multiple of 8" in lib.sgpt_last_error()
+
+
 def test_attention_empty_batch_is_a_no_op():
     """T == 0 needs no max_seqlen and launches nothing (valid on a machine without a GPU)."""
     from sgpt_b200 import _lib
