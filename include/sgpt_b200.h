@@ -292,6 +292,21 @@ int sgpt_search(const void* Q, const void* C, const float* q_scale, const float*
 int sgpt_search_packed(const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq, int64_t n,
                        int D, int k, int64_t id_base, uint64_t* out_packed, void* ws, int64_t ws_bytes,
                        sgpt_stream_t stream);
+/* Range search: every document of one shard whose score is >= threshold (the `cos_scores >= threshold` sets of
+ *     community_detection, ST/util.py:385-448, without the [nq, n] score matrix).  Q, C, q_scale, c_scale, D and id_base
+ *     as sgpt_search (NULL scale = dot product; a NaN score is -1, XS:99); any nq (blocks of 256 queries reuse ws).
+ *     out_counts int64[nq] (device) is always written: the number of documents with score >= threshold.  With
+ *     off[q] = counts[0] + ... + counts[q-1], query q's entries go to out_scores fp32 / out_ids int64
+ *     [off[q], off[q] + counts[q]) if and only if off[q] + counts[q] <= cap, in ascending id order, ids offset by
+ *     id_base; entries of queries that do not fit are not written and the rest of both buffers keeps its bits (cap = 0
+ *     only counts).  The output depends only on the input (no atomics decide the order).  SGPT_ERR_INVALID for a NaN
+ *     threshold, D % 8 != 0, n >= 2^31, nq < 0, cap < 0, null outputs that would be written and a workspace smaller
+ *     than sgpt_range_search_workspace_bytes(nq, n). */
+int64_t sgpt_range_search_workspace_bytes(int nq, int64_t n);
+int sgpt_range_search(const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq, int64_t n,
+                      int D, float threshold, int64_t id_base, int64_t* out_counts, int64_t cap, float* out_scores,
+                      int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
+
 /* S3 on packed lists: in_packed uint64[G,nq,k] (the all-gathered sgpt_search_packed outputs; chunk = shard in
  *     XS:121-132) -> out_scores fp32[nq,k], out_ids int64[nq,k]; ids < 0 and ids == exclude_ids[q] (XS:118) dropped.
  *     Every input list must be in the order sgpt_search_packed writes (score descending, id ascending on ties, empty

@@ -93,6 +93,8 @@ _SIGNATURES = {
     "sgpt_gather_connect": (i32, [vp, vp]),
     "sgpt_gather_destroy": (None, [vp]),
     "sgpt_search_gather": (i32, [vp, vp, vp, vp, vp, i32, i64, i32, i32, i64, vp, vp, vp, vp, i64, vp]),
+    "sgpt_range_search_workspace_bytes": (i64, [i32, i64]),
+    "sgpt_range_search": (i32, [vp, vp, vp, vp, i32, i64, i32, f32, i64, vp, i64, vp, vp, vp, i64, vp]),
 }
 
 ABI_VERSION = 3  # include/sgpt_b200.h SGPT_ABI_VERSION these signatures / struct layouts were written for

@@ -26,6 +26,15 @@ def _check_score_function(score_function: str) -> None:
                 score_function))
 
 
+def resolve_score_function(score_function) -> str:
+    """"cos_sim" / "dot", or the reference's ``cos_sim`` / ``dot_score`` callables recognised by name."""
+    if callable(score_function):
+        score_function = {"cos_sim": "cos_sim", "pytorch_cos_sim": "cos_sim", "dot_score": "dot"}.get(
+            getattr(score_function, "__name__", ""), None)
+    _check_score_function(score_function)
+    return score_function
+
+
 def to_bf16_rows(x: torch.Tensor) -> torch.Tensor:
     """fp32 [n, D] (device) -> bf16 [n, D] (round-to-nearest-even) with the library's conversion kernel."""
     x = x.contiguous()
@@ -107,17 +116,25 @@ class CorpusShard:
         shard.n = n
         return shard
 
-    def _prepare(self, queries: torch.Tensor, k: int, score_function: str):
-        """Queries -> bf16 rows + 1/||q|| (cos_sim) + a workspace large enough for this search."""
+    def _queries(self, queries: torch.Tensor, score_function: str):
+        """Queries -> bf16 rows + 1/||q|| of the rounded rows (cos_sim) + the shard's scale pointer (or None: dot)."""
         _check_score_function(score_function)
         q = queries.to(self.device)
         qb = q.contiguous() if q.dtype == torch.bfloat16 else to_bf16_rows(q.float())
         cos = score_function == "cos_sim"
         q_scale = row_inv_norms(qb) if cos else None
-        need = _lib.lib().sgpt_search_workspace_bytes(qb.shape[0], self.n, k)
+        return qb, q_scale, (self.inv_norms.data_ptr() if cos else None)
+
+    def _workspace(self, need: int) -> torch.Tensor:
         if self._ws is None or self._ws.numel() < need:
             self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
-        return qb, q_scale, (self.inv_norms.data_ptr() if cos else None)
+        return self._ws
+
+    def _prepare(self, queries: torch.Tensor, k: int, score_function: str):
+        """Queries -> bf16 rows + 1/||q|| (cos_sim) + a workspace large enough for this search."""
+        qb, q_scale, c_scale = self._queries(queries, score_function)
+        self._workspace(_lib.lib().sgpt_search_workspace_bytes(qb.shape[0], self.n, k))
+        return qb, q_scale, c_scale
 
     def search(self, queries: torch.Tensor, k: int, score_function: str = "cos_sim") -> Tuple[torch.Tensor, torch.Tensor]:
         """Exact top-k of this shard for fp32/bf16 queries [Q, D] (device).
@@ -150,6 +167,66 @@ class CorpusShard:
                                                self._ws.numel(), _lib.current_stream())
         _lib.check(rc, "sgpt_search_packed")
         return out
+
+    def view(self, start: int, end: int) -> "CorpusShard":
+        """Documents [start, end) of this shard as a shard of their own that shares the vectors; its ids are the
+        positions ``start ..`` inside this shard.  (The norms are copied: the kernels read them 16 bytes at a time.)"""
+        v = object.__new__(CorpusShard)
+        v.dim, v.capacity, v.id_base, v.device = self.dim, end - start, int(start), self.device
+        v.vectors = self.vectors[start:end]
+        v.inv_norms = self.inv_norms[start:end].clone()
+        v.n = end - start
+        v._ws = None
+        return v
+
+    def _range_call(self, qb: torch.Tensor, q_scale: Optional[torch.Tensor], c_scale: Optional[int], threshold: float,
+                    counts: torch.Tensor, cap: int, out_s: Optional[torch.Tensor], out_i: Optional[torch.Tensor]) -> None:
+        """One sgpt_range_search of the bf16 query rows qb (include/sgpt_b200.h): counts int64[Q] always, the entries of
+        the queries that fit into `cap` into out_s / out_i."""
+        nq = qb.shape[0]
+        ws = self._workspace(_lib.lib().sgpt_range_search_workspace_bytes(nq, self.n))
+        with torch.cuda.device(self.device):
+            rc = _lib.lib().sgpt_range_search(qb.data_ptr(), self.vectors.data_ptr(), _lib.ptr(q_scale), c_scale, nq,
+                                              self.n, self.dim, float(threshold), self.id_base, counts.data_ptr(), cap,
+                                              _lib.ptr(out_s), _lib.ptr(out_i), ws.data_ptr(), ws.numel(),
+                                              _lib.current_stream())
+        _lib.check(rc, "sgpt_range_search")
+
+    def _range(self, qb: torch.Tensor, q_scale: Optional[torch.Tensor], c_scale: Optional[int], threshold: float,
+               capacity: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        nq = qb.shape[0]
+        cap = max(4096, 64 * nq) if capacity is None else max(1, int(capacity))
+        counts = torch.empty(nq, dtype=torch.int64, device=self.device)
+        out_s = torch.empty(cap, dtype=torch.float32, device=self.device)
+        out_i = torch.empty(cap, dtype=torch.int64, device=self.device)
+        self._range_call(qb, q_scale, c_scale, threshold, counts, cap, out_s, out_i)
+        offsets = torch.zeros(nq + 1, dtype=torch.int64, device=self.device)
+        torch.cumsum(counts, 0, out=offsets[1:])
+        total = int(offsets[-1])
+        if total > cap:
+            # the queries that fitted are a prefix: grow the buffer and run the others once more into its tail
+            first = int(torch.searchsorted(offsets[1:], cap, right=True))
+            done = int(offsets[first])
+            grown_s = torch.empty(total, dtype=torch.float32, device=self.device)
+            grown_i = torch.empty(total, dtype=torch.int64, device=self.device)
+            grown_s[:done].copy_(out_s[:done])
+            grown_i[:done].copy_(out_i[:done])
+            rest = torch.empty(nq - first, dtype=torch.int64, device=self.device)
+            self._range_call(qb[first:], None if q_scale is None else q_scale[first:], c_scale, threshold, rest,
+                             total - done, grown_s[done:], grown_i[done:])
+            out_s, out_i = grown_s, grown_i
+        return offsets, out_s[:total], out_i[:total]
+
+    def range_search(self, queries: torch.Tensor, threshold: float, score_function: str = "cos_sim"
+                     ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """Every document whose score against a query is >= threshold, for fp32/bf16 queries [Q, D] (device).
+
+        Returns (offsets int64 [Q+1], scores fp32 [E], global ids int64 [E]) on the device: query q's documents are
+        entries offsets[q] .. offsets[q+1], in ascending id order.  Queries are rounded to bf16 and scored exactly as in
+        ``search``; a NaN score counts as -1.  The output buffer starts at 64 entries per query and grows once, for the
+        queries that did not fit."""
+        qb, q_scale, c_scale = self._queries(queries, score_function)
+        return self._range(qb, q_scale, c_scale, threshold)
 
 
 def unpack_topk(packed: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -196,10 +273,7 @@ def semantic_search(query_embeddings: torch.Tensor, corpus_embeddings: Union[tor
     "dot" or the reference's ``cos_sim`` / ``dot_score`` callables (recognised by name); the chunk sizes of the reference
     are accepted and ignored — the kernel streams the whole shard once and needs no score-matrix chunks."""
     del query_chunk_size, corpus_chunk_size
-    if callable(score_function):
-        score_function = {"cos_sim": "cos_sim", "pytorch_cos_sim": "cos_sim", "dot_score": "dot"}.get(
-            getattr(score_function, "__name__", ""), None)
-    _check_score_function(score_function)
+    score_function = resolve_score_function(score_function)
     q = torch.as_tensor(query_embeddings)
     if q.dim() == 1:
         q = q.unsqueeze(0)  # ST/util.py:214-217
