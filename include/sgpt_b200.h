@@ -316,6 +316,41 @@ int sgpt_topk_merge_packed(const uint64_t* in_packed, int G, int nq, int k, floa
                            const int64_t* exclude_ids, sgpt_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * int8 corpus shards: half the bytes per document of a bf16 shard, read by an int8 wgmma filter GEMM (s32 accumulate).
+ *
+ * Quantization of a row x (fp32, or bf16 widened to fp32) into q int8[D], scale fp32, cos_scale fp32, all in fp32
+ * round-to-nearest arithmetic:
+ *   amax = max |x_i|;
+ *   a row holding a NaN or +-inf: q = 0, scale = cos_scale = NaN (every score against it is NaN, i.e. -1 as XS:99);
+ *   amax == 0: q = 0, scale = cos_scale = 0;
+ *   otherwise m = 127.0f / amax, q_i = clamp(rint(x_i * m), -127, 127) (rint: half to even), scale = amax / 127.0f,
+ *   ss = sum q_i^2 (exact in integers), cos_scale = scale / fmaxf(scale * sqrtf((float)ss), 1e-12f) — F.normalize of the
+ *   dequantized row (ST/util.py:41-42) folded with the dequantization scale.
+ * Score: score[q,j] = fixnan(float_rn(sum_d Q[q,d] C[j,d]) * q_scale[q] * c_scale[j]), evaluated in that order; the dot
+ *   product is exact in s32 (D % 16 == 0 for the TMA row pitch and D <= 65536, so no int8 input, -128 included, can
+ *   overflow).  q_scale / c_scale: `scale` for dot products, `cos_scale` for cos_sim; NULL = 1.
+ * The _i8 entry points take the arguments of their bf16 counterparts with Q int8[nq,D] and C int8[n,D], return results
+ * in the same order (top-k: score descending, ties by ascending id, as above) and use the same workspace sizes
+ * (sgpt_search_workspace_bytes, sgpt_range_search_workspace_bytes).  Arguments are checked as for the bf16 entry points,
+ * and D % 16 != 0 or D > 65536 are rejected with SGPT_ERR_INVALID, before any CUDA call.
+ * ------------------------------------------------------------------------------------------------------------------ */
+/* x fp32[n,D] (x_bf16 = 0) or bf16[n,D] (x_bf16 = 1) -> q_out int8[n,D], scale_out / cos_scale_out fp32[n]; x and q_out
+ *     16-byte aligned. */
+int sgpt_quantize_rows_i8(const void* x, int x_bf16, void* q_out, float* scale_out, float* cos_scale_out, int64_t n,
+                          int D, sgpt_stream_t stream);
+int sgpt_scores_i8(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* scores, int64_t lds,
+                   int nq, int64_t n, int D, sgpt_stream_t stream);
+int sgpt_search_i8(const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq, int64_t n, int D,
+                   int k, int64_t id_base, float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes,
+                   sgpt_stream_t stream);
+int sgpt_search_packed_i8(const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq, int64_t n,
+                          int D, int k, int64_t id_base, uint64_t* out_packed, void* ws, int64_t ws_bytes,
+                          sgpt_stream_t stream);
+int sgpt_range_search_i8(const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq, int64_t n,
+                         int D, float threshold, int64_t id_base, int64_t* out_counts, int64_t cap, float* out_scores,
+                         int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * §8e without a collective library call: the per-shard top-k lists are PUSHED into every rank's gather buffer by the
  * final selection kernel itself (stores through NVLink peer mappings + a system-scope release per query) and merged by
  * a kernel that acquires those per-query counters — the reference's sequential chunk/heapq merge (XS:80-132) with
@@ -335,6 +370,10 @@ void sgpt_gather_destroy(sgpt_gather_t g);
 int sgpt_search_gather(sgpt_gather_t g, const void* Q, const void* C, const float* q_scale, const float* c_scale,
                        int nq, int64_t n, int D, int k, int64_t id_base, const int64_t* exclude_ids, float* out_scores,
                        int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
+/* The same on an int8 shard (Q int8[nq,D], C int8[n,D]; see the int8 shard section above). */
+int sgpt_search_gather_i8(sgpt_gather_t g, const void* Q, const void* C, const float* q_scale, const float* c_scale,
+                          int nq, int64_t n, int D, int k, int64_t id_base, const int64_t* exclude_ids, float* out_scores,
+                          int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Residual stream in bf16 (SGPT_RESID_BF16=1 when the model handle is created; default fp32).  HF keeps hidden_states in

@@ -95,6 +95,12 @@ _SIGNATURES = {
     "sgpt_search_gather": (i32, [vp, vp, vp, vp, vp, i32, i64, i32, i32, i64, vp, vp, vp, vp, i64, vp]),
     "sgpt_range_search_workspace_bytes": (i64, [i32, i64]),
     "sgpt_range_search": (i32, [vp, vp, vp, vp, i32, i64, i32, f32, i64, vp, i64, vp, vp, vp, i64, vp]),
+    "sgpt_quantize_rows_i8": (i32, [vp, i32, vp, vp, vp, i64, i32, vp]),
+    "sgpt_scores_i8": (i32, [vp, vp, vp, vp, vp, i64, i32, i64, i32, vp]),
+    "sgpt_search_i8": (i32, [vp, vp, vp, vp, i32, i64, i32, i32, i64, vp, vp, vp, i64, vp]),
+    "sgpt_search_packed_i8": (i32, [vp, vp, vp, vp, i32, i64, i32, i32, i64, vp, vp, i64, vp]),
+    "sgpt_range_search_i8": (i32, [vp, vp, vp, vp, i32, i64, i32, f32, i64, vp, i64, vp, vp, vp, i64, vp]),
+    "sgpt_search_gather_i8": (i32, [vp, vp, vp, vp, vp, i32, i64, i32, i32, i64, vp, vp, vp, vp, i64, vp]),
 }
 
 ABI_VERSION = 3  # include/sgpt_b200.h SGPT_ABI_VERSION these signatures / struct layouts were written for

@@ -11,19 +11,21 @@
 
 namespace sgpt {
 
-template <int BN, class Epi, int CL = 1>
+template <int BN, class Epi, int CL = 1, bool kS8 = false>
 static int launch_gemm(const void* a, int64_t lda, const void* b, int64_t ldb, int M, int N, int K,
                        const typename Epi::Params& ep, cudaStream_t stream, int cat = kCatGemm,
                        TileMap tmap = TileMap()) {
   using Cfg = GemmCfg<BN, EpiStaging<Epi>::value>;
+  // one 128-byte row segment per box row: 64 bf16 or 128 int8
+  auto make_map = kS8 ? make_tma_2d_u8 : make_tma_2d_bf16;
+  const uint32_t box_k = kS8 ? 2 * kGemmBK : kGemmBK;
   CUtensorMap ta, tb;
-  int rc = make_tma_2d_bf16(&ta, a, static_cast<uint64_t>(M), static_cast<uint64_t>(K), static_cast<uint64_t>(lda),
-                            kGemmBM, kGemmBK);
+  int rc = make_map(&ta, a, static_cast<uint64_t>(M), static_cast<uint64_t>(K), static_cast<uint64_t>(lda), kGemmBM,
+                    box_k);
   if (rc != SGPT_OK) return rc;
-  rc = make_tma_2d_bf16(&tb, b, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldb), BN,
-                        kGemmBK);
+  rc = make_map(&tb, b, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldb), BN, box_k);
   if (rc != SGPT_OK) return rc;
-  auto kern = gemm_bf16_tn_kernel<BN, Epi, CL>;
+  auto kern = gemm_bf16_tn_kernel<BN, Epi, CL, kS8>;
   static PerDeviceOnce attr_once;
   if (attr_once.first()) {
     SGPT_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
@@ -88,7 +90,12 @@ FilterGeometry filter_geometry(long long tiles, int nq) {
 // nq <= 128: one CTA per work unit (M = 128).  128 < nq <= 256: two CTAs per work unit, each with 128 of the queries and
 // the same corpus tile — the second read of the tile is an L2 hit, so one pass over the shard from HBM serves 256 queries.
 template <class P>
-static int launch_filter_gemm(const void* Q, const void* C, int nq, int n, int D, const P& p, cudaStream_t stream, TileMap tm) {
+static int launch_filter_gemm(const void* Q, const void* C, int nq, int n, int D, const P& p, cudaStream_t stream, TileMap tm,
+                              bool s8) {
+  if (s8) {
+    if (nq > kGemmBM) return launch_gemm<kSimBN, EpiFilterRows, 2, true>(Q, D, C, D, nq, n, D, p, stream, kCatScores, tm);
+    return launch_gemm<kSimBN, EpiFilterRows, 1, true>(Q, D, C, D, nq, n, D, p, stream, kCatScores, tm);
+  }
   if (nq > kGemmBM) return launch_gemm<kSimBN, EpiFilterRows, 2>(Q, D, C, D, nq, n, D, p, stream, kCatScores, tm);
   return launch_gemm<kSimBN, EpiFilterRows, 1>(Q, D, C, D, nq, n, D, p, stream, kCatScores, tm);
 }
@@ -96,7 +103,7 @@ static int launch_filter_gemm(const void* Q, const void* C, int nq, int n, int D
 int launch_filter_candidates(const void* Q, const void* C, const float* q_scale, const float* c_scale,
                              const float* tau, const float* tau_hi, uint2* cand, int* counts, int* counts_back,
                              long long stride_q, int L, int group0, int nq, int n, int D, int tile_mode, int tile_stride,
-                             cudaStream_t stream) {
+                             bool s8, cudaStream_t stream) {
   SGPT_REQUIRE(nq <= 2 * kGemmBM, "filter GEMM: at most %d queries per launch (got %d)", 2 * kGemmBM, nq);
   TileMap tm;
   tm.mode = tile_mode;
@@ -106,11 +113,11 @@ int launch_filter_candidates(const void* Q, const void* C, const float* q_scale,
                g.L);
   EpiFilterRows::Params p{q_scale, c_scale, tau, tau_hi, cand, counts, counts_back, stride_q, L, group0, nq, nullptr, 0, 0,
                           nq > kGemmBM ? 1 : 0};
-  return launch_filter_gemm(Q, C, nq, n, D, p, stream, tm);
+  return launch_filter_gemm(Q, C, nq, n, D, p, stream, tm, s8);
 }
 
 int launch_sample_maxima(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* pool,
-                         long long stride_p, int Lp, int nq, int n, int D, int tile_stride, cudaStream_t stream) {
+                         long long stride_p, int Lp, int nq, int n, int D, int tile_stride, bool s8, cudaStream_t stream) {
   SGPT_REQUIRE(nq <= 2 * kGemmBM, "sample GEMM: at most %d queries per launch (got %d)", 2 * kGemmBM, nq);
   TileMap tm;
   tm.mode = 1;
@@ -120,7 +127,7 @@ int launch_sample_maxima(const void* Q, const void* C, const float* q_scale, con
                "sample GEMM: maxima lists too small (Lp=%d < %d)", Lp, g.L / 4);
   EpiFilterRows::Params p{q_scale, c_scale, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, 0, nq, pool, stride_p, Lp,
                           nq > kGemmBM ? 1 : 0};
-  return launch_filter_gemm(Q, C, nq, n, D, p, stream, tm);
+  return launch_filter_gemm(Q, C, nq, n, D, p, stream, tm, s8);
 }
 
 }  // namespace sgpt
@@ -331,4 +338,18 @@ extern "C" int sgpt_scores(const void* Q, const void* C, const float* q_scale, c
   EpiScoresF32::Params p{scores, q_scale, c_scale, static_cast<long long>(lds)};
   // lanes = queries (A operand), columns = corpus rows (B operand, streamed once from HBM)
   return launch_gemm<128, EpiScoresF32>(Q, D, C, D, nq, static_cast<int>(n), D, p, stream, kCatScores);
+}
+
+extern "C" int sgpt_scores_i8(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* scores,
+                              int64_t lds, int nq, int64_t n, int D, sgpt_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  SGPT_REQUIRE(nq >= 0 && n >= 0, "sgpt_scores_i8: bad sizes nq=%d n=%lld", nq, (long long)n);
+  SGPT_REQUIRE(D > 0 && D % 16 == 0 && D <= kMaxDimI8, "sgpt_scores_i8: D=%d must be a positive multiple of 16, at most %d",
+               D, kMaxDimI8);
+  SGPT_REQUIRE(n < (1ll << 31), "sgpt_scores_i8: shard too large for one launch (n=%lld)", (long long)n);
+  SGPT_REQUIRE(lds >= n, "sgpt_scores_i8: lds < n");
+  SGPT_REQUIRE(nq == 0 || n == 0 || scores != nullptr, "sgpt_scores_i8: null output");
+  if (nq == 0 || n == 0) return SGPT_OK;
+  EpiScoresF32::Params p{scores, q_scale, c_scale, static_cast<long long>(lds)};
+  return launch_gemm<128, EpiScoresF32, 1, true>(Q, D, C, D, nq, static_cast<int>(n), D, p, stream, kCatScores);
 }

@@ -1,4 +1,5 @@
-// Persistent, warp-specialised wgmma GEMM for sm_90a:  C[M,N] = A[M,K] * B[N,K]^T  (bf16 in, fp32 accumulate).
+// Persistent, warp-specialised wgmma GEMM for sm_90a:  C[M,N] = A[M,K] * B[N,K]^T  (bf16 in, fp32 accumulate; int8 in,
+// s32 accumulate for the similarity kernels, see kS8).
 //
 //   A : activations / queries, row-major [M,K]  -> K-major wgmma operand A
 //   B : nn.Linear weight [out,in] / corpus shard [n,D], row-major [N,K] -> K-major wgmma operand B
@@ -23,6 +24,8 @@
 //   EpiStaged<Op> (similarity scores)  smem transpose so that lane = column pair and each warp instruction touches one
 //                 contiguous row segment.
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace sgpt {
@@ -97,12 +100,26 @@ __device__ __forceinline__ void wgmma_fence_acc(float (&d)[N]) {
 #pragma unroll
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+template <int N>
+__device__ __forceinline__ void wgmma_fence_acc(int32_t (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
 
 template <int BN>
-__device__ __forceinline__ void wgmma_bf16(float (&d)[BN / 2], uint64_t da, uint64_t db, int scale_d) {
+__device__ __forceinline__ void wgmma_mma(float (&d)[BN / 2], uint64_t da, uint64_t db, int scale_d) {
   if constexpr (BN == 128) wgmma_bf16_m64n128(d, da, db, scale_d);
   else wgmma_bf16_m64n256(d, da, db, scale_d);
 }
+template <int BN>
+__device__ __forceinline__ void wgmma_mma(int32_t (&d)[BN / 2], uint64_t da, uint64_t db, int scale_d) {
+  if constexpr (BN == 128) wgmma_s8_m64n128(d, da, db, scale_d);
+  else wgmma_s8_m64n256(d, da, db, scale_d);
+}
+
+// accumulator element -> the fp32 bits parked in shared memory (an s32 dot product is rounded to nearest: cvt.rn.f32.s32)
+__device__ __forceinline__ uint32_t acc_bits(float x) { return __float_as_uint(x); }
+__device__ __forceinline__ uint32_t acc_bits(int32_t x) { return __float_as_uint(__int2float_rn(x)); }
 
 // Optional selection of N-tiles: the similarity search scans a strided sample of corpus tiles first (to establish
 // per-query thresholds) and the remaining tiles afterwards.
@@ -149,11 +166,18 @@ struct TileMap {
 // CL = 2: two CTAs per work unit on the same N-tile and adjacent M-tiles (CTA r of the unit owns rows [128 r, 128 r + 128)
 //   of a 256 x BN tile group): the similarity search scans up to 256 queries per pass over the corpus this way, and both
 //   CTAs of a unit share the candidate-list group of the unit (EpiFilterRows).
-template <int BN, class Epi, int CL = 1>
+// kS8: int8 operands (int8 corpus shards, similarity epilogues only).  A K-block is then 128 int8 = the same 128 bytes per
+//   row as 64 bf16, so the stage layout, TMA boxes, descriptor steps and ring are unchanged; wgmma k32 accumulates in s32,
+//   exact for |dot| < 2^31, and the accumulator is converted to fp32 where it is parked in shared memory, so every
+//   epilogue runs unchanged.
+template <int BN, class Epi, int CL = 1, bool kS8 = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, int M,
                     int N, int K, const __grid_constant__ typename Epi::Params ep, TileMap tmap) {
   using Cfg = GemmCfg<BN, EpiStaging<Epi>::value>;
+  using Acc = typename std::conditional<kS8, int32_t, float>::type;
+  constexpr int kBK = kS8 ? 2 * kGemmBK : kGemmBK;  // K elements per k-block (128 bytes per row either way)
+  constexpr int kMmaK = kS8 ? 32 : 16;              // K elements per wgmma
   constexpr int kStages = Cfg::kStages;
   static_assert(CL == 1 || CL == 2, "work unit size");
   static_assert(Epi::kEpiWarps == 4 || Epi::kEpiWarps == 8, "4 or 8 epilogue warps");
@@ -178,7 +202,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
   const int n_tiles = tmap.count((N + BN - 1) / BN);                  // N-tiles this launch visits
   const int ksplit = tmap.ksplit;
   const int num_tiles = m_tiles * n_tiles * ksplit;  // work units
-  const int num_kb = (K + kGemmBK - 1) / kGemmBK;
+  const int num_kb = (K + kBK - 1) / kBK;
   const int kb_per = (num_kb + ksplit - 1) / ksplit;  // k-blocks per slice (the host keeps every slice non-empty)
 
   if (warp == kWarpProducer && lane == 0) {
@@ -213,8 +237,8 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
           uint8_t* sa = smem_tiles + stage * Cfg::kStageBytes;
           uint8_t* sb = sa + Cfg::kABytes;
           mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-          tma_load_2d(sa, &tma_a, &full_bar[stage], kb * kGemmBK, m0);
-          tma_load_2d(sb, &tma_b, &full_bar[stage], kb * kGemmBK, n0);
+          tma_load_2d(sa, &tma_a, &full_bar[stage], kb * kBK, m0);
+          tma_load_2d(sb, &tma_b, &full_bar[stage], kb * kBK, n0);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
@@ -256,9 +280,9 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
         Epi::template pre_tile<kColsPerWarp, kSlabBytes>(st, ep, m0, n0, lane, stage_slab, M, N);
       }
 
-      float acc[BN / 2];
+      Acc acc[BN / 2];
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      for (int i = 0; i < BN / 2; ++i) acc[i] = Acc(0);
       const int kb_begin = ks * kb_per, kb_end = min(num_kb, kb_begin + kb_per);
       int prev_stage = -1;
       for (int kb = kb_begin; kb < kb_end; ++kb) {
@@ -269,7 +293,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
         wgmma_fence_acc(acc);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < kGemmBK / 16; ++k) wgmma_bf16<BN>(acc, da + 2 * k, db + 2 * k, (kb > kb_begin || k > 0) ? 1 : 0);
+        for (int k = 0; k < kBK / kMmaK; ++k) wgmma_mma<BN>(acc, da + 2 * k, db + 2 * k, (kb > kb_begin || k > 0) ? 1 : 0);
         wgmma_commit();
         wgmma_fence_acc(acc);
         if constexpr (BN == 128) {
@@ -303,8 +327,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
             const uint32_t col = 8 * j + 2 * (t & 3);
             const uint32_t chunk = col >> 2;
             const uint32_t phys = (chunk & ~7u) | ((chunk & 7u) ^ sw);
-            sts_v2(rbase + phys * 16 + (col & 3u) * 4, __float_as_uint(acc[4 * j + 2 * h]),
-                   __float_as_uint(acc[4 * j + 2 * h + 1]));
+            sts_v2(rbase + phys * 16 + (col & 3u) * 4, acc_bits(acc[4 * j + 2 * h]), acc_bits(acc[4 * j + 2 * h + 1]));
           }
         }
       }

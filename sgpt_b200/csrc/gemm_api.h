@@ -6,6 +6,8 @@
 namespace sgpt {
 
 constexpr int kSimBN = 256;  // corpus rows per similarity tile (N-tile width of the query x corpus GEMM)
+// int8 operands: at most this many dimensions, so that no s32 dot product can overflow (2^16 x 128 x 128 = 2^30)
+constexpr int kMaxDimI8 = 65536;
 
 // Geometry of the candidate lists the filter GEMM writes for a launch over `tiles` corpus tiles: every (CTA, column
 // half) is a group with a private list of `L` entries per query (worst case: every score of every visited tile).
@@ -19,16 +21,16 @@ FilterGeometry filter_geometry(long long tiles, int nq);
 // index) to the list cand[q * stride_q + (group0 + g) * L + ...] — scores >= tau_hi[q] at its front, the others at its
 // back (tau_hi == nullptr: all at the front) — and writes counts / counts_back[(group0 + g) * nq + q] for the groups g of
 // this launch (filter_geometry of the visited tile count).  tile_mode/tile_stride select the corpus tiles visited
-// (gemm.cuh TileMap).  nq <= 256 (above 128: CTA pairs, M = 256).
+// (gemm.cuh TileMap).  nq <= 256 (above 128: CTA pairs, M = 256).  s8: Q and C are int8 rows (gemm.cuh kS8), else bf16.
 int launch_filter_candidates(const void* Q, const void* C, const float* q_scale, const float* c_scale,
                              const float* tau, const float* tau_hi, uint2* cand, int* counts, int* counts_back,
                              long long stride_q, int L, int group0, int nq, int n, int D, int tile_mode, int tile_stride,
-                             cudaStream_t stream);
+                             bool s8, cudaStream_t stream);
 
 // The same GEMM over every tile_stride-th corpus tile in sample mode: pool[q * stride_p + g * Lp + ...] receives the
 // maximum score of every 4 consecutive documents the group visited (filter_geometry(sampled tiles).L / 4 floats per list,
 // unused slots = 0xffffffff).  Input of launch_tau_select (topk.cuh).
 int launch_sample_maxima(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* pool,
-                         long long stride_p, int Lp, int nq, int n, int D, int tile_stride, cudaStream_t stream);
+                         long long stride_p, int Lp, int nq, int n, int D, int tile_stride, bool s8, cudaStream_t stream);
 
 }  // namespace sgpt

@@ -193,13 +193,17 @@ extern "C" int64_t sgpt_range_search_workspace_bytes(int nq, int64_t n) {
   return kHeadBytes + b;
 }
 
-extern "C" int sgpt_range_search(const void* Q, const void* Cm, const float* q_scale, const float* c_scale, int nq,
-                                 int64_t n, int D, float threshold, int64_t id_base, int64_t* out_counts, int64_t cap,
-                                 float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes,
-                                 sgpt_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+// s8: Q and C are int8 rows (gemm.cuh kS8); everything after the filter GEMM is the same
+static int range_search(const void* Q, const void* Cm, const float* q_scale, const float* c_scale, int nq, int64_t n, int D,
+                        float threshold, int64_t id_base, int64_t* out_counts, int64_t cap, float* out_scores,
+                        int64_t* out_ids, void* ws, int64_t ws_bytes, bool s8, cudaStream_t stream) {
   SGPT_REQUIRE(threshold == threshold, "sgpt_range_search: threshold is NaN");
-  SGPT_REQUIRE(D > 0 && D % 8 == 0, "sgpt_range_search: D=%d must be a positive multiple of 8", D);
+  if (s8)
+    SGPT_REQUIRE(D > 0 && D % 16 == 0 && D <= kMaxDimI8,
+                 "sgpt_range_search: int8 D=%d must be a positive multiple of 16, at most %d", D, kMaxDimI8);
+  else
+    SGPT_REQUIRE(D > 0 && D % 8 == 0, "sgpt_range_search: D=%d must be a positive multiple of 8", D);
+  const size_t row_bytes = static_cast<size_t>(D) * (s8 ? 1 : 2);
   SGPT_REQUIRE(n >= 0 && n < (1ll << 31), "sgpt_range_search: shard size n=%lld outside [0, 2^31)", (long long)n);
   SGPT_REQUIRE(nq >= 0 && cap >= 0, "sgpt_range_search: bad sizes nq=%d cap=%lld", nq, (long long)cap);
   SGPT_REQUIRE(nq == 0 || out_counts != nullptr, "sgpt_range_search: null out_counts");
@@ -234,12 +238,12 @@ extern "C" int sgpt_range_search(const void* Q, const void* Cm, const float* q_s
     int* qcount = reinterpret_cast<int*>(w);
     w += align256(nb * 4);
     long long* qoff = reinterpret_cast<long long*>(w);
-    const void* Qb = static_cast<const uint8_t*>(Q) + static_cast<size_t>(q0) * D * 2;
+    const void* Qb = static_cast<const uint8_t*>(Q) + static_cast<size_t>(q0) * row_bytes;
     const float* qs = q_scale ? q_scale + q0 : nullptr;
 
     if (n > 0) {
       int rc = launch_filter_candidates(Qb, Cm, qs, c_scale, tau, nullptr, cand, cnt, nullptr, l.stride_q, l.g.L, 0, nb,
-                                        static_cast<int>(n), D, /*tile_mode=*/0, 1, stream);
+                                        static_cast<int>(n), D, /*tile_mode=*/0, 1, s8, stream);
       if (rc != SGPT_OK) return rc;
     }
     LaunchScope _ls(kCatTopk, stream);
@@ -259,4 +263,20 @@ extern "C" int sgpt_range_search(const void* Q, const void* Cm, const float* q_s
     }
   }
   return SGPT_OK;
+}
+
+extern "C" int sgpt_range_search(const void* Q, const void* Cm, const float* q_scale, const float* c_scale, int nq,
+                                 int64_t n, int D, float threshold, int64_t id_base, int64_t* out_counts, int64_t cap,
+                                 float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes,
+                                 sgpt_stream_t stream_) {
+  return range_search(Q, Cm, q_scale, c_scale, nq, n, D, threshold, id_base, out_counts, cap, out_scores, out_ids, ws,
+                      ws_bytes, false, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int sgpt_range_search_i8(const void* Q, const void* Cm, const float* q_scale, const float* c_scale, int nq,
+                                    int64_t n, int D, float threshold, int64_t id_base, int64_t* out_counts, int64_t cap,
+                                    float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes,
+                                    sgpt_stream_t stream_) {
+  return range_search(Q, Cm, q_scale, c_scale, nq, n, D, threshold, id_base, out_counts, cap, out_scores, out_ids, ws,
+                      ws_bytes, true, static_cast<cudaStream_t>(stream_));
 }

@@ -80,19 +80,7 @@ class PeerGather:
                exclude_ids: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
         """Local exact top-k of `shard` (CorpusShard) -> push to all ranks -> merge.  Identical (scores fp32 [Q,k], ids
         int64 [Q,k]) on every rank."""
-        from . import _lib
-
-        qb, q_scale, c_scale = shard._prepare(queries, k, score_function)
-        nq = qb.shape[0]
-        out_s = torch.empty((nq, k), dtype=torch.float32, device=self.device)
-        out_i = torch.empty((nq, k), dtype=torch.int64, device=self.device)
-        with torch.cuda.device(self.device):
-            rc = self._lib.sgpt_search_gather(self._handle, qb.data_ptr(), shard.vectors.data_ptr(), _lib.ptr(q_scale),
-                                              c_scale, nq, shard.n, shard.dim, k, shard.id_base, _lib.ptr(exclude_ids),
-                                              out_s.data_ptr(), out_i.data_ptr(), shard._ws.data_ptr(),
-                                              shard._ws.numel(), _lib.current_stream())
-        _lib.check(rc, "sgpt_search_gather")
-        return out_s, out_i
+        return shard.search_gather(self._handle, queries, k, score_function, exclude_ids)
 
     def close(self):
         if getattr(self, "_handle", None):
@@ -136,14 +124,16 @@ class ShardedDenseRetrievalExactSearch:
     documents into one resident ``CorpusShard``, scans it once, and the per-rank top-(k+1) lists meet in one all-gather
     followed by the merge kernel — the reference's "chunk, top-k, heapq merge" with chunk = rank.  Every rank returns the
     same ``Dict[qid, Dict[cid, float]]``.  ``shard_factory(dim, capacity)`` / ``merge`` default to ``CorpusShard`` and the
-    CUDA merge kernel; the CPU tests inject stand-ins and run it on ``gloo``.
+    CUDA merge kernel; the CPU tests inject stand-ins and run it on ``gloo``.  ``shard_dtype="int8"`` stores the resident
+    shards as int8 (half the memory per document, CorpusShard) instead of bf16.
     """
 
     def __init__(self, model, batch_size: int = 128, corpus_chunk_size: int = 50000, group=None,
                  shard_factory: Optional[Callable] = None, merge: Optional[Callable] = None, peer_gather: bool = False,
-                 **kwargs):
+                 shard_dtype: str = "bf16", **kwargs):
         self.model, self.batch_size, self.corpus_chunk_size = model, batch_size, corpus_chunk_size
         self.group, self.shard_factory, self.merge = group, shard_factory, merge
+        self.shard_dtype = shard_dtype
         self.peer_gather = peer_gather  # exchange through NVLink peer mappings (PeerGather) instead of one NCCL all-gather
         self.show_progress_bar, self.convert_to_tensor = True, True
         self.results = {}
@@ -174,7 +164,8 @@ class ShardedDenseRetrievalExactSearch:
             from .index import CorpusShard
 
             # the shard numbers its rows rank * cap + j, so a merged id still names its owner: (id // cap, id % cap)
-            shard = CorpusShard(q_emb.shape[1], max(len(mine), 1), device=self.device, id_base=rank * cap)
+            shard = CorpusShard(q_emb.shape[1], max(len(mine), 1), device=self.device, id_base=rank * cap,
+                                dtype=self.shard_dtype)
         else:
             shard = self.shard_factory(q_emb.shape[1], max(len(mine), 1))
         for batch_num, start in enumerate(range(0, len(mine), self.corpus_chunk_size)):

@@ -3,6 +3,10 @@
 A shard holds the embeddings of a contiguous range of documents as a bf16 matrix [n, D] (read once per search at
 HBM speed) plus fp32 1/||row|| of the STORED rows, so cosine scores are exactly ``cos_sim`` of the stored vectors
 (sentence_transformers/util.py:24-43) and dot scores are exactly ``dot_score`` (:46-63).
+
+An int8 shard (``dtype="int8"``) holds int8 rows [n, D] with a per-row scale and cos-scale instead: half the bytes per
+document, so twice the documents per GPU and half the HBM traffic per search.  Queries are quantized the same way, and
+scores are those of the dequantized vectors (include/sgpt_b200.h, int8 corpus shards).
 """
 from __future__ import annotations
 
@@ -16,6 +20,7 @@ import torch
 from . import _lib
 
 SCORE_FUNCTIONS = ("cos_sim", "dot")
+SHARD_DTYPES = ("bf16", "int8")
 
 
 def _check_score_function(score_function: str) -> None:
@@ -45,6 +50,22 @@ def to_bf16_rows(x: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def quantize_rows_i8(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """fp32 or bf16 [n, D] (device) -> (int8 [n, D], scale fp32 [n], cos_scale fp32 [n]) with the library's quantizer."""
+    if x.dtype != torch.bfloat16:
+        x = x.float()
+    x = x.contiguous()
+    n, D = x.shape
+    q = torch.empty((n, D), dtype=torch.int8, device=x.device)
+    scale = torch.empty(n, dtype=torch.float32, device=x.device)
+    cos_scale = torch.empty(n, dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.lib().sgpt_quantize_rows_i8(x.data_ptr(), int(x.dtype == torch.bfloat16), q.data_ptr(),
+                                                    scale.data_ptr(), cos_scale.data_ptr(), n, D, _lib.current_stream()),
+                   "sgpt_quantize_rows_i8")
+    return q, scale, cos_scale
+
+
 def row_inv_norms(x_bf16: torch.Tensor) -> torch.Tensor:
     n, D = x_bf16.shape
     out = torch.empty(n, dtype=torch.float32, device=x_bf16.device)
@@ -53,32 +74,55 @@ def row_inv_norms(x_bf16: torch.Tensor) -> torch.Tensor:
     return out
 
 
-class CorpusShard:
-    """Documents [id_base, id_base + n) of a corpus, resident in the HBM of one GPU."""
+def _check_dtype(dtype: str, dim: int) -> None:
+    if dtype not in SHARD_DTYPES:
+        raise ValueError(f"shard dtype {dtype!r} must be one of {SHARD_DTYPES}")
+    if dim % (16 if dtype == "int8" else 8) != 0:
+        raise ValueError(f"embedding dimension must be a multiple of {16 if dtype == 'int8' else 8} for {dtype} shards")
+    if dtype == "int8" and dim > 65536:
+        raise ValueError("int8 shards hold at most 65536 dimensions")
 
-    def __init__(self, dim: int, capacity: int, device="cuda:0", id_base: int = 0):
-        if dim % 8 != 0:
-            raise ValueError("embedding dimension must be a multiple of 8")
-        self.dim, self.capacity, self.id_base = int(dim), int(capacity), int(id_base)
+
+class CorpusShard:
+    """Documents [id_base, id_base + n) of a corpus, resident in the HBM of one GPU.
+
+    ``dtype="bf16"``: ``vectors`` bf16 [capacity, D] and ``inv_norms`` fp32.  ``dtype="int8"``: ``vectors`` int8
+    [capacity, D], ``scales`` and ``cos_scales`` fp32 (include/sgpt_b200.h, int8 corpus shards)."""
+
+    def __init__(self, dim: int, capacity: int, device="cuda:0", id_base: int = 0, dtype: str = "bf16"):
+        _check_dtype(dtype, dim)
+        self.dim, self.capacity, self.id_base, self.dtype = int(dim), int(capacity), int(id_base), dtype
         self.device = torch.device(device)
-        self.vectors = torch.empty((self.capacity, self.dim), dtype=torch.bfloat16, device=self.device)
-        self.inv_norms = torch.empty(self.capacity, dtype=torch.float32, device=self.device)
+        if dtype == "int8":
+            self.vectors = torch.empty((self.capacity, self.dim), dtype=torch.int8, device=self.device)
+            self.scales = torch.empty(self.capacity, dtype=torch.float32, device=self.device)
+            self.cos_scales = torch.empty(self.capacity, dtype=torch.float32, device=self.device)
+        else:
+            self.vectors = torch.empty((self.capacity, self.dim), dtype=torch.bfloat16, device=self.device)
+            self.inv_norms = torch.empty(self.capacity, dtype=torch.float32, device=self.device)
         self.n = 0
         self._ws: Optional[torch.Tensor] = None
 
     @classmethod
-    def from_embeddings(cls, emb: torch.Tensor, device=None, id_base: int = 0) -> "CorpusShard":
+    def from_embeddings(cls, emb: torch.Tensor, device=None, id_base: int = 0, dtype: str = "bf16") -> "CorpusShard":
         device = device or emb.device
-        shard = cls(emb.shape[1], emb.shape[0], device=device, id_base=id_base)
+        shard = cls(emb.shape[1], emb.shape[0], device=device, id_base=id_base, dtype=dtype)
         shard.add(emb)
         return shard
 
     def add(self, emb: torch.Tensor) -> None:
-        """Append fp32 (or bf16) embeddings [m, D]; they are stored bf16-rounded."""
+        """Append fp32 (or bf16) embeddings [m, D]; a bf16 shard stores them bf16-rounded, an int8 shard quantized."""
         m = emb.shape[0]
         if self.n + m > self.capacity:
             raise ValueError(f"shard capacity {self.capacity} exceeded ({self.n} + {m})")
         emb = emb.to(self.device)
+        if self.dtype == "int8":
+            q, scale, cos_scale = quantize_rows_i8(emb)
+            self.vectors[self.n:self.n + m].copy_(q)
+            self.scales[self.n:self.n + m].copy_(scale)
+            self.cos_scales[self.n:self.n + m].copy_(cos_scale)
+            self.n += m
+            return
         rows = emb if emb.dtype == torch.bfloat16 else to_bf16_rows(emb.float())
         self.vectors[self.n:self.n + m].copy_(rows)
         self.inv_norms[self.n:self.n + m].copy_(row_inv_norms(self.vectors[self.n:self.n + m]))
@@ -89,39 +133,68 @@ class CorpusShard:
 
     # ---- persistence (replaces the pickle-per-chunk embedding cache of BDR:311-323, 336-342) ----------------------
     def save(self, path: str) -> None:
-        """Write the shard as ``path/{vectors.npy (bf16 bit patterns as uint16), inv_norms.npy, meta.json}``; one
-        directory per rank for a sharded corpus."""
+        """Write the shard as ``path/{vectors.npy, <scales>, meta.json}``; one directory per rank for a sharded corpus.
+        bf16: vectors.npy holds the bf16 bit patterns as uint16, inv_norms.npy the fp32 1/||row||.  int8: vectors.npy
+        holds the int8 rows, scales.npy fp32 [n, 2] the (scale, cos_scale) of every row."""
         os.makedirs(path, exist_ok=True)
-        np.save(os.path.join(path, "vectors.npy"), self.stored().view(torch.int16).cpu().numpy().view(np.uint16))
-        np.save(os.path.join(path, "inv_norms.npy"), self.inv_norms[:self.n].cpu().numpy())
+        if self.dtype == "int8":
+            np.save(os.path.join(path, "vectors.npy"), self.stored().cpu().numpy())
+            np.save(os.path.join(path, "scales.npy"),
+                    torch.stack([self.scales[:self.n], self.cos_scales[:self.n]], 1).cpu().numpy())
+        else:
+            np.save(os.path.join(path, "vectors.npy"), self.stored().view(torch.int16).cpu().numpy().view(np.uint16))
+            np.save(os.path.join(path, "inv_norms.npy"), self.inv_norms[:self.n].cpu().numpy())
         with open(os.path.join(path, "meta.json"), "w") as f:
-            json.dump({"format": "sgpt_b200.CorpusShard/1", "dtype": "bf16", "dim": self.dim, "n": self.n,
+            json.dump({"format": "sgpt_b200.CorpusShard/1", "dtype": self.dtype, "dim": self.dim, "n": self.n,
                        "id_base": self.id_base}, f)
 
     @classmethod
     def load(cls, path: str, device="cuda:0", capacity: Optional[int] = None) -> "CorpusShard":
-        """Reload a shard written by ``save`` (bit-identical vectors and norms, so identical search results)."""
+        """Reload a shard written by ``save`` (bit-identical vectors and scales, so identical search results).  The
+        files are checked against meta.json before anything is allocated on the device."""
         with open(os.path.join(path, "meta.json")) as f:
             meta = json.load(f)
-        if meta.get("format") != "sgpt_b200.CorpusShard/1" or meta.get("dtype") != "bf16":
+        if meta.get("format") != "sgpt_b200.CorpusShard/1":
             raise ValueError(f"{path}: not a CorpusShard directory ({meta})")
-        vec = np.load(os.path.join(path, "vectors.npy"), mmap_mode="r")
-        inv = np.load(os.path.join(path, "inv_norms.npy"))
+        dtype = meta.get("dtype")
+        if dtype not in SHARD_DTYPES:
+            raise ValueError(f"{path}: unknown shard dtype {dtype!r} (expected one of {SHARD_DTYPES})")
         n, dim = int(meta["n"]), int(meta["dim"])
-        if vec.shape != (n, dim) or vec.dtype != np.uint16 or inv.shape != (n,):
-            raise ValueError(f"{path}: array shapes {vec.shape}/{inv.shape} do not match meta {meta}")
-        shard = cls(dim, max(n, capacity or n), device=device, id_base=int(meta["id_base"]))
-        shard.vectors[:n].copy_(torch.from_numpy(np.array(vec).view(np.int16)).view(torch.bfloat16))
-        shard.inv_norms[:n].copy_(torch.from_numpy(inv))
+        vec = np.load(os.path.join(path, "vectors.npy"), mmap_mode="r")
+        if dtype == "int8":
+            sc = np.load(os.path.join(path, "scales.npy"))
+            if vec.shape != (n, dim) or vec.dtype != np.int8 or sc.shape != (n, 2) or sc.dtype != np.float32:
+                raise ValueError(f"{path}: array shapes {vec.shape}/{sc.shape} do not match meta {meta}")
+        else:
+            inv = np.load(os.path.join(path, "inv_norms.npy"))
+            if vec.shape != (n, dim) or vec.dtype != np.uint16 or inv.shape != (n,):
+                raise ValueError(f"{path}: array shapes {vec.shape}/{inv.shape} do not match meta {meta}")
+        shard = cls(dim, max(n, capacity or n), device=device, id_base=int(meta["id_base"]), dtype=dtype)
+        if dtype == "int8":
+            shard.vectors[:n].copy_(torch.from_numpy(np.array(vec)))
+            shard.scales[:n].copy_(torch.from_numpy(np.ascontiguousarray(sc[:, 0])))
+            shard.cos_scales[:n].copy_(torch.from_numpy(np.ascontiguousarray(sc[:, 1])))
+        else:
+            shard.vectors[:n].copy_(torch.from_numpy(np.array(vec).view(np.int16)).view(torch.bfloat16))
+            shard.inv_norms[:n].copy_(torch.from_numpy(inv))
         shard.n = n
         return shard
 
+    def _fn(self, name: str):
+        """The library entry point `name` for this shard's format (the `_i8` variant on an int8 shard)."""
+        return getattr(_lib.lib(), name + "_i8" if self.dtype == "int8" else name)
+
     def _queries(self, queries: torch.Tensor, score_function: str):
-        """Queries -> bf16 rows + 1/||q|| of the rounded rows (cos_sim) + the shard's scale pointer (or None: dot)."""
+        """Queries -> rows in the shard's format + their scales + the shard's scale pointer.  bf16: bf16 rows, 1/||q||
+        of the rounded rows for cos_sim and no scales (None) for dot.  int8: quantized rows, cos_scale (cos_sim) or scale
+        (dot) of queries and documents."""
         _check_score_function(score_function)
         q = queries.to(self.device)
-        qb = q.contiguous() if q.dtype == torch.bfloat16 else to_bf16_rows(q.float())
         cos = score_function == "cos_sim"
+        if self.dtype == "int8":
+            q8, scale, cos_scale = quantize_rows_i8(q)
+            return q8, (cos_scale if cos else scale), (self.cos_scales if cos else self.scales).data_ptr()
+        qb = q.contiguous() if q.dtype == torch.bfloat16 else to_bf16_rows(q.float())
         q_scale = row_inv_norms(qb) if cos else None
         return qb, q_scale, (self.inv_norms.data_ptr() if cos else None)
 
@@ -131,7 +204,7 @@ class CorpusShard:
         return self._ws
 
     def _prepare(self, queries: torch.Tensor, k: int, score_function: str):
-        """Queries -> bf16 rows + 1/||q|| (cos_sim) + a workspace large enough for this search."""
+        """Queries -> rows and scales (``_queries``) + a workspace large enough for this search."""
         qb, q_scale, c_scale = self._queries(queries, score_function)
         self._workspace(_lib.lib().sgpt_search_workspace_bytes(qb.shape[0], self.n, k))
         return qb, q_scale, c_scale
@@ -141,14 +214,15 @@ class CorpusShard:
 
         Returns (scores fp32 [Q,k] descending, global ids int64 [Q,k]); when the shard has fewer than k documents the
         tail is (-inf, -1).  Queries are rounded to bf16 (the tensor-core input type); their 1/||q|| is taken from the
-        rounded rows so the result equals cos_sim of the stored/rounded vectors evaluated in fp32.
+        rounded rows so the result equals cos_sim of the stored/rounded vectors evaluated in fp32.  On an int8 shard the
+        queries are quantized like the documents, and the scores are those of the dequantized vectors.
         """
         qb, q_scale, c_scale = self._prepare(queries, k, score_function)
         nq = qb.shape[0]
         out_s = torch.empty((nq, k), dtype=torch.float32, device=self.device)
         out_i = torch.empty((nq, k), dtype=torch.int64, device=self.device)
         with torch.cuda.device(self.device):
-            rc = _lib.lib().sgpt_search(qb.data_ptr(), self.vectors.data_ptr(), _lib.ptr(q_scale), c_scale, nq, self.n,
+            rc = self._fn("sgpt_search")(qb.data_ptr(), self.vectors.data_ptr(), _lib.ptr(q_scale), c_scale, nq, self.n,
                                         self.dim, k, self.id_base, out_s.data_ptr(), out_i.data_ptr(),
                                         self._ws.data_ptr(), self._ws.numel(), _lib.current_stream())
         _lib.check(rc, "sgpt_search")
@@ -162,31 +236,51 @@ class CorpusShard:
         nq = qb.shape[0]
         out = torch.empty((nq, k), dtype=torch.int64, device=self.device)
         with torch.cuda.device(self.device):
-            rc = _lib.lib().sgpt_search_packed(qb.data_ptr(), self.vectors.data_ptr(), _lib.ptr(q_scale), c_scale, nq,
+            rc = self._fn("sgpt_search_packed")(qb.data_ptr(), self.vectors.data_ptr(), _lib.ptr(q_scale), c_scale, nq,
                                                self.n, self.dim, k, self.id_base, out.data_ptr(), self._ws.data_ptr(),
                                                self._ws.numel(), _lib.current_stream())
         _lib.check(rc, "sgpt_search_packed")
         return out
 
+    def search_gather(self, gather_handle, queries: torch.Tensor, k: int, score_function: str = "cos_sim",
+                      exclude_ids: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``sgpt_search_gather`` on this shard (dist.PeerGather): local exact top-k, pushed to every rank of the gather
+        context `gather_handle` and merged there.  Returns the merged (scores fp32 [Q,k], ids int64 [Q,k])."""
+        qb, q_scale, c_scale = self._prepare(queries, k, score_function)
+        nq = qb.shape[0]
+        out_s = torch.empty((nq, k), dtype=torch.float32, device=self.device)
+        out_i = torch.empty((nq, k), dtype=torch.int64, device=self.device)
+        with torch.cuda.device(self.device):
+            rc = self._fn("sgpt_search_gather")(gather_handle, qb.data_ptr(), self.vectors.data_ptr(), _lib.ptr(q_scale),
+                                                c_scale, nq, self.n, self.dim, k, self.id_base, _lib.ptr(exclude_ids),
+                                                out_s.data_ptr(), out_i.data_ptr(), self._ws.data_ptr(), self._ws.numel(),
+                                                _lib.current_stream())
+        _lib.check(rc, "sgpt_search_gather")
+        return out_s, out_i
+
     def view(self, start: int, end: int) -> "CorpusShard":
         """Documents [start, end) of this shard as a shard of their own that shares the vectors; its ids are the
-        positions ``start ..`` inside this shard.  (The norms are copied: the kernels read them 16 bytes at a time.)"""
+        positions ``start ..`` inside this shard.  (The scales are copied: the kernels read them 16 bytes at a time.)"""
         v = object.__new__(CorpusShard)
-        v.dim, v.capacity, v.id_base, v.device = self.dim, end - start, int(start), self.device
+        v.dim, v.capacity, v.id_base, v.device, v.dtype = self.dim, end - start, int(start), self.device, self.dtype
         v.vectors = self.vectors[start:end]
-        v.inv_norms = self.inv_norms[start:end].clone()
+        if self.dtype == "int8":
+            v.scales = self.scales[start:end].clone()
+            v.cos_scales = self.cos_scales[start:end].clone()
+        else:
+            v.inv_norms = self.inv_norms[start:end].clone()
         v.n = end - start
         v._ws = None
         return v
 
     def _range_call(self, qb: torch.Tensor, q_scale: Optional[torch.Tensor], c_scale: Optional[int], threshold: float,
                     counts: torch.Tensor, cap: int, out_s: Optional[torch.Tensor], out_i: Optional[torch.Tensor]) -> None:
-        """One sgpt_range_search of the bf16 query rows qb (include/sgpt_b200.h): counts int64[Q] always, the entries of
-        the queries that fit into `cap` into out_s / out_i."""
+        """One sgpt_range_search of the query rows qb, in the shard's format (include/sgpt_b200.h): counts int64[Q]
+        always, the entries of the queries that fit into `cap` into out_s / out_i."""
         nq = qb.shape[0]
         ws = self._workspace(_lib.lib().sgpt_range_search_workspace_bytes(nq, self.n))
         with torch.cuda.device(self.device):
-            rc = _lib.lib().sgpt_range_search(qb.data_ptr(), self.vectors.data_ptr(), _lib.ptr(q_scale), c_scale, nq,
+            rc = self._fn("sgpt_range_search")(qb.data_ptr(), self.vectors.data_ptr(), _lib.ptr(q_scale), c_scale, nq,
                                               self.n, self.dim, float(threshold), self.id_base, counts.data_ptr(), cap,
                                               _lib.ptr(out_s), _lib.ptr(out_i), ws.data_ptr(), ws.numel(),
                                               _lib.current_stream())
@@ -222,7 +316,7 @@ class CorpusShard:
         """Every document whose score against a query is >= threshold, for fp32/bf16 queries [Q, D] (device).
 
         Returns (offsets int64 [Q+1], scores fp32 [E], global ids int64 [E]) on the device: query q's documents are
-        entries offsets[q] .. offsets[q+1], in ascending id order.  Queries are rounded to bf16 and scored exactly as in
+        entries offsets[q] .. offsets[q+1], in ascending id order.  Queries are converted and scored exactly as in
         ``search``; a NaN score counts as -1.  The output buffer starts at 64 entries per query and grows once, for the
         queries that did not fit."""
         qb, q_scale, c_scale = self._queries(queries, score_function)
