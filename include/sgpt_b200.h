@@ -376,6 +376,40 @@ int sgpt_search_gather_i8(sgpt_gather_t g, const void* Q, const void* C, const f
                           int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Filtered (masked) search: the same searches over the ALLOWED documents of a shard only (document deletion, per-tenant
+ * or per-query filters).  One entry point per operation; `dtype` selects the shard format (SGPT_DTYPE_BF16: the
+ * arguments of the bf16 entry point; SGPT_DTYPE_I8: those of its _i8 twin).  The unmasked entry points are these with a
+ * null mask, and the workspace sizes are the same.
+ *   Mask: uint32 words (device); bit j % 32 of word j / 32 set = local document j allowed.  mask_pitch_words = 0: one
+ *     bitmap [ceil(n/32)] shared by all queries; mask_pitch_words >= ceil(n/32): one bitmap per query, [nq][pitch].
+ *     mask == NULL (with pitch 0): every document allowed.  Bits at or past n are ignored.
+ *   Results: exactly those of the unmasked call computed over the allowed documents only — top-k in (score descending,
+ *     id ascending) order with the same tie rule, tail (-inf, -1) when fewer than k documents are allowed; range search
+ *     counts and returns allowed documents only, in ascending id order.  Masked documents never appear, also when every
+ *     document is masked.  With a NULL or all-ones mask every output is bit-identical to the unmasked entry point.
+ *   SGPT_ERR_INVALID, before any CUDA call, for an unknown dtype, a negative pitch, 0 < pitch < ceil(n/32) and a
+ *     non-zero pitch with a NULL mask, besides the rejections of the unmasked entry point.
+ * ------------------------------------------------------------------------------------------------------------------ */
+#define SGPT_DTYPE_BF16 0
+#define SGPT_DTYPE_I8 1
+int sgpt_search_masked(int dtype, const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq,
+                       int64_t n, int D, int k, int64_t id_base, const uint32_t* mask, int64_t mask_pitch_words,
+                       float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
+int sgpt_search_packed_masked(int dtype, const void* Q, const void* C, const float* q_scale, const float* c_scale,
+                              int nq, int64_t n, int D, int k, int64_t id_base, const uint32_t* mask,
+                              int64_t mask_pitch_words, uint64_t* out_packed, void* ws, int64_t ws_bytes,
+                              sgpt_stream_t stream);
+int sgpt_range_search_masked(int dtype, const void* Q, const void* C, const float* q_scale, const float* c_scale,
+                             int nq, int64_t n, int D, float threshold, int64_t id_base, const uint32_t* mask,
+                             int64_t mask_pitch_words, int64_t* out_counts, int64_t cap, float* out_scores,
+                             int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
+/* The mask applies to this rank's shard only (local document indices); the other ranks pass their own. */
+int sgpt_search_gather_masked(int dtype, sgpt_gather_t g, const void* Q, const void* C, const float* q_scale,
+                              const float* c_scale, int nq, int64_t n, int D, int k, int64_t id_base,
+                              const uint32_t* mask, int64_t mask_pitch_words, const int64_t* exclude_ids,
+                              float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Residual stream in bf16 (SGPT_RESID_BF16=1 when the model handle is created; default fp32).  HF keeps hidden_states in
  * the model dtype, i.e. bf16 for the reference's bf16 configs (BASELINE configs 3-5); the `_ex` entry points take the
  * residual stream as `const void*` + a flag.  sgpt_linear(..., SGPT_EPI_RESID_BF16) adds into it with a bf16 TMA reduce.

@@ -101,7 +101,14 @@ _SIGNATURES = {
     "sgpt_search_packed_i8": (i32, [vp, vp, vp, vp, i32, i64, i32, i32, i64, vp, vp, i64, vp]),
     "sgpt_range_search_i8": (i32, [vp, vp, vp, vp, i32, i64, i32, f32, i64, vp, i64, vp, vp, vp, i64, vp]),
     "sgpt_search_gather_i8": (i32, [vp, vp, vp, vp, vp, i32, i64, i32, i32, i64, vp, vp, vp, vp, i64, vp]),
+    "sgpt_search_masked": (i32, [i32, vp, vp, vp, vp, i32, i64, i32, i32, i64, vp, i64, vp, vp, vp, i64, vp]),
+    "sgpt_search_packed_masked": (i32, [i32, vp, vp, vp, vp, i32, i64, i32, i32, i64, vp, i64, vp, vp, i64, vp]),
+    "sgpt_range_search_masked": (i32, [i32, vp, vp, vp, vp, i32, i64, i32, f32, i64, vp, i64, vp, i64, vp, vp, vp, i64,
+                                       vp]),
+    "sgpt_search_gather_masked": (i32, [i32, vp, vp, vp, vp, vp, i32, i64, i32, i32, i64, vp, i64, vp, vp, vp, vp, i64,
+                                        vp]),
 }
+DTYPE_BF16, DTYPE_I8 = 0, 1
 
 ABI_VERSION = 3  # include/sgpt_b200.h SGPT_ABI_VERSION these signatures / struct layouts were written for
 IPC_HANDLE_BYTES = 64

@@ -89,21 +89,40 @@ FilterGeometry filter_geometry(long long tiles, int nq) {
 
 // nq <= 128: one CTA per work unit (M = 128).  128 < nq <= 256: two CTAs per work unit, each with 128 of the queries and
 // the same corpus tile — the second read of the tile is an L2 hit, so one pass over the shard from HBM serves 256 queries.
-template <class P>
-static int launch_filter_gemm(const void* Q, const void* C, int nq, int n, int D, const P& p, cudaStream_t stream, TileMap tm,
-                              bool s8) {
+template <class Epi>
+static int launch_filter_gemm(const void* Q, const void* C, int nq, int n, int D, const typename Epi::Params& p,
+                              cudaStream_t stream, TileMap tm, bool s8) {
   if (s8) {
-    if (nq > kGemmBM) return launch_gemm<kSimBN, EpiFilterRows, 2, true>(Q, D, C, D, nq, n, D, p, stream, kCatScores, tm);
-    return launch_gemm<kSimBN, EpiFilterRows, 1, true>(Q, D, C, D, nq, n, D, p, stream, kCatScores, tm);
+    if (nq > kGemmBM) return launch_gemm<kSimBN, Epi, 2, true>(Q, D, C, D, nq, n, D, p, stream, kCatScores, tm);
+    return launch_gemm<kSimBN, Epi, 1, true>(Q, D, C, D, nq, n, D, p, stream, kCatScores, tm);
   }
-  if (nq > kGemmBM) return launch_gemm<kSimBN, EpiFilterRows, 2>(Q, D, C, D, nq, n, D, p, stream, kCatScores, tm);
-  return launch_gemm<kSimBN, EpiFilterRows, 1>(Q, D, C, D, nq, n, D, p, stream, kCatScores, tm);
+  if (nq > kGemmBM) return launch_gemm<kSimBN, Epi, 2>(Q, D, C, D, nq, n, D, p, stream, kCatScores, tm);
+  return launch_gemm<kSimBN, Epi, 1>(Q, D, C, D, nq, n, D, p, stream, kCatScores, tm);
+}
+
+int check_doc_mask(const char* fn, long long n, DocMask mask) {
+  const long long words = (n + 31) / 32;
+  SGPT_REQUIRE(mask.pitch >= 0, "%s: negative mask pitch %lld", fn, mask.pitch);
+  SGPT_REQUIRE(mask.pitch == 0 || mask.bits != nullptr, "%s: mask pitch %lld without a mask", fn, mask.pitch);
+  SGPT_REQUIRE(mask.pitch == 0 || mask.pitch >= words, "%s: mask pitch %lld words is below ceil(n / 32) = %lld", fn,
+               mask.pitch, words);
+  return SGPT_OK;
+}
+
+// the masked epilogue only when a mask is given: unmasked searches run the unmasked instantiations
+static int launch_filter_any(const void* Q, const void* C, int nq, int n, int D, const EpiFilterRows::Params& p,
+                             DocMask mask, cudaStream_t stream, TileMap tm, bool s8) {
+  if (mask.bits == nullptr) return launch_filter_gemm<EpiFilterRows>(Q, C, nq, n, D, p, stream, tm, s8);
+  FilterRowsParams pm = p;
+  pm.mask = mask.bits;
+  pm.mask_pitch = mask.pitch;
+  return launch_filter_gemm<EpiFilterRowsMasked>(Q, C, nq, n, D, pm, stream, tm, s8);
 }
 
 int launch_filter_candidates(const void* Q, const void* C, const float* q_scale, const float* c_scale,
                              const float* tau, const float* tau_hi, uint2* cand, int* counts, int* counts_back,
                              long long stride_q, int L, int group0, int nq, int n, int D, int tile_mode, int tile_stride,
-                             bool s8, cudaStream_t stream) {
+                             DocMask mask, bool s8, cudaStream_t stream) {
   SGPT_REQUIRE(nq <= 2 * kGemmBM, "filter GEMM: at most %d queries per launch (got %d)", 2 * kGemmBM, nq);
   TileMap tm;
   tm.mode = tile_mode;
@@ -111,13 +130,14 @@ int launch_filter_candidates(const void* Q, const void* C, const float* q_scale,
   const FilterGeometry g = filter_geometry(tm.count((n + kSimBN - 1) / kSimBN), nq);
   SGPT_REQUIRE(L >= g.L && (L % 2) == 0 && (stride_q % 2) == 0, "filter GEMM: candidate lists too small (L=%d < %d)", L,
                g.L);
-  EpiFilterRows::Params p{q_scale, c_scale, tau, tau_hi, cand, counts, counts_back, stride_q, L, group0, nq, nullptr, 0, 0,
-                          nq > kGemmBM ? 1 : 0};
-  return launch_filter_gemm(Q, C, nq, n, D, p, stream, tm, s8);
+  FilterRowsParams p{q_scale, c_scale, tau, tau_hi, cand, counts, counts_back, stride_q, L, group0, nq, nullptr, 0, 0,
+                     nq > kGemmBM ? 1 : 0};
+  return launch_filter_any(Q, C, nq, n, D, p, mask, stream, tm, s8);
 }
 
 int launch_sample_maxima(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* pool,
-                         long long stride_p, int Lp, int nq, int n, int D, int tile_stride, bool s8, cudaStream_t stream) {
+                         long long stride_p, int Lp, int nq, int n, int D, int tile_stride, DocMask mask, bool s8,
+                         cudaStream_t stream) {
   SGPT_REQUIRE(nq <= 2 * kGemmBM, "sample GEMM: at most %d queries per launch (got %d)", 2 * kGemmBM, nq);
   TileMap tm;
   tm.mode = 1;
@@ -125,9 +145,23 @@ int launch_sample_maxima(const void* Q, const void* C, const float* q_scale, con
   const FilterGeometry g = filter_geometry(tm.count((n + kSimBN - 1) / kSimBN), nq);
   SGPT_REQUIRE(Lp >= g.L / 4 && (Lp % 8) == 0 && (stride_p % 8) == 0 && stride_p >= static_cast<long long>(g.groups) * Lp,
                "sample GEMM: maxima lists too small (Lp=%d < %d)", Lp, g.L / 4);
-  EpiFilterRows::Params p{q_scale, c_scale, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, 0, nq, pool, stride_p, Lp,
-                          nq > kGemmBM ? 1 : 0};
-  return launch_filter_gemm(Q, C, nq, n, D, p, stream, tm, s8);
+  FilterRowsParams p{q_scale, c_scale, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, 0, nq, pool, stride_p, Lp,
+                     nq > kGemmBM ? 1 : 0};
+  return launch_filter_any(Q, C, nq, n, D, p, mask, stream, tm, s8);
+}
+
+int launch_scores(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* scores, long long lds,
+                  int nq, int n, int D, DocMask mask, bool s8, cudaStream_t stream) {
+  if (nq == 0 || n == 0) return SGPT_OK;
+  if (mask.bits == nullptr) {
+    EpiScoresF32::Params p{scores, q_scale, c_scale, lds, nullptr, 0};
+    // lanes = queries (A operand), columns = corpus rows (B operand, streamed once from HBM)
+    if (s8) return launch_gemm<128, EpiScoresF32, 1, true>(Q, D, C, D, nq, n, D, p, stream, kCatScores);
+    return launch_gemm<128, EpiScoresF32>(Q, D, C, D, nq, n, D, p, stream, kCatScores);
+  }
+  EpiScoresF32Masked::Params p{scores, q_scale, c_scale, lds, mask.bits, mask.pitch};
+  if (s8) return launch_gemm<128, EpiScoresF32Masked, 1, true>(Q, D, C, D, nq, n, D, p, stream, kCatScores);
+  return launch_gemm<128, EpiScoresF32Masked>(Q, D, C, D, nq, n, D, p, stream, kCatScores);
 }
 
 }  // namespace sgpt
@@ -334,10 +368,7 @@ extern "C" int sgpt_scores(const void* Q, const void* C, const float* q_scale, c
                (long long)n, D);
   SGPT_REQUIRE(n < (1ll << 31), "sgpt_scores: shard too large for one launch (n=%lld)", (long long)n);
   SGPT_REQUIRE(lds >= n, "sgpt_scores: lds < n");
-  if (nq == 0 || n == 0) return SGPT_OK;
-  EpiScoresF32::Params p{scores, q_scale, c_scale, static_cast<long long>(lds)};
-  // lanes = queries (A operand), columns = corpus rows (B operand, streamed once from HBM)
-  return launch_gemm<128, EpiScoresF32>(Q, D, C, D, nq, static_cast<int>(n), D, p, stream, kCatScores);
+  return launch_scores(Q, C, q_scale, c_scale, scores, lds, nq, static_cast<int>(n), D, DocMask(), false, stream);
 }
 
 extern "C" int sgpt_scores_i8(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* scores,
@@ -349,7 +380,5 @@ extern "C" int sgpt_scores_i8(const void* Q, const void* C, const float* q_scale
   SGPT_REQUIRE(n < (1ll << 31), "sgpt_scores_i8: shard too large for one launch (n=%lld)", (long long)n);
   SGPT_REQUIRE(lds >= n, "sgpt_scores_i8: lds < n");
   SGPT_REQUIRE(nq == 0 || n == 0 || scores != nullptr, "sgpt_scores_i8: null output");
-  if (nq == 0 || n == 0) return SGPT_OK;
-  EpiScoresF32::Params p{scores, q_scale, c_scale, static_cast<long long>(lds)};
-  return launch_gemm<128, EpiScoresF32, 1, true>(Q, D, C, D, nq, static_cast<int>(n), D, p, stream, kCatScores);
+  return launch_scores(Q, C, q_scale, c_scale, scores, lds, nq, static_cast<int>(n), D, DocMask(), true, stream);
 }

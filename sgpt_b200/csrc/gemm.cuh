@@ -854,13 +854,27 @@ __device__ __forceinline__ float2 slab_read(uint32_t slab, int r, int lane) {
   return lds_v2(slab + r * 256u + ((lane ^ (r & 15)) << 3));
 }
 
+// Document mask of the masked searches (include/sgpt_b200.h): bit j % 32 of word j / 32 of a query's bitmap set = local
+// document j allowed; pitch 0 = one bitmap for every query, else query q's bitmap starts at word q * pitch.
+__device__ __forceinline__ const uint32_t* mask_row(const uint32_t* mask, long long pitch, int q) {
+  return mask + static_cast<long long>(q) * pitch;
+}
+
+// Bits of a masked score (a NaN with the sign bit): score_key maps them to the invalid key 0, so the selection kernels
+// (topk.cu) treat the document as absent, exactly like an empty slot.
+constexpr uint32_t kMaskedScoreBits = 0xffffffffu;
+
 // scores_f32[q, doc] = fixnan(acc * row_scale[q] * col_scale[doc])       (cos_sim / dot_score, NaN -> -1)
-struct OpScoresF32 {
+// kMasked: masked documents get kMaskedScoreBits instead (the dense plan of the masked search).
+template <bool kMasked>
+struct OpScoresF32T {
   struct Params {
     float* out;
     const float* row_scale;  // per query  (1/||q|| for cos_sim; null = 1)
     const float* col_scale;  // per doc    (1/||d|| for cos_sim; null = 1)
     long long ldc;
+    const uint32_t* mask;    // kMasked: document bitmaps
+    long long mask_pitch;    // kMasked: words between consecutive queries' bitmaps (0 = shared)
   };
   static __device__ __forceinline__ void rows(const Params& p, uint32_t slab, int m0, int rows, int col, int N,
                                               int lane) {
@@ -874,6 +888,16 @@ struct OpScoresF32 {
     float* dst = p.out + static_cast<size_t>(m0) * p.ldc + col;
     float my_rs = 1.f;  // lane r keeps row m0 + r's scale; broadcast per row with a shuffle
     if (p.row_scale && lane < rows) my_rs = __ldg(p.row_scale + m0 + lane);
+    // (col is even: both columns of the lane sit in one mask word)
+    const uint32_t shared_word = (kMasked && p.mask_pitch == 0 && ok0) ? __ldg(p.mask + (col >> 5)) : 0u;
+    auto masked = [&](int row, float& x, float& y) {
+      if constexpr (kMasked) {
+        const uint32_t w = p.mask_pitch == 0 ? shared_word
+                                             : (ok0 ? __ldg(mask_row(p.mask, p.mask_pitch, row) + (col >> 5)) : 0u);
+        if (!((w >> (col & 31)) & 1u)) x = __uint_as_float(kMaskedScoreBits);
+        if (!((w >> ((col + 1) & 31)) & 1u)) y = __uint_as_float(kMaskedScoreBits);
+      }
+    };
     int r = 0;
     for (; r + 8 <= rows; r += 8) {
       float2 a[8];
@@ -885,6 +909,7 @@ struct OpScoresF32 {
         float x = a[u].x * rs * c0, y = a[u].y * rs * c1;
         x = (x != x) ? -1.f : x;
         y = (y != y) ? -1.f : y;
+        masked(m0 + r + u, x, y);
         if (vec) *reinterpret_cast<float2*>(dst) = make_float2(x, y);
         else {
           if (ok0) dst[0] = x;
@@ -899,6 +924,7 @@ struct OpScoresF32 {
       float x = a.x * rs * c0, y = a.y * rs * c1;
       x = (x != x) ? -1.f : x;
       y = (y != y) ? -1.f : y;
+      masked(m0 + r, x, y);
       if (vec) *reinterpret_cast<float2*>(dst) = make_float2(x, y);
       else {
         if (ok0) dst[0] = x;
@@ -927,25 +953,37 @@ struct OpScoresF32 {
 // score of a distinct real document, so the k-th largest of a query's maxima is a valid lower bound of its final k-th
 // best score — at a quarter of the entries (and no document indices) the full sample would need.  Slots this thread never
 // fills are written as 0xffffffff (maps to the invalid key 0 of the selection kernels).
-struct EpiFilterRows {
-  struct Params {
-    const float* row_scale;  // [M] or null
-    const float* col_scale;  // [N] or null
-    const float* tau;        // [M] per-query admission threshold; null -> admit everything
-    const float* tau_hi;     // [M] upper threshold (>= tau) or null: scores >= tau_hi are appended at the FRONT of the list,
-                             // scores in [tau, tau_hi) at its BACK (filled downwards from slot L - 1); null -> all front
-    uint2* cand;             // [M][groups][L]
-    int* counts;             // [groups][M] front entries
-    int* counts_back;        // [groups][M] back entries (only with tau_hi)
-    long long stride_q;      // entries between consecutive queries' list blocks
-    int L;                   // entries per (query, group) list
-    int group0;              // first group index this launch writes
-    int nq;
-    float* pool;             // sample mode: [M][groups][Lp] block maxima (cand / counts / tau unused)
-    long long stride_p;      // floats between consecutive queries' blocks of `pool`
-    int Lp;                  // floats per (query, group): 32 x tiles per CTA
-    int pair;                // 1: launched with two CTAs per work unit (CL = 2: 256 queries per scan)
-  };
+//
+// kMasked (the masked searches): only documents whose bit is set in the query's bitmap (Params::mask) are admitted, and
+// a sample maximum is taken over those documents only; a 4-document block without any is an unused slot (0xffffffff),
+// so every valid maximum is still the score of a distinct ALLOWED document and tau stays a lower bound of the k-th best
+// allowed score (-inf, i.e. admit every allowed document, when the sample holds fewer than k maxima).  The four mask
+// words of the warp's half tile are fetched in pre_tile with the document scales.  The unmasked instantiation compiles
+// to the code it had before the mask existed.
+struct FilterRowsParams {
+  const float* row_scale;  // [M] or null
+  const float* col_scale;  // [N] or null
+  const float* tau;        // [M] per-query admission threshold; null -> admit everything
+  const float* tau_hi;     // [M] upper threshold (>= tau) or null: scores >= tau_hi are appended at the FRONT of the list,
+                           // scores in [tau, tau_hi) at its BACK (filled downwards from slot L - 1); null -> all front
+  uint2* cand;             // [M][groups][L]
+  int* counts;             // [groups][M] front entries
+  int* counts_back;        // [groups][M] back entries (only with tau_hi)
+  long long stride_q;      // entries between consecutive queries' list blocks
+  int L;                   // entries per (query, group) list
+  int group0;              // first group index this launch writes
+  int nq;
+  float* pool;             // sample mode: [M][groups][Lp] block maxima (cand / counts / tau unused)
+  long long stride_p;      // floats between consecutive queries' blocks of `pool`
+  int Lp;                  // floats per (query, group): 32 x tiles per CTA
+  int pair;                // 1: launched with two CTAs per work unit (CL = 2: 256 queries per scan)
+  const uint32_t* mask;    // kMasked: document bitmaps of the launch's queries
+  long long mask_pitch;    // kMasked: words between consecutive queries' bitmaps (0 = one bitmap for all)
+};
+
+template <bool kMasked>
+struct EpiFilterRowsT {
+  using Params = FilterRowsParams;
   struct State {
     int cnt;    // front entries (sample mode: maxima written)
     int cnt_b;  // back entries
@@ -957,6 +995,11 @@ struct EpiFilterRows {
     float4 cs;
     float rs, tau, tau_hi;
   };
+  // kMasked: this query's mask words of documents n0 .. n0 + 127 (words past the shard's last document are never read:
+  // bits at or past N are ignored)
+  static __device__ __forceinline__ const uint32_t* mask_words(const Params& p, int q, int n0) {
+    return mask_row(p.mask, p.mask_pitch, q) + (n0 >> 5);
+  }
   static constexpr int kEpiWarps = 8;
   static constexpr int kStagingBytes = 1024;  // (none used)
   // one group per (work-unit slot, column half): with two CTAs per unit (Params::pair = 1: up to 256 queries per scan, CTA r
@@ -986,6 +1029,16 @@ struct EpiFilterRows {
         st.cs.w = __ldg(p.col_scale + min(c + 3, N - 1));
       }
     }
+    if constexpr (kMasked) {
+      // Only an L1 prefetch here: four words held in registers across the mainloop would push the 168-register kernel
+      // into spills.  tile() loads them from L1 (the 16 bytes may straddle two lines when the pitch is not a multiple of 4)
+      if (qok && n0 < N) {
+        const uint32_t* w = mask_words(p, q, n0);
+        const int last = min(3, (N - 1 - n0) >> 5);
+        asm volatile("prefetch.global.L1 [%0];" ::"l"(w));
+        asm volatile("prefetch.global.L1 [%0];" ::"l"(w + last));
+      }
+    }
   }
   static __device__ __forceinline__ void finish(State& st, const Params& p, int lane_row) {
     if (lane_row >= p.nq) return;
@@ -1012,6 +1065,12 @@ struct EpiFilterRows {
     const float csv[4] = {st.cs.x, st.cs.y, st.cs.z, st.cs.w};
     uint2* dst = p.cand + static_cast<long long>(qok ? q : 0) * p.stride_q + static_cast<long long>(group_of(p)) * p.L;
     int cnt = st.cnt, cnt_b = st.cnt_b;
+    uint32_t mw[4] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu};  // bit i of mw[j]: document n0 + 32 j + i allowed
+    if constexpr (kMasked) {
+      const uint32_t* w = mask_words(p, qok ? q : 0, n0);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) mw[j] = (qok && n0 + 32 * j < N) ? __ldg(w + j) : 0u;
+    }
 #pragma unroll 1
     for (int c = 0; c < COLS; c += 32) {
       const int n = n0 + c;
@@ -1019,6 +1078,8 @@ struct EpiFilterRows {
       uint32_t v[32];
       acc_ld_32(trow + 4 * c, v);
       const bool full = (n + 32 <= N);
+      // bit i: document n + i may be admitted (selects instead of mw[c >> 5]: a dynamic index would put mw in local memory)
+      const uint32_t allow = c == 0 ? mw[0] : c == 32 ? mw[1] : c == 64 ? mw[2] : mw[3];
       // scale of column c + i: component i % 4 of lane (c + i) / 4 (all lanes take part: the loop is warp-uniform)
       float cs[32];
 #pragma unroll
@@ -1044,8 +1105,14 @@ struct EpiFilterRows {
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           float mx = -INFINITY;
+          bool any = false;
 #pragma unroll
-          for (int u = 0; u < 4; ++u) mx = (full || n + 4 * j + u < N) ? fmaxf(mx, x[4 * j + u]) : mx;
+          for (int u = 0; u < 4; ++u) {
+            const bool ok = (full || n + 4 * j + u < N) && (!kMasked || ((allow >> (4 * j + u)) & 1u));
+            mx = ok ? fmaxf(mx, x[4 * j + u]) : mx;
+            any = any || ok;
+          }
+          if constexpr (kMasked) mx = any ? mx : __uint_as_float(kMaskedScoreBits);  // no allowed document: unused slot
           m[j] = mx;
         }
         if (qok && cnt + 8 <= p.Lp) {
@@ -1062,7 +1129,8 @@ struct EpiFilterRows {
         // score of every tile this CTA visits (checked by the launcher).
 #pragma unroll
         for (int i = 0; i < 32; ++i) {
-          const bool pass = (full || n + i < N) && x[i] >= tau;  // tau = +inf for rows beyond the query count
+          // tau = +inf for rows beyond the query count
+          const bool pass = (full || n + i < N) && x[i] >= tau && (!kMasked || ((allow >> i) & 1u));
           const bool hi = x[i] >= tau_hi;
           const uint32_t slot = static_cast<uint32_t>(hi ? cnt : (p.L - 1 - cnt_b));  // unsigned: one IMAD.WIDE.U32 per address
           // (a predicated store in PTX: as plain C++ the compiler wraps the store and its address arithmetic in a branch)
@@ -1080,7 +1148,8 @@ struct EpiFilterRows {
     st.cnt_b = cnt_b;
   }
 };
-using EpiFilterCandidates = EpiFilterRows;
+using EpiFilterRows = EpiFilterRowsT<false>;
+using EpiFilterRowsMasked = EpiFilterRowsT<true>;
 
 
 template <bool kGelu>
@@ -1117,6 +1186,7 @@ struct EpiDebugNull {
     }
   }
 };
-using EpiScoresF32 = EpiStaged<OpScoresF32>;
+using EpiScoresF32 = EpiStaged<OpScoresF32T<false>>;
+using EpiScoresF32Masked = EpiStaged<OpScoresF32T<true>>;
 
 }  // namespace sgpt

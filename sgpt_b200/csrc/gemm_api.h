@@ -17,20 +17,37 @@ struct FilterGeometry {
 };
 FilterGeometry filter_geometry(long long tiles, int nq);
 
+// Document mask of a launch's queries (include/sgpt_b200.h, masked searches): bits == nullptr = every document allowed;
+// otherwise query q of the launch reads the bitmap at bits + q * pitch (pitch 0: one bitmap shared by all queries).
+struct DocMask {
+  const uint32_t* bits = nullptr;
+  long long pitch = 0;
+};
+// SGPT_OK, or SGPT_ERR_INVALID with the message set for a negative pitch, 0 < pitch < ceil(n / 32) or a pitch without a
+// bitmap (no CUDA call)
+int check_doc_mask(const char* fn, long long n, DocMask mask);
+
 // Similarity GEMM whose epilogue appends every score >= tau[q] (tau == nullptr: every score) as (score bits, local doc
 // index) to the list cand[q * stride_q + (group0 + g) * L + ...] — scores >= tau_hi[q] at its front, the others at its
 // back (tau_hi == nullptr: all at the front) — and writes counts / counts_back[(group0 + g) * nq + q] for the groups g of
 // this launch (filter_geometry of the visited tile count).  tile_mode/tile_stride select the corpus tiles visited
 // (gemm.cuh TileMap).  nq <= 256 (above 128: CTA pairs, M = 256).  s8: Q and C are int8 rows (gemm.cuh kS8), else bf16.
+// Documents the mask excludes are never admitted.
 int launch_filter_candidates(const void* Q, const void* C, const float* q_scale, const float* c_scale,
                              const float* tau, const float* tau_hi, uint2* cand, int* counts, int* counts_back,
                              long long stride_q, int L, int group0, int nq, int n, int D, int tile_mode, int tile_stride,
-                             bool s8, cudaStream_t stream);
+                             DocMask mask, bool s8, cudaStream_t stream);
 
 // The same GEMM over every tile_stride-th corpus tile in sample mode: pool[q * stride_p + g * Lp + ...] receives the
-// maximum score of every 4 consecutive documents the group visited (filter_geometry(sampled tiles).L / 4 floats per list,
-// unused slots = 0xffffffff).  Input of launch_tau_select (topk.cuh).
+// maximum score of every 4 consecutive (allowed) documents the group visited (filter_geometry(sampled tiles).L / 4 floats
+// per list, unused slots = 0xffffffff).  Input of launch_tau_select (topk.cuh).
 int launch_sample_maxima(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* pool,
-                         long long stride_p, int Lp, int nq, int n, int D, int tile_stride, bool s8, cudaStream_t stream);
+                         long long stride_p, int Lp, int nq, int n, int D, int tile_stride, DocMask mask, bool s8,
+                         cudaStream_t stream);
+
+// Dense scores [nq, lds] (sgpt_scores / sgpt_scores_i8); with a mask, masked documents get score bits 0xffffffff, which
+// the selection kernels treat as absent (topk.cu score_key: invalid key 0).
+int launch_scores(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* scores, long long lds,
+                  int nq, int n, int D, DocMask mask, bool s8, cudaStream_t stream);
 
 }  // namespace sgpt

@@ -378,7 +378,7 @@ __global__ void __launch_bounds__(kTopkThreads, 1) topk_select_kernel(TopkSrc sr
     uint32_t local = 0;
     if (cached) {
       for (uint32_t j = tid; j < flat_total; j += kTopkThreads) local += (ckeys[j] != 0);
-    } else if (src.ids == nullptr && src.packed == nullptr) {
+    } else if (src.ids == nullptr && src.packed == nullptr && !src.dense_masked) {
       for (int g = tid; g < nl; g += kTopkThreads) local += static_cast<uint32_t>(list_len(src, q, g));
     } else {
       for_each_elem<false>(src, nl, q, tid, s_off, s_len, [&](int g, long long i, bool) { local += (load_elem(src, q, g, i).key != 0); });

@@ -27,6 +27,9 @@ struct TopkSrc {
   // per-query switch (two-pass search): the selection kernel returns at once for queries with run_flag[q] == 0 — they were
   // answered by the front-list kernel (launch_front_select) launched just before it
   const int* run_flag = nullptr;
+  // dense rows that may hold masked entries (score bits 0xffffffff, the invalid key: the masked search's dense plan):
+  // the valid elements must be counted instead of taken to be every column
+  int dense_masked = 0;
   long long id_base = 0;
   int G = 1;                         // lists per query
   int nq = 0;

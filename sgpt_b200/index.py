@@ -7,6 +7,11 @@ HBM speed) plus fp32 1/||row|| of the STORED rows, so cosine scores are exactly 
 An int8 shard (``dtype="int8"``) holds int8 rows [n, D] with a per-row scale and cos-scale instead: half the bytes per
 document, so twice the documents per GPU and half the HBM traffic per search.  Queries are quantized the same way, and
 scores are those of the dequantized vectors (include/sgpt_b200.h, int8 corpus shards).
+
+Every search takes an optional document filter ``allow=`` (a boolean device tensor [n] shared by all queries, or [Q, n]
+with one row per query), and ``CorpusShard.remove`` deletes documents from a built shard.  Both become one document
+bitmap per search (``pack_mask``; include/sgpt_b200.h, masked searches): the result is exactly the search over the
+allowed, undeleted documents.
 """
 from __future__ import annotations
 
@@ -74,6 +79,35 @@ def row_inv_norms(x_bf16: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def pack_mask(allow: torch.Tensor) -> torch.Tensor:
+    """Boolean [..., n] -> the library's document bitmap, int32 [..., ceil(n / 32)] (the bits of uint32 words): bit
+    j % 32 of word j // 32 is allow[..., j]; the bits past n are 0."""
+    n = allow.shape[-1]
+    words = (n + 31) // 32
+    bits = torch.zeros((*allow.shape[:-1], words * 32), dtype=torch.int64, device=allow.device)
+    bits[..., :n] = allow.to(torch.bool)
+    w = (bits.view(*allow.shape[:-1], words, 32) << torch.arange(32, device=allow.device)).sum(-1)
+    return torch.where(w >= 2 ** 31, w - 2 ** 32, w).to(torch.int32)
+
+
+def unpack_mask(words: torch.Tensor, n: int) -> torch.Tensor:
+    """Inverse of ``pack_mask``: int32 [..., W] -> boolean [..., n] (n <= 32 W)."""
+    w = words.to(torch.int64) & 0xFFFFFFFF
+    bits = (w.unsqueeze(-1) >> torch.arange(32, device=words.device)) & 1
+    return bits.reshape(*words.shape[:-1], -1)[..., :n].to(torch.bool)
+
+
+def _bit_slice(words: torch.Tensor, start: int, n: int) -> torch.Tensor:
+    """Bits [start, start + n) of a bitmap (int32 words, at least one word beyond the last one read) as a bitmap of
+    their own (bit 0 = bit `start`); the bits past n are whatever follows in `words`."""
+    w0, r, nw = start // 32, start % 32, (n + 31) // 32
+    if r == 0:
+        return words[w0:w0 + nw]
+    w = words[w0:w0 + nw + 1].to(torch.int64) & 0xFFFFFFFF
+    s = ((w[:-1] >> r) | (w[1:] << (32 - r))) & 0xFFFFFFFF
+    return torch.where(s >= 2 ** 31, s - 2 ** 32, s).to(torch.int32)
+
+
 def _check_dtype(dtype: str, dim: int) -> None:
     if dtype not in SHARD_DTYPES:
         raise ValueError(f"shard dtype {dtype!r} must be one of {SHARD_DTYPES}")
@@ -87,7 +121,11 @@ class CorpusShard:
     """Documents [id_base, id_base + n) of a corpus, resident in the HBM of one GPU.
 
     ``dtype="bf16"``: ``vectors`` bf16 [capacity, D] and ``inv_norms`` fp32.  ``dtype="int8"``: ``vectors`` int8
-    [capacity, D], ``scales`` and ``cos_scales`` fp32 (include/sgpt_b200.h, int8 corpus shards)."""
+    [capacity, D], ``scales`` and ``cos_scales`` fp32 (include/sgpt_b200.h, int8 corpus shards).
+
+    Deleted documents (``remove``) are bits of a device bitmap int32 [capacity / 32 + 1] that the shard and its views
+    share (``_deleted``: the words and whether any bit was ever set; ``_deleted_at``: the bit of this shard's row 0).
+    Every search leaves them out; ids never change."""
 
     def __init__(self, dim: int, capacity: int, device="cuda:0", id_base: int = 0, dtype: str = "bf16"):
         _check_dtype(dtype, dim)
@@ -102,6 +140,9 @@ class CorpusShard:
             self.inv_norms = torch.empty(self.capacity, dtype=torch.float32, device=self.device)
         self.n = 0
         self._ws: Optional[torch.Tensor] = None
+        self._deleted = {"words": torch.zeros(self.capacity // 32 + 2, dtype=torch.int32, device=self.device),
+                         "any": False}
+        self._deleted_at = 0
 
     @classmethod
     def from_embeddings(cls, emb: torch.Tensor, device=None, id_base: int = 0, dtype: str = "bf16") -> "CorpusShard":
@@ -144,9 +185,13 @@ class CorpusShard:
         else:
             np.save(os.path.join(path, "vectors.npy"), self.stored().view(torch.int16).cpu().numpy().view(np.uint16))
             np.save(os.path.join(path, "inv_norms.npy"), self.inv_norms[:self.n].cpu().numpy())
+        # deleted.npy: uint32 [ceil(n / 32)], bit j % 32 of word j // 32 set = document j deleted
+        deleted = _bit_slice(self._deleted["words"], self._deleted_at, self.n) & pack_mask(
+            torch.ones(self.n, dtype=torch.bool, device=self.device))
+        np.save(os.path.join(path, "deleted.npy"), deleted.cpu().numpy().view(np.uint32))
         with open(os.path.join(path, "meta.json"), "w") as f:
             json.dump({"format": "sgpt_b200.CorpusShard/1", "dtype": self.dtype, "dim": self.dim, "n": self.n,
-                       "id_base": self.id_base}, f)
+                       "id_base": self.id_base, "deleted": "deleted.npy"}, f)
 
     @classmethod
     def load(cls, path: str, device="cuda:0", capacity: Optional[int] = None) -> "CorpusShard":
@@ -169,6 +214,12 @@ class CorpusShard:
             inv = np.load(os.path.join(path, "inv_norms.npy"))
             if vec.shape != (n, dim) or vec.dtype != np.uint16 or inv.shape != (n,):
                 raise ValueError(f"{path}: array shapes {vec.shape}/{inv.shape} do not match meta {meta}")
+        deleted = None
+        if meta.get("deleted") is not None:  # directories written before deletions existed have none
+            deleted = np.load(os.path.join(path, meta["deleted"]))
+            if deleted.shape != ((n + 31) // 32,) or deleted.dtype != np.uint32:
+                raise ValueError(f"{path}: deletion bitmap {deleted.shape}/{deleted.dtype} does not match meta {meta} "
+                                 f"(expected uint32 [{(n + 31) // 32}])")
         shard = cls(dim, max(n, capacity or n), device=device, id_base=int(meta["id_base"]), dtype=dtype)
         if dtype == "int8":
             shard.vectors[:n].copy_(torch.from_numpy(np.array(vec)))
@@ -178,11 +229,56 @@ class CorpusShard:
             shard.vectors[:n].copy_(torch.from_numpy(np.array(vec).view(np.int16)).view(torch.bfloat16))
             shard.inv_norms[:n].copy_(torch.from_numpy(inv))
         shard.n = n
+        if deleted is not None and deleted.any():
+            # (bits past n are dropped: rows added later start undeleted)
+            words = torch.from_numpy(deleted.view(np.int32).copy()).to(shard.device)
+            shard._deleted["words"][:len(deleted)].copy_(words & pack_mask(torch.ones(n, dtype=torch.bool,
+                                                                                      device=shard.device)))
+            shard._deleted["any"] = True
         return shard
 
-    def _fn(self, name: str):
-        """The library entry point `name` for this shard's format (the `_i8` variant on an int8 shard)."""
-        return getattr(_lib.lib(), name + "_i8" if self.dtype == "int8" else name)
+    # ---- deletions -------------------------------------------------------------------------------------------------
+    def remove(self, ids) -> None:
+        """Delete documents by global id (id_base .. id_base + n - 1): no search, range search or gather returns them
+        afterwards.  Ids never change (there is no compaction); deleting a document twice is allowed.  A view shares
+        the deletions of the shard it was taken from."""
+        ids = torch.as_tensor(ids, dtype=torch.int64).to(self.device).reshape(-1)
+        if ids.numel() == 0:
+            return
+        local = ids - self.id_base
+        if bool(((local < 0) | (local >= self.n)).any()):
+            raise ValueError(f"remove: ids must lie in [{self.id_base}, {self.id_base + self.n})")
+        words = self._deleted["words"]
+        bits = unpack_mask(words, words.numel() * 32)
+        bits[local + self._deleted_at] = True
+        words.copy_(pack_mask(bits))
+        self._deleted["any"] = True
+
+    @property
+    def n_deleted(self) -> int:
+        """Number of deleted documents among this shard's n."""
+        if not self._deleted["any"] or self.n == 0:
+            return 0
+        return int(unpack_mask(_bit_slice(self._deleted["words"], self._deleted_at, self.n), self.n).sum())
+
+    def _mask(self, allow: Optional[torch.Tensor], nq: int) -> Tuple[Optional[torch.Tensor], int]:
+        """(bitmap, pitch in words) of a search of nq queries: `allow` (bool [n] or [nq, n], or None) without the deleted
+        documents; (None, 0) when every document is allowed."""
+        deleted = _bit_slice(self._deleted["words"], self._deleted_at, self.n) if self._deleted["any"] else None
+        if allow is None:
+            return (None, 0) if deleted is None else (torch.bitwise_not(deleted).contiguous(), 0)
+        allow = torch.as_tensor(allow, device=self.device)
+        if allow.dtype != torch.bool or allow.shape not in ((self.n,), (nq, self.n)):
+            raise ValueError(f"allow must be a boolean tensor [{self.n}] or [{nq}, {self.n}], got {allow.dtype} "
+                             f"{tuple(allow.shape)}")
+        m = pack_mask(allow)
+        if deleted is not None:
+            m = m & torch.bitwise_not(deleted)
+        return m.contiguous(), (m.shape[1] if m.dim() == 2 and self.n > 0 else 0)
+
+    def _dtype_id(self) -> int:
+        """The `dtype` argument of the masked entry points for this shard's format."""
+        return _lib.DTYPE_I8 if self.dtype == "int8" else _lib.DTYPE_BF16
 
     def _queries(self, queries: torch.Tensor, score_function: str):
         """Queries -> rows in the shard's format + their scales + the shard's scale pointer.  bf16: bf16 rows, 1/||q||
@@ -209,58 +305,73 @@ class CorpusShard:
         self._workspace(_lib.lib().sgpt_search_workspace_bytes(qb.shape[0], self.n, k))
         return qb, q_scale, c_scale
 
-    def search(self, queries: torch.Tensor, k: int, score_function: str = "cos_sim") -> Tuple[torch.Tensor, torch.Tensor]:
+    def search(self, queries: torch.Tensor, k: int, score_function: str = "cos_sim",
+               allow: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
         """Exact top-k of this shard for fp32/bf16 queries [Q, D] (device).
 
         Returns (scores fp32 [Q,k] descending, global ids int64 [Q,k]); when the shard has fewer than k documents the
         tail is (-inf, -1).  Queries are rounded to bf16 (the tensor-core input type); their 1/||q|| is taken from the
         rounded rows so the result equals cos_sim of the stored/rounded vectors evaluated in fp32.  On an int8 shard the
         queries are quantized like the documents, and the scores are those of the dequantized vectors.
+
+        ``allow``: boolean device tensor [n] (all queries) or [Q, n] (one row per query) of the documents that may be
+        returned; deleted documents (``remove``) never are.  The result is exactly the search over those documents, with
+        the tail (-inf, -1) when fewer than k are allowed.
         """
         qb, q_scale, c_scale = self._prepare(queries, k, score_function)
         nq = qb.shape[0]
+        mask, pitch = self._mask(allow, nq)
         out_s = torch.empty((nq, k), dtype=torch.float32, device=self.device)
         out_i = torch.empty((nq, k), dtype=torch.int64, device=self.device)
         with torch.cuda.device(self.device):
-            rc = self._fn("sgpt_search")(qb.data_ptr(), self.vectors.data_ptr(), _lib.ptr(q_scale), c_scale, nq, self.n,
-                                        self.dim, k, self.id_base, out_s.data_ptr(), out_i.data_ptr(),
-                                        self._ws.data_ptr(), self._ws.numel(), _lib.current_stream())
+            rc = _lib.lib().sgpt_search_masked(self._dtype_id(), qb.data_ptr(), self.vectors.data_ptr(),
+                                               _lib.ptr(q_scale), c_scale, nq, self.n, self.dim, k, self.id_base,
+                                               _lib.ptr(mask), pitch, out_s.data_ptr(), out_i.data_ptr(),
+                                               self._ws.data_ptr(), self._ws.numel(), _lib.current_stream())
         _lib.check(rc, "sgpt_search")
         return out_s, out_i
 
-    def search_packed(self, queries: torch.Tensor, k: int, score_function: str = "cos_sim") -> torch.Tensor:
+    def search_packed(self, queries: torch.Tensor, k: int, score_function: str = "cos_sim",
+                      allow: Optional[torch.Tensor] = None) -> torch.Tensor:
         """The same search with the result as ONE tensor of packed 8-byte entries, int64 [Q,k] whose low 32 bits are the
         fp32 score and high 32 bits the int32 global id (-inf / -1 = empty): what a rank contributes to the single
-        all-gather of a sharded search (SURVEY.md §8e).  Needs id_base + n < 2^31."""
+        all-gather of a sharded search (SURVEY.md §8e).  Needs id_base + n < 2^31.  ``allow`` as in ``search``."""
         qb, q_scale, c_scale = self._prepare(queries, k, score_function)
         nq = qb.shape[0]
+        mask, pitch = self._mask(allow, nq)
         out = torch.empty((nq, k), dtype=torch.int64, device=self.device)
         with torch.cuda.device(self.device):
-            rc = self._fn("sgpt_search_packed")(qb.data_ptr(), self.vectors.data_ptr(), _lib.ptr(q_scale), c_scale, nq,
-                                               self.n, self.dim, k, self.id_base, out.data_ptr(), self._ws.data_ptr(),
-                                               self._ws.numel(), _lib.current_stream())
+            rc = _lib.lib().sgpt_search_packed_masked(self._dtype_id(), qb.data_ptr(), self.vectors.data_ptr(),
+                                                      _lib.ptr(q_scale), c_scale, nq, self.n, self.dim, k, self.id_base,
+                                                      _lib.ptr(mask), pitch, out.data_ptr(), self._ws.data_ptr(),
+                                                      self._ws.numel(), _lib.current_stream())
         _lib.check(rc, "sgpt_search_packed")
         return out
 
     def search_gather(self, gather_handle, queries: torch.Tensor, k: int, score_function: str = "cos_sim",
-                      exclude_ids: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+                      exclude_ids: Optional[torch.Tensor] = None, allow: Optional[torch.Tensor] = None
+                      ) -> Tuple[torch.Tensor, torch.Tensor]:
         """``sgpt_search_gather`` on this shard (dist.PeerGather): local exact top-k, pushed to every rank of the gather
-        context `gather_handle` and merged there.  Returns the merged (scores fp32 [Q,k], ids int64 [Q,k])."""
+        context `gather_handle` and merged there.  Returns the merged (scores fp32 [Q,k], ids int64 [Q,k]).  ``allow``
+        (as in ``search``) and the deletions filter this rank's documents; every rank passes its own."""
         qb, q_scale, c_scale = self._prepare(queries, k, score_function)
         nq = qb.shape[0]
+        mask, pitch = self._mask(allow, nq)
         out_s = torch.empty((nq, k), dtype=torch.float32, device=self.device)
         out_i = torch.empty((nq, k), dtype=torch.int64, device=self.device)
         with torch.cuda.device(self.device):
-            rc = self._fn("sgpt_search_gather")(gather_handle, qb.data_ptr(), self.vectors.data_ptr(), _lib.ptr(q_scale),
-                                                c_scale, nq, self.n, self.dim, k, self.id_base, _lib.ptr(exclude_ids),
-                                                out_s.data_ptr(), out_i.data_ptr(), self._ws.data_ptr(), self._ws.numel(),
-                                                _lib.current_stream())
+            rc = _lib.lib().sgpt_search_gather_masked(self._dtype_id(), gather_handle, qb.data_ptr(),
+                                                      self.vectors.data_ptr(), _lib.ptr(q_scale), c_scale, nq, self.n,
+                                                      self.dim, k, self.id_base, _lib.ptr(mask), pitch,
+                                                      _lib.ptr(exclude_ids), out_s.data_ptr(), out_i.data_ptr(),
+                                                      self._ws.data_ptr(), self._ws.numel(), _lib.current_stream())
         _lib.check(rc, "sgpt_search_gather")
         return out_s, out_i
 
     def view(self, start: int, end: int) -> "CorpusShard":
         """Documents [start, end) of this shard as a shard of their own that shares the vectors; its ids are the
-        positions ``start ..`` inside this shard.  (The scales are copied: the kernels read them 16 bytes at a time.)"""
+        positions ``start ..`` inside this shard.  (The scales are copied: the kernels read them 16 bytes at a time.)
+        The view shares this shard's deletions, in both directions."""
         v = object.__new__(CorpusShard)
         v.dim, v.capacity, v.id_base, v.device, v.dtype = self.dim, end - start, int(start), self.device, self.dtype
         v.vectors = self.vectors[start:end]
@@ -271,29 +382,34 @@ class CorpusShard:
             v.inv_norms = self.inv_norms[start:end].clone()
         v.n = end - start
         v._ws = None
+        v._deleted, v._deleted_at = self._deleted, self._deleted_at + int(start)
         return v
 
     def _range_call(self, qb: torch.Tensor, q_scale: Optional[torch.Tensor], c_scale: Optional[int], threshold: float,
-                    counts: torch.Tensor, cap: int, out_s: Optional[torch.Tensor], out_i: Optional[torch.Tensor]) -> None:
-        """One sgpt_range_search of the query rows qb, in the shard's format (include/sgpt_b200.h): counts int64[Q]
-        always, the entries of the queries that fit into `cap` into out_s / out_i."""
+                    counts: torch.Tensor, cap: int, out_s: Optional[torch.Tensor], out_i: Optional[torch.Tensor],
+                    mask: Tuple[Optional[torch.Tensor], int] = (None, 0)) -> None:
+        """One sgpt_range_search_masked of the query rows qb, in the shard's format (include/sgpt_b200.h): counts
+        int64[Q] always, the entries of the queries that fit into `cap` into out_s / out_i.  mask: (bitmap, pitch) of
+        ``_mask`` for these queries."""
         nq = qb.shape[0]
         ws = self._workspace(_lib.lib().sgpt_range_search_workspace_bytes(nq, self.n))
         with torch.cuda.device(self.device):
-            rc = self._fn("sgpt_range_search")(qb.data_ptr(), self.vectors.data_ptr(), _lib.ptr(q_scale), c_scale, nq,
-                                              self.n, self.dim, float(threshold), self.id_base, counts.data_ptr(), cap,
-                                              _lib.ptr(out_s), _lib.ptr(out_i), ws.data_ptr(), ws.numel(),
-                                              _lib.current_stream())
+            rc = _lib.lib().sgpt_range_search_masked(self._dtype_id(), qb.data_ptr(), self.vectors.data_ptr(),
+                                                     _lib.ptr(q_scale), c_scale, nq, self.n, self.dim, float(threshold),
+                                                     self.id_base, _lib.ptr(mask[0]), mask[1], counts.data_ptr(), cap,
+                                                     _lib.ptr(out_s), _lib.ptr(out_i), ws.data_ptr(), ws.numel(),
+                                                     _lib.current_stream())
         _lib.check(rc, "sgpt_range_search")
 
     def _range(self, qb: torch.Tensor, q_scale: Optional[torch.Tensor], c_scale: Optional[int], threshold: float,
-               capacity: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+               capacity: Optional[int] = None, mask: Tuple[Optional[torch.Tensor], int] = (None, 0)
+               ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         nq = qb.shape[0]
         cap = max(4096, 64 * nq) if capacity is None else max(1, int(capacity))
         counts = torch.empty(nq, dtype=torch.int64, device=self.device)
         out_s = torch.empty(cap, dtype=torch.float32, device=self.device)
         out_i = torch.empty(cap, dtype=torch.int64, device=self.device)
-        self._range_call(qb, q_scale, c_scale, threshold, counts, cap, out_s, out_i)
+        self._range_call(qb, q_scale, c_scale, threshold, counts, cap, out_s, out_i, mask)
         offsets = torch.zeros(nq + 1, dtype=torch.int64, device=self.device)
         torch.cumsum(counts, 0, out=offsets[1:])
         total = int(offsets[-1])
@@ -306,21 +422,22 @@ class CorpusShard:
             grown_s[:done].copy_(out_s[:done])
             grown_i[:done].copy_(out_i[:done])
             rest = torch.empty(nq - first, dtype=torch.int64, device=self.device)
+            rest_mask = (mask[0][first:], mask[1]) if mask[1] > 0 else mask  # per-query bitmaps: rows of the rest
             self._range_call(qb[first:], None if q_scale is None else q_scale[first:], c_scale, threshold, rest,
-                             total - done, grown_s[done:], grown_i[done:])
+                             total - done, grown_s[done:], grown_i[done:], rest_mask)
             out_s, out_i = grown_s, grown_i
         return offsets, out_s[:total], out_i[:total]
 
-    def range_search(self, queries: torch.Tensor, threshold: float, score_function: str = "cos_sim"
-                     ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    def range_search(self, queries: torch.Tensor, threshold: float, score_function: str = "cos_sim",
+                     allow: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Every document whose score against a query is >= threshold, for fp32/bf16 queries [Q, D] (device).
 
         Returns (offsets int64 [Q+1], scores fp32 [E], global ids int64 [E]) on the device: query q's documents are
         entries offsets[q] .. offsets[q+1], in ascending id order.  Queries are converted and scored exactly as in
         ``search``; a NaN score counts as -1.  The output buffer starts at 64 entries per query and grows once, for the
-        queries that did not fit."""
+        queries that did not fit.  ``allow`` as in ``search``: only allowed, undeleted documents are counted and returned."""
         qb, q_scale, c_scale = self._queries(queries, score_function)
-        return self._range(qb, q_scale, c_scale, threshold)
+        return self._range(qb, q_scale, c_scale, threshold, mask=self._mask(allow, qb.shape[0]))
 
 
 def unpack_topk(packed: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:

@@ -23,6 +23,9 @@ _MEMBERS_PER_BLOCK = 1 << 26    # community members fetched per range search cal
 def _as_shard(embeddings: Union[torch.Tensor, CorpusShard]) -> CorpusShard:
     """The embeddings as a shard whose ids are row positions 0 .. N-1."""
     if isinstance(embeddings, CorpusShard):
+        if embeddings.n_deleted > 0:
+            # deleted rows would still be mined as queries: refuse rather than return pairs of deleted documents
+            raise ValueError(f"mining a CorpusShard with deleted documents ({embeddings.n_deleted}) is not supported")
         return embeddings.view(0, embeddings.n)
     emb = torch.as_tensor(embeddings)
     if emb.dim() == 1:
