@@ -188,10 +188,8 @@ typedef struct sgpt_model_weights {
 typedef struct sgpt_model* sgpt_model_t;
 
 /* Replaces AutoModel.from_pretrained(...).to(device) at BDR:123 / ST/models/Transformer.py:38 (weights are handed
- * over already on the device; the handle borrows them and owns its activation workspace and the LayerNorm-folded copies
- * it derives at creation: per layer w_qkv, b_qkv, w_fc, b_fc and ln1 / ln2 are folded into library-owned buffers
- * (sgpt_fold_layernorm) and are NOT referenced after sgpt_model_create returns — the caller may free them; wte, wpe, w_o,
- * b_o, w_proj, b_proj, ln_f and the embedding LayerNorm stay borrowed).  Synchronises the device. */
+ * over already on the device).  The handle borrows every weight buffer for its whole lifetime: none of them may be freed
+ * or changed before sgpt_model_destroy.  It owns only its activation workspace.  Synchronises the device. */
 int sgpt_model_create(const sgpt_model_config* cfg, const sgpt_model_weights* w, sgpt_model_t* out);
 void sgpt_model_destroy(sgpt_model_t m);
 
@@ -425,35 +423,6 @@ int sgpt_pool_ex2(const void* x, int x_bf16, const int32_t* pos, const int32_t* 
                   float* row_stats_ws, int B, int T, int d, int mode, int clamp_denominator, int normalize,
                   int accumulate, float out_scale, sgpt_stream_t stream);
 int sgpt_bf16_to_f32(const void* x, float* y, int64_t count, sgpt_stream_t stream);
-
-/* ------------------------------------------------------------------------------------------------------------------
- * LayerNorm without a pass of its own (F2 fused into F3 / F6 / F7).  HF applies ln_1 / ln_2 as separate modules
- * (HF:gpt_neo/modeling_gpt_neo.py:332,345); here
- *   - the kernels that write the residual stream also emit xb = bf16(resid) and, per row and 128-column group, the
- *     partial sums (sum x, sum x^2): sgpt_resid_stats (after the embedding) and sgpt_linear_resid_ln (out-proj / c_proj:
- *     resid += x w^T + bias in place, one TMA load + store of the residual tile in the GEMM epilogue);
- *   - the consuming GEMM runs on xb with gamma folded into its weights (sgpt_fold_layernorm, once per model):
- *     out = act( r_t * (xb W'^T) - r_t mu_t * colsum + bias' ), (mu_t, r_t) rebuilt from the partial sums
- *     (sgpt_linear_lnfold; sgpt_linear_qkv_rotary_lnfold adds GPT-J's rotary embedding);
- *   - ln_f + pooling read the same partial sums (sgpt_pool_partials).
- * row_stats: float2[M, n_groups], n_groups = ceil(d / 128).  eps: LayerNorm epsilon.
- * ------------------------------------------------------------------------------------------------------------------ */
-int sgpt_fold_layernorm(const void* w, const float* gamma, const float* beta, const float* bias, void* w_out,
-                        float* colsum_out, float* bias_out, int N, int K, sgpt_stream_t stream);
-int sgpt_resid_stats(const float* resid, void* xb, float* stats, int T, int d, sgpt_stream_t stream);
-int sgpt_linear_lnfold(const void* x_bf16, int64_t ldx, const void* w_folded, int64_t ldw, const float* bias_folded,
-                       const float* colsum, const float* row_stats, int n_groups, float eps, void* out, int64_t ldo,
-                       int M, int N, int K, int gelu, sgpt_stream_t stream);
-int sgpt_linear_qkv_rotary_lnfold(const void* x_bf16, int64_t ldx, const void* w_folded, const float* bias_folded,
-                                  const float* colsum, const float* row_stats, int n_groups, float eps, void* qkv,
-                                  const int32_t* pos, const float* cos_sin, int M, int d_model, int head_dim,
-                                  int rotary_dim, int max_pos, sgpt_stream_t stream);
-int sgpt_linear_resid_ln(const void* x, int64_t ldx, const void* w, int64_t ldw, const float* bias, float* resid,
-                         void* xb_out, float* stats_out, int M, int N, int K, sgpt_stream_t stream);
-int sgpt_pool_partials(const float* x, const int32_t* pos, const int32_t* cu_seqlens, const float* gamma,
-                       const float* beta, float eps, const float* pos_weights, int n_pos_weights, float* out,
-                       const float* partial_stats, int n_partials, float* sumsq_ws, int B, int T, int d, int mode,
-                       int clamp_denominator, int normalize, int accumulate, float out_scale, sgpt_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Measurement hooks (bench.py): launch counters are always on; with profiling enabled every kernel launch issued

@@ -81,12 +81,6 @@ _SIGNATURES = {
     "sgpt_layernorm_gather_ex": (i32, [vp, i32, vp, vp, vp, vp, i32, i32, f32, vp]),
     "sgpt_pool_ex2": (i32, [vp, i32, vp, vp, vp, vp, f32, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32, f32, vp]),
     "sgpt_bf16_to_f32": (i32, [vp, vp, i64, vp]),
-    "sgpt_fold_layernorm": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, vp]),
-    "sgpt_resid_stats": (i32, [vp, vp, vp, i32, i32, vp]),
-    "sgpt_linear_lnfold": (i32, [vp, i64, vp, i64, vp, vp, vp, i32, f32, vp, i64, i32, i32, i32, i32, vp]),
-    "sgpt_linear_qkv_rotary_lnfold": (i32, [vp, i64, vp, vp, vp, vp, i32, f32, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
-    "sgpt_linear_resid_ln": (i32, [vp, i64, vp, i64, vp, vp, vp, vp, i32, i32, i32, vp]),
-    "sgpt_pool_partials": (i32, [vp, vp, vp, vp, vp, f32, vp, i32, vp, vp, i32, vp, i32, i32, i32, i32, i32, i32, i32, f32, vp]),
     "sgpt_search_packed": (i32, [vp, vp, vp, vp, i32, i64, i32, i32, i64, vp, vp, i64, vp]),
     "sgpt_topk_merge_packed": (i32, [vp, i32, i32, i32, vp, vp, vp, vp]),
     "sgpt_gather_create": (i32, [i32, i32, i32, i32, C.POINTER(vp), vp]),

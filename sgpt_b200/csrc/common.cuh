@@ -352,33 +352,6 @@ __device__ __forceinline__ void named_bar_sync(int id, int count) {
 // ---------------------------------------------------------------------------------------------------------------
 // numerics
 // ---------------------------------------------------------------------------------------------------------------
-// LayerNorm statistics of a residual-stream row from its partial sums.  The kernels that WRITE the residual stream (token
-// embedding, out-proj / c_proj epilogues) leave, per row and per group of 128 columns, (sum x, sum x^2) in
-// stats[row * P + group] (P = ceil(d / 128)); the kernels that consume LN(row) — the QKV / c_fc GEMM epilogues with the
-// LayerNorm folded into the weights, and the ln_f + pooling kernel — rebuild mean and 1/sqrt(var + eps) from them in a
-// fixed summation order (deterministic).  rm = rstd * mean.
-struct LnRow {
-  float r, rm;
-};
-__device__ __forceinline__ LnRow ln_row_from_partials(const float2* __restrict__ stats, int P, float inv_d, float eps,
-                                                      int row, int M) {
-  float s1 = 0.f, s2 = 0.f;
-  if (row < M) {
-    const float2* s = stats + static_cast<size_t>(row) * P;
-    for (int g = 0; g < P; ++g) {
-      const float2 t = __ldg(s + g);
-      s1 += t.x;
-      s2 += t.y;
-    }
-  }
-  const float mean = s1 * inv_d;
-  const float var = fmaxf(s2 * inv_d - mean * mean, 0.f);
-  LnRow o;
-  o.r = rsqrtf(var + eps);
-  o.rm = o.r * mean;
-  return o;
-}
-
 // gelu_new(x) = 0.5 x (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3)))   (HF activations.py NewGELUActivation)
 __device__ __forceinline__ float gelu_new(float x) {
   const float k0 = 0.7978845608028654f, k1 = 0.044715f;

@@ -436,68 +436,6 @@ __global__ void __launch_bounds__(256) row_stats_kernel(const void* __restrict__
   if (active && l == 0) stats[row] = make_float2(mean, rsqrtf(var + eps));
 }
 
-// Residual stream -> what the LayerNorm-folded GEMMs consume: xb = bf16(resid) and, per row and 128-column group, the
-// partial sums (sum x, sum x^2) (common.cuh ln_row_from_partials).  16 lanes per (row, group): each lane one 32-byte
-// vector of 8 floats — 512-byte contiguous reads, 256-byte contiguous writes; used once per forward (after the token
-// embedding); inside the blocks the out-proj / c_proj epilogues produce both themselves.
-__global__ void __launch_bounds__(256) resid_stats_kernel(const float4* __restrict__ x, uint4* __restrict__ xb,
-                                                          float2* __restrict__ stats, int T, int d, int P) {
-  pdl_sync();  // programmatic dependent launch: see common.cuh
-  const long long total = static_cast<long long>(T) * P;
-  const int sub = threadIdx.x & 15;
-  for (long long i = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) >> 4; i < ((total + 15) & ~15ll);
-       i += (static_cast<long long>(gridDim.x) * blockDim.x) >> 4) {
-    const bool live = i < total;
-    const int t = live ? static_cast<int>(i / P) : 0;
-    const int g = live ? static_cast<int>(i - static_cast<long long>(t) * P) : 0;
-    const int col = g * 128 + sub * 8;
-    float s1 = 0.f, s2 = 0.f;
-    if (live && col < d) {
-      const float4* src = x + (static_cast<size_t>(t) * d + col) / 4;
-      const float4 a = src[0], b = src[1];
-      s1 = ((a.x + a.y) + (a.z + a.w)) + ((b.x + b.y) + (b.z + b.w));
-      s2 = ((a.x * a.x + a.y * a.y) + (a.z * a.z + a.w * a.w)) + ((b.x * b.x + b.y * b.y) + (b.z * b.z + b.w * b.w));
-      xb[(static_cast<size_t>(t) * d + col) / 8] =
-          make_uint4(pack_bf16(a.x, a.y), pack_bf16(a.z, a.w), pack_bf16(b.x, b.y), pack_bf16(b.z, b.w));
-    }
-#pragma unroll
-    for (int o = 8; o > 0; o >>= 1) {
-      s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-      s2 += __shfl_xor_sync(0xffffffffu, s2, o);
-    }
-    if (live && sub == 0) stats[i] = make_float2(s1, s2);
-  }
-}
-
-// Fold a LayerNorm into the linear layer that consumes it (gemm.cuh OpTmaLnBiasActBF16), once per model:
-//   w_out[n, k] = bf16(w[n, k] * gamma[k]);  colsum[n] = sum_k float(w_out[n, k]);  bias_out[n] = bias[n] + sum_k beta[k] w[n, k]
-// One warp per output row n.
-__global__ void __launch_bounds__(256) fold_layernorm_kernel(const __nv_bfloat16* __restrict__ w,
-                                                             const float* __restrict__ gamma,
-                                                             const float* __restrict__ beta,
-                                                             const float* __restrict__ bias,
-                                                             __nv_bfloat16* __restrict__ w_out,
-                                                             float* __restrict__ colsum, float* __restrict__ bias_out,
-                                                             int N, int K) {
-  const int n = blockIdx.x * 8 + (threadIdx.x >> 5);
-  if (n >= N) return;
-  const int lane = threadIdx.x & 31;
-  float cs = 0.f, bs = 0.f;
-  for (int k = lane; k < K; k += 32) {
-    const float wv = __bfloat162float(w[static_cast<size_t>(n) * K + k]);
-    const __nv_bfloat16 f = __float2bfloat16_rn(wv * gamma[k]);
-    w_out[static_cast<size_t>(n) * K + k] = f;
-    cs += __bfloat162float(f);
-    bs = fmaf(beta[k], wv, bs);
-  }
-  cs = warp_sum(cs);
-  bs = warp_sum(bs);
-  if (lane == 0) {
-    colsum[n] = cs;
-    bias_out[n] = bs + (bias != nullptr ? bias[n] : 0.f);
-  }
-}
-
 // Choose (threads-per-row, float4-per-thread) so the row lives in registers: d <= 1024 -> one warp per row.
 #define SGPT_ROW_DISPATCH(KERNEL, d4, T, stream, ...)                                               \
   do {                                                                                              \
@@ -528,7 +466,7 @@ __global__ void __launch_bounds__(128) pool_kernel(const void* __restrict__ x, c
                                                    const float4* __restrict__ g, const float4* __restrict__ bta,
                                                    float4* __restrict__ out, float* __restrict__ sumsq, int d4,
                                                    int mode, int clamp_den, int accumulate, float out_scale,
-                                                   int n_partials, float eps, int x_bf16) {
+                                                   int x_bf16) {
   pdl_sync();  // programmatic dependent launch: see common.cuh
   __shared__ float4 part[4][32];
   __shared__ float wpart[4];
@@ -552,15 +490,7 @@ __global__ void __launch_bounds__(128) pool_kernel(const void* __restrict__ x, c
     if (w != 0.f && col_ok) {
       float4 v = ld_row4(x, static_cast<size_t>(t) * d4 + col, x_bf16);
       if (stats != nullptr) {
-        // n_partials == 0: stats[t] = (mean, rstd) from row_stats_kernel; > 0: the partial sums left by the kernel that
-        // wrote the residual stream (no separate pass over it)
-        float2 s;
-        if (n_partials > 0) {
-          const LnRow lr = ln_row_from_partials(stats, n_partials, 0.25f / static_cast<float>(d4), eps, t, t + 1);
-          s = make_float2(lr.rm / lr.r, lr.r);
-        } else {
-          s = __ldg(stats + t);
-        }
+        const float2 s = __ldg(stats + t);  // (mean, rstd) from row_stats_kernel
         const float wr = w * s.y;
         acc.x += wr * (v.x - s.x); acc.y += wr * (v.y - s.x); acc.z += wr * (v.z - s.x); acc.w += wr * (v.w - s.x);
       } else {
@@ -960,11 +890,11 @@ extern "C" int sgpt_layernorm_f32_inplace(float* x, const float* gamma, const fl
   return SGPT_OK;
 }
 
-// shared launcher: `stats` is either (mean, rstd) per row (n_partials == 0) or the [T, n_partials] partial sums
+// `stats`: (mean, rstd) per row, or null (no ln_f)
 static int pool_launch(const void* x, int x_bf16, const int32_t* pos, const int32_t* cu_seqlens, const float* gamma,
-                       const float* beta, float eps, const float* pos_weights, int n_pos_weights, float* out,
-                       const float2* stats, int n_partials, float* sumsq, int B, int d, int mode, int clamp_denominator,
-                       int normalize, int accumulate, float out_scale, cudaStream_t stream) {
+                       const float* beta, const float* pos_weights, int n_pos_weights, float* out, const float2* stats,
+                       float* sumsq, int B, int d, int mode, int clamp_denominator, int normalize, int accumulate,
+                       float out_scale, cudaStream_t stream) {
   const int d4 = d / 4;
   if (normalize) SGPT_CHECK_CUDA(cudaMemsetAsync(sumsq, 0, sizeof(float) * B, stream));
   dim3 grid(B, (d4 + 31) / 32);
@@ -972,7 +902,7 @@ static int pool_launch(const void* x, int x_bf16, const int32_t* pos, const int3
                                 pos_weights, n_pos_weights, cu_seqlens, stats, reinterpret_cast<const float4*>(gamma),
                                 reinterpret_cast<const float4*>(beta), reinterpret_cast<float4*>(out),
                                 normalize ? sumsq : nullptr, d4, mode, clamp_denominator, accumulate, out_scale,
-                                n_partials, eps, x_bf16));
+                                x_bf16));
   if (normalize) {
     SGPT_CHECK_CUDA(launch_kernel(l2_scale_rows_kernel, dim3(grid_for(static_cast<long long>(B) * d4, 256)), dim3(256),
                                   0, stream, reinterpret_cast<float4*>(out), sumsq, B, d4));
@@ -1027,54 +957,9 @@ extern "C" int sgpt_pool_ex2(const void* x, int x_bf16, const int32_t* pos, cons
     SGPT_CHECK_CUDA(cudaGetLastError());
     stats = reinterpret_cast<const float2*>(row_stats_ws);
   }
-  return pool_launch(x, x_bf16, pos, cu_seqlens, gamma, beta, eps, pos_weights, n_pos_weights, out, stats, 0,
+  return pool_launch(x, x_bf16, pos, cu_seqlens, gamma, beta, pos_weights, n_pos_weights, out, stats,
                      normalize ? row_stats_ws + 2 * static_cast<size_t>(T) : nullptr, B, d, mode, clamp_denominator,
                      normalize, accumulate, out_scale, stream);
-}
-
-// ln_f + pooling from the partial row sums the residual-producing kernels left behind (one pass over the residual
-// stream instead of two): partial_stats float2[T, n_partials], sumsq_ws float[B] (only with normalize).
-extern "C" int sgpt_pool_partials(const float* x, const int32_t* pos, const int32_t* cu_seqlens, const float* gamma,
-                                  const float* beta, float eps, const float* pos_weights, int n_pos_weights, float* out,
-                                  const float* partial_stats, int n_partials, float* sumsq_ws, int B, int T, int d,
-                                  int mode, int clamp_denominator, int normalize, int accumulate, float out_scale,
-                                  sgpt_stream_t stream_) {
-  (void)T;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  int rc = pool_check(pos, gamma, beta, pos_weights, n_pos_weights, d, mode);
-  if (rc != SGPT_OK) return rc;
-  SGPT_REQUIRE(gamma != nullptr && partial_stats != nullptr && n_partials > 0,
-               "sgpt_pool_partials: gamma/beta and the partial row sums are required");
-  SGPT_REQUIRE(!normalize || sumsq_ws != nullptr, "sgpt_pool_partials: normalize needs sumsq_ws");
-  if (B == 0) return SGPT_OK;
-  LaunchScope _ls(kCatPool, stream);
-  return pool_launch(x, 0, pos, cu_seqlens, gamma, beta, eps, pos_weights, n_pos_weights, out,
-                     reinterpret_cast<const float2*>(partial_stats), n_partials, sumsq_ws, B, d, mode, clamp_denominator,
-                     normalize, accumulate, out_scale, stream);
-}
-
-extern "C" int sgpt_resid_stats(const float* resid, void* xb, float* stats, int T, int d, sgpt_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SGPT_REQUIRE(T >= 0 && d > 0 && d % 8 == 0, "sgpt_resid_stats: d=%d must be a positive multiple of 8", d);
-  if (T == 0) return SGPT_OK;
-  const int P = (d + 127) / 128;
-  LaunchScope _ls(kCatLayerNorm, stream);
-  SGPT_CHECK_CUDA(launch_kernel(resid_stats_kernel, dim3(grid_for(static_cast<long long>(T) * P * 16, 256)), dim3(256), 0,
-                                stream, reinterpret_cast<const float4*>(resid), static_cast<uint4*>(xb),
-                                reinterpret_cast<float2*>(stats), T, d, P));
-  return SGPT_OK;
-}
-
-extern "C" int sgpt_fold_layernorm(const void* w, const float* gamma, const float* beta, const float* bias, void* w_out,
-                                   float* colsum_out, float* bias_out, int N, int K, sgpt_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SGPT_REQUIRE(N > 0 && K > 0 && w != nullptr && gamma != nullptr && beta != nullptr && w_out != nullptr &&
-                   colsum_out != nullptr && bias_out != nullptr, "sgpt_fold_layernorm: bad arguments");
-  LaunchScope _ls(kCatMisc, stream);
-  fold_layernorm_kernel<<<(N + 7) / 8, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(w), gamma, beta, bias,
-                                                         static_cast<__nv_bfloat16*>(w_out), colsum_out, bias_out, N, K);
-  SGPT_CHECK_CUDA(cudaGetLastError());
-  return SGPT_OK;
 }
 
 extern "C" int sgpt_pool_accumulate(const float* x, const int32_t* pos, const int32_t* cu_seqlens, const float* gamma,

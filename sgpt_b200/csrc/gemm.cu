@@ -280,87 +280,6 @@ extern "C" int sgpt_linear_qkv_rotary(const void* x, int64_t ldx, const void* w_
   return launch_linear<EpiRotaryBF16>(x, ldx, w_qkv, d_model, M, N, d_model, p, stream);
 }
 
-// F2+F3 / F2+F6 with the LayerNorm folded into the GEMM (gemm.cuh OpTmaLnBiasActBF16): x_bf16 is the bf16 copy of the
-// residual stream, w the gamma-folded weight, bias / colsum the folded vectors, row_stats the partial sums.
-extern "C" int sgpt_linear_lnfold(const void* x_bf16, int64_t ldx, const void* w_folded, int64_t ldw,
-                                  const float* bias_folded, const float* colsum, const float* row_stats, int n_groups,
-                                  float eps, void* out, int64_t ldo, int M, int N, int K, int gelu,
-                                  sgpt_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SGPT_REQUIRE(M >= 0 && N > 0 && K > 0, "sgpt_linear_lnfold: bad sizes M=%d N=%d K=%d", M, N, K);
-  SGPT_REQUIRE(K % 8 == 0 && ldx % 8 == 0 && ldw % 8 == 0 && ldo % 8 == 0, "sgpt_linear_lnfold: K, ldx, ldw, ldo must be multiples of 8");
-  SGPT_REQUIRE(ldx >= K && ldw >= K && ldo >= N, "sgpt_linear_lnfold: row pitch smaller than the row");
-  SGPT_REQUIRE(bias_folded != nullptr && colsum != nullptr && row_stats != nullptr && n_groups > 0,
-               "sgpt_linear_lnfold: folded bias / column sums / row statistics are required");
-  SGPT_REQUIRE(N % 4 == 0, "sgpt_linear_lnfold: N must be a multiple of 4");
-  if (M == 0) return SGPT_OK;
-  CUtensorMap om;
-  int rc = make_tma_2d_bf16(&om, out, static_cast<uint64_t>(M), static_cast<uint64_t>(N), static_cast<uint64_t>(ldo), 32, 64);
-  if (rc != SGPT_OK) return rc;
-  const float inv_d = 1.0f / static_cast<float>(K);
-  if (gelu) {
-    EpiLnBiasActBF16<true>::Params p{om, bias_folded, colsum, reinterpret_cast<const float2*>(row_stats), n_groups, inv_d, eps,
-                                     out, static_cast<int>(ldo)};
-    return launch_linear<EpiLnBiasActBF16<true>>(x_bf16, ldx, w_folded, ldw, M, N, K, p, stream);
-  }
-  EpiLnBiasActBF16<false>::Params p{om, bias_folded, colsum, reinterpret_cast<const float2*>(row_stats), n_groups, inv_d, eps,
-                                    out, static_cast<int>(ldo)};
-  return launch_linear<EpiLnBiasActBF16<false>>(x_bf16, ldx, w_folded, ldw, M, N, K, p, stream);
-}
-
-extern "C" int sgpt_linear_qkv_rotary_lnfold(const void* x_bf16, int64_t ldx, const void* w_folded,
-                                             const float* bias_folded, const float* colsum, const float* row_stats,
-                                             int n_groups, float eps, void* qkv, const int32_t* pos,
-                                             const float* cos_sin, int M, int d_model, int head_dim, int rotary_dim,
-                                             int max_pos, sgpt_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SGPT_REQUIRE(M >= 0 && d_model > 0 && d_model % 8 == 0 && ldx % 8 == 0 && ldx >= d_model,
-               "sgpt_linear_qkv_rotary_lnfold: bad sizes M=%d d=%d ldx=%lld", M, d_model, (long long)ldx);
-  SGPT_REQUIRE(head_dim > 0 && d_model % head_dim == 0 && head_dim % 8 == 0, "sgpt_linear_qkv_rotary_lnfold: bad head_dim %d",
-               head_dim);
-  SGPT_REQUIRE(rotary_dim >= 0 && rotary_dim <= head_dim && rotary_dim % 8 == 0,
-               "sgpt_linear_qkv_rotary_lnfold: rotary_dim %d must be a multiple of 8 and <= head_dim", rotary_dim);
-  SGPT_REQUIRE(pos != nullptr && cos_sin != nullptr && max_pos > 0, "sgpt_linear_qkv_rotary_lnfold: pos / cos_sin missing");
-  SGPT_REQUIRE(bias_folded != nullptr && colsum != nullptr && row_stats != nullptr && n_groups > 0,
-               "sgpt_linear_qkv_rotary_lnfold: folded bias / column sums / row statistics are required");
-  if (M == 0) return SGPT_OK;
-  const int N = 3 * d_model;
-  CUtensorMap om;
-  int rc = make_tma_2d_bf16(&om, qkv, static_cast<uint64_t>(M), static_cast<uint64_t>(N), static_cast<uint64_t>(N), 32, 64);
-  if (rc != SGPT_OK) return rc;
-  EpiLnRotaryBF16::Params p{{om, pos, reinterpret_cast<const float2*>(cos_sin), M, d_model, head_dim, rotary_dim, max_pos, qkv, N},
-                            bias_folded, colsum, reinterpret_cast<const float2*>(row_stats), n_groups,
-                            1.0f / static_cast<float>(d_model), eps, qkv, N};
-  return launch_linear<EpiLnRotaryBF16>(x_bf16, ldx, w_folded, d_model, M, N, d_model, p, stream);
-}
-
-// F5 / F6b with the statistics of the NEXT LayerNorm (gemm.cuh EpiResidLn): resid += x w^T + bias in place, plus the
-// bf16 copy and the per-(row, 128-column group) partial sums of the new residual.
-extern "C" int sgpt_linear_resid_ln(const void* x, int64_t ldx, const void* w, int64_t ldw, const float* bias,
-                                    float* resid, void* xb_out, float* stats_out, int M, int N, int K,
-                                    sgpt_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SGPT_REQUIRE(M >= 0 && N > 0 && K > 0, "sgpt_linear_resid_ln: bad sizes M=%d N=%d K=%d", M, N, K);
-  SGPT_REQUIRE(K % 8 == 0 && ldx % 8 == 0 && ldw % 8 == 0 && ldx >= K && ldw >= K, "sgpt_linear_resid_ln: bad pitches");
-  SGPT_REQUIRE(N % 64 == 0, "sgpt_linear_resid_ln: N=%d must be a multiple of 64", N);
-  SGPT_REQUIRE(resid != nullptr && xb_out != nullptr && stats_out != nullptr, "sgpt_linear_resid_ln: null output");
-  if (M == 0) return SGPT_OK;
-  EpiResidLn::Params p;
-  int rc = make_tma_2d_f32(&p.resid_map, resid, static_cast<uint64_t>(M), static_cast<uint64_t>(N), static_cast<uint64_t>(N), 32, 32);
-  if (rc != SGPT_OK) return rc;
-  rc = make_tma_2d_bf16(&p.xb_map, xb_out, static_cast<uint64_t>(M), static_cast<uint64_t>(N), static_cast<uint64_t>(N), 32, 64);
-  if (rc != SGPT_OK) return rc;
-  p.bias = bias;
-  p.stats = reinterpret_cast<float2*>(stats_out);
-  p.P = (N + 127) / 128;
-  {
-    static const int l2pf = [] { const char* e = getenv("SGPT_RESID_L2_PREFETCH"); return (e != nullptr && e[0] == '0') ? 0 : 1; }();
-    p.l2_prefetch = l2pf;
-  }
-  // 128-wide tiles and four epilogue warps: each warp owns exactly one 128-column statistics group
-  return launch_gemm<128, EpiResidLn, 1>(x, ldx, w, ldw, M, N, K, p, stream);
-}
-
 extern "C" int sgpt_scores(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* scores,
                            int64_t lds, int nq, int64_t n, int D, sgpt_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);

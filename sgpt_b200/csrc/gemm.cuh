@@ -53,11 +53,6 @@ struct GemmCfg {
   static_assert(kSmemBytes <= 232448, "exceeds the 227 KB per-CTA shared memory limit");
 };
 
-template <class Epi, class = void>
-struct EpiHasPrefetch { static constexpr bool value = false; };
-template <class Epi>
-struct EpiHasPrefetch<Epi, decltype((void)&Epi::prefetch_next)> { static constexpr bool value = true; };
-
 // Epilogue states with a `ks` member are told which K slice of a split-K launch the current work unit covers
 template <class State, class = void>
 struct StateHasKs { static constexpr bool value = false; };
@@ -190,7 +185,6 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
   float* stage_base = reinterpret_cast<float*>(acc_smem + Cfg::kAccBytes);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(acc_smem + Cfg::kAccBytes + Cfg::kStagingBytes);
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* epi_bars = empty_bar + kStages;  // 2 mbarriers per epilogue warp (EpiResidLn's residual loads)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -254,7 +248,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
     float* stage_slab = stage_base + (epi_warp ? warp : 0) * (kSlabBytes / 4);
     const uint32_t acc_base = smem_u32(acc_smem);
     typename Epi::State st;
-    if (epi_warp) Epi::init(st, ep, ew * 32 + lane, epi_bars + 2 * warp);
+    if (epi_warp) Epi::init(st, ep);
     int stage = 0;
     uint32_t phase = 0;
     for (int unit = cid; unit < num_tiles; unit += ncl) {
@@ -266,17 +260,8 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
       const int m0 = (mg * CL + crank) * kGemmBM + ew * 32;  // this warp's 32-row slab
       const int n0 = tmap.map(ntile) * BN + half * kColsPerWarp;
       if (epi_warp) {
-        // work that does not depend on the accumulator (EpiResidLn: the first residual loads, and an L2 prefetch of the
-        // residual boxes of the tile after this one; row constants) overlaps the mainloop
-        if constexpr (EpiHasPrefetch<Epi>::value) {
-          const int nt = (unit + ncl) / ksplit;  // (split-K is never combined with a prefetching epilogue)
-          if (unit + ncl < num_tiles) {
-            int mg2, nt2;
-            tmap.coords(nt, m_tiles, n_tiles, mg2, nt2);
-            Epi::prefetch_next(ep, (mg2 * CL + crank) * kGemmBM + ew * 32, tmap.map(nt2) * BN + half * kColsPerWarp, lane,
-                               M, N);
-          }
-        }
+        // work that does not depend on the accumulator (EpiFilterRows: the document scales and thresholds of the tile)
+        // overlaps the mainloop
         Epi::template pre_tile<kColsPerWarp, kSlabBytes>(st, ep, m0, n0, lane, stage_slab, M, N);
       }
 
@@ -350,12 +335,9 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
 // ---------------------------------------------------------------------------------------------------------------
 // TMA epilogue driver: accumulator -> registers (thread = row) -> Op (bias / activation) -> swizzled smem box -> TMA
 // ---------------------------------------------------------------------------------------------------------------
-template <class Row>
 struct EpiTmaState {
   uint32_t it;  // boxes issued so far by this warp (selects the double buffer)
   uint32_t ks;  // K slice of the current work unit (split-K launches; 0 otherwise): only slice 0 adds the bias
-  Row row;      // per-row constants of the CURRENT tile (LayerNorm mean / rstd), fetched in pre_tile: the loads overlap
-                // the wait for the accumulator instead of sitting at the head of the epilogue's critical path
 };
 
 // Ops whose result is ADDED to the output (TMA reduce-add) can run split-K: they declare kSplitK and take a flag that
@@ -368,14 +350,12 @@ struct OpSplitK<Op, decltype((void)Op::kSplitK)> { static constexpr bool value =
 template <class Op, int kDebug = 0>  // kDebug: 1 = skip the TMA store (timing experiment), 2 = skip the smem-reuse wait
 struct EpiTma {
   using Params = typename Op::Params;
-  using State = EpiTmaState<typename Op::Row>;
+  using State = EpiTmaState;
   static constexpr int kEpiWarps = 8;                 // 2 warps per 32-row slab; each owns ONE 4 KB smem box
   static constexpr int kCols = 128 / Op::kElemBytes;  // columns per 128-byte row segment: 64 (bf16) or 32 (fp32)
-  static __device__ __forceinline__ void init(State& st, const Params&, int, uint64_t*) { st.it = 0; st.ks = 0; }
+  static __device__ __forceinline__ void init(State& st, const Params&) { st.it = 0; st.ks = 0; }
   template <int BN, int kSlabBytes>
-  static __device__ __forceinline__ void pre_tile(State& st, const Params& p, int m0, int, int lane, float*, int M, int) {
-    if (m0 < M) st.row = Op::row_init(p, m0 + lane, M);
-  }
+  static __device__ __forceinline__ void pre_tile(State&, const Params&, int, int, int, float*, int, int) {}
   static __device__ __forceinline__ void finish(State&, const Params&, int lane_row) {
     if ((lane_row & 31) == 0) bulk_wait_group<0>();  // all stores of this warp have fully completed
   }
@@ -385,7 +365,6 @@ struct EpiTma {
                                               float* slab, int M, int N) {
     if (m0 >= M) return;  // whole 32-row slab out of range (warp-uniform)
     const uint32_t sbase = smem_u32(slab);
-    const typename Op::Row rc = st.row;  // per-row constants (thread = row), fetched in pre_tile
 #pragma unroll 1
     for (int c = 0; c < BN; c += kCols) {
       const int n = n0 + c;
@@ -411,9 +390,9 @@ struct EpiTma {
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         if constexpr (OpSplitK<Op>::value)
-          Op::chunk(p, rc, &v[j * (kCols / 8)], n + j * (kCols / 8), N, m0 + lane, o[j], st.ks == 0);
+          Op::chunk(p, &v[j * (kCols / 8)], n + j * (kCols / 8), N, m0 + lane, o[j], st.ks == 0);
         else
-          Op::chunk(p, rc, &v[j * (kCols / 8)], n + j * (kCols / 8), N, m0 + lane, o[j]);
+          Op::chunk(p, &v[j * (kCols / 8)], n + j * (kCols / 8), N, m0 + lane, o[j]);
       }
       if (kDebug == 4) {  // experiment: straight 16-byte global stores from the thread = row layout (no smem, no TMA)
         if (m0 + lane < M) {
@@ -453,10 +432,8 @@ struct OpTmaBiasActBF16 {
     void* out_ptr;        // same tensor as out_map (direct-store variant)
     int ldc;
   };
-  struct Row {};
-  static __device__ __forceinline__ Row row_init(const Params&, int, int) { return Row(); }
   // 8 consecutive columns starting at `col` -> 16 bytes
-  static __device__ __forceinline__ void chunk(const Params& p, const Row&, const uint32_t* acc, int col, int N,
+  static __device__ __forceinline__ void chunk(const Params& p, const uint32_t* acc, int col, int N,
                                                int /*row*/, uint32_t (&o)[4]) {
     float x[8];
     if (p.bias && col + 8 <= N) {
@@ -494,9 +471,7 @@ struct OpTmaRotaryBF16 {
     void* out_ptr;
     int ldc;
   };
-  struct Row {};
-  static __device__ __forceinline__ Row row_init(const Params&, int, int) { return Row(); }
-  static __device__ __forceinline__ void chunk(const Params& p, const Row&, const uint32_t* acc, int col, int N, int row,
+  static __device__ __forceinline__ void chunk(const Params& p, const uint32_t* acc, int col, int N, int row,
                                                uint32_t (&o)[4]) {
     float x[8];
 #pragma unroll
@@ -533,11 +508,9 @@ struct OpTmaResidAddF32 {
     void* out_ptr;
     int ldc;
   };
-  struct Row {};
-  static __device__ __forceinline__ Row row_init(const Params&, int, int) { return Row(); }
   // 4 consecutive columns -> 16 bytes
   static constexpr bool kSplitK = true;
-  static __device__ __forceinline__ void chunk(const Params& p, const Row&, const uint32_t* acc, int col, int N,
+  static __device__ __forceinline__ void chunk(const Params& p, const uint32_t* acc, int col, int N,
                                                int /*row*/, uint32_t (&o)[4], bool add_bias) {
     const float* bias = add_bias ? p.bias : nullptr;
     if (bias && col + 4 <= N) {
@@ -566,10 +539,8 @@ struct OpTmaResidAddBF16 {
     void* out_ptr;
     int ldc;
   };
-  struct Row {};
-  static __device__ __forceinline__ Row row_init(const Params&, int, int) { return Row(); }
   static constexpr bool kSplitK = true;
-  static __device__ __forceinline__ void chunk(const Params& p, const Row&, const uint32_t* acc, int col, int N,
+  static __device__ __forceinline__ void chunk(const Params& p, const uint32_t* acc, int col, int N,
                                                int /*row*/, uint32_t (&o)[4], bool add_bias) {
     const float* bias = add_bias ? p.bias : nullptr;
     float x[8];
@@ -591,217 +562,6 @@ struct OpTmaResidAddBF16 {
   }
 };
 
-// ---- LayerNorm folded into the consumer GEMM -------------------------------------------------------------------------
-// y = LN(x) W^T + b  with  LN(x) = (x - mu) r (*) gamma + beta   is evaluated as
-//     y[t, n] = r_t * (xb W'^T)[t, n] - r_t mu_t * c[n] + b'[n],
-// W' = bf16(W (*) gamma) (gamma folded into the weight columns when the model is created), c[n] = sum_k W'[n, k] (fp32, of
-// the ROUNDED folded weights so that the mean term cancels exactly against the GEMM), b'[n] = b[n] + sum_k beta_k W[n, k],
-// xb = bf16 copy of the fp32 residual stream (written by the kernel that produced the residual), and (mu_t, r_t) from
-// the row's partial sums (ln_row_from_partials).  The separate LayerNorm pass over the residual stream (read 4 B + write
-// 2 B per element, twice per block) disappears; the GEMM reads the same number of bytes as before.
-// out_bf16[m, n] = act(r_m * acc - rm_m * colsum[n] + bias[n])
-template <bool kGelu>
-struct OpTmaLnBiasActBF16 {
-  static constexpr int kElemBytes = 2;
-  struct Params {
-    CUtensorMap out_map;   // bf16 [M, N], box 32 rows x 64 cols, SWIZZLE_128B
-    const float* bias;     // b'  [N]
-    const float* colsum;   // c   [N]
-    const float2* stats;   // [M, P] partial (sum x, sum x^2)
-    int P;
-    float inv_d, eps;
-    void* out_ptr;
-    int ldc;
-  };
-  using Row = LnRow;
-  static __device__ __forceinline__ Row row_init(const Params& p, int row, int M) {
-    return ln_row_from_partials(p.stats, p.P, p.inv_d, p.eps, row, M);
-  }
-  static __device__ __forceinline__ void chunk(const Params& p, const Row& rc, const uint32_t* acc, int col, int N,
-                                               int /*row*/, uint32_t (&o)[4]) {
-    float x[8];
-    if (col + 8 <= N) {
-      const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + col));
-      const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + col) + 1);
-      const float4 c0 = __ldg(reinterpret_cast<const float4*>(p.colsum + col));
-      const float4 c1 = __ldg(reinterpret_cast<const float4*>(p.colsum + col) + 1);
-      const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-      const float cc[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
-#pragma unroll
-      for (int i = 0; i < 8; ++i) x[i] = fmaf(rc.r, __uint_as_float(acc[i]), fmaf(-rc.rm, cc[i], bb[i]));
-    } else {
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-        x[i] = fmaf(rc.r, __uint_as_float(acc[i]), fmaf(-rc.rm, bias_at(p.colsum, col + i, N), bias_at(p.bias, col + i, N)));
-    }
-    if (kGelu) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) x[i] = gelu_new(x[i]);
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) o[i] = pack_bf16(x[2 * i], x[2 * i + 1]);
-  }
-  static __device__ __forceinline__ void issue(const Params& p, const void* box, int n, int m0) {
-    tma_store_2d(&p.out_map, box, n, m0);
-  }
-};
-
-// GPT-J q/k/v projection with ln_1 folded in (as above, no activation) followed by the rotary embedding of OpTmaRotaryBF16.
-struct OpTmaLnRotaryBF16 {
-  static constexpr int kElemBytes = 2;
-  struct Params {
-    OpTmaRotaryBF16::Params rot;
-    const float* bias;     // b' [3d]
-    const float* colsum;   // c  [3d]
-    const float2* stats;
-    int P;
-    float inv_d, eps;
-    void* out_ptr;  // (direct-store debug variant of the driver only)
-    int ldc;
-  };
-  using Row = LnRow;
-  static __device__ __forceinline__ Row row_init(const Params& p, int row, int M) {
-    return ln_row_from_partials(p.stats, p.P, p.inv_d, p.eps, row, M);
-  }
-  static __device__ __forceinline__ void chunk(const Params& p, const Row& rc, const uint32_t* acc, int col, int N, int row,
-                                               uint32_t (&o)[4]) {
-    uint32_t y[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i)
-      y[i] = __float_as_uint(fmaf(rc.r, __uint_as_float(acc[i]),
-                                  fmaf(-rc.rm, bias_at(p.colsum, col + i, N), bias_at(p.bias, col + i, N))));
-    OpTmaRotaryBF16::chunk(p.rot, OpTmaRotaryBF16::Row(), y, col, N, row, o);
-  }
-  static __device__ __forceinline__ void issue(const Params& p, const void* box, int n, int m0) {
-    tma_store_2d(&p.rot.out_map, box, n, m0);
-  }
-};
-
-// ---- residual epilogue that also feeds the NEXT LayerNorm --------------------------------------------------------------
-// resid_f32[m, n] = resid_f32[m, n] + acc + bias[n]  (out-proj / c_proj), and in the same pass
-//     xb_bf16[m, n] = bf16(new residual)                       (A operand of the next QKV / c_fc GEMM)
-//     stats[m, n / 128] = (sum, sum of squares) of the new residual over this warp's 128 columns
-// The old residual is fetched by TMA into a per-warp smem box (two boxes in flight: the first two loads of a tile are
-// issued before the tile's mainloop, the rest chase the stores), updated in place by the row-owning threads and written
-// back with a TMA store; the bf16 copy leaves through a second box.  4 epilogue warps on 128-wide tiles (each warp then
-// owns exactly one 128-column statistics group).  N % 64 == 0.
-struct EpiResidLn {
-  struct Params {
-    CUtensorMap resid_map;  // fp32 [M, N], box 32 rows x 32 cols, SWIZZLE_128B (load and store)
-    CUtensorMap xb_map;     // bf16 [M, N], box 32 rows x 64 cols, SWIZZLE_128B
-    const float* bias;      // may be null
-    float2* stats;          // [M, P]
-    int P;
-    int l2_prefetch;        // prefetch the NEXT tile's residual boxes into L2 one tile ahead (hides the HBM latency)
-  };
-  struct State {
-    uint32_t it;     // residual boxes processed so far by this warp (selects the load buffer and its barrier phase)
-    uint64_t* bars;  // two mbarriers of this warp
-  };
-  static constexpr int kEpiWarps = 4;
-  static constexpr int kStagingBytes = 4 * 12288;  // per warp: two fp32 load/store boxes + one bf16 store box
-  static __device__ __forceinline__ void init(State& st, const Params&, int lane_row, uint64_t* bars) {
-    st.it = 0;
-    st.bars = bars;
-    if ((lane_row & 31) == 0) {
-      mbar_init(&bars[0], 1);
-      mbar_init(&bars[1], 1);
-      fence_mbar_init();
-    }
-    __syncwarp();
-  }
-  static __device__ __forceinline__ void finish(State&, const Params&, int lane_row) {
-    if ((lane_row & 31) == 0) bulk_wait_group<0>();
-  }
-  // called right before pre_tile of the current tile with the coordinates of the tile AFTER it
-  static __device__ __forceinline__ void prefetch_next(const Params& p, int m0, int n0, int lane, int M, int N) {
-    if (!p.l2_prefetch || m0 >= M || lane != 0) return;
-    const int nb = boxes(n0, N, 128);
-    for (int j = 0; j < nb; ++j) tma_prefetch_l2_2d(&p.resid_map, n0 + 32 * j, m0);
-  }
-  static __device__ __forceinline__ int boxes(int n0, int N, int cols) {
-    if (n0 >= N) return 0;
-    const int left = (N - n0) >> 5;
-    return left < (cols >> 5) ? left : (cols >> 5);
-  }
-
-  template <int COLS, int kSlabBytes>
-  static __device__ __forceinline__ void pre_tile(State& st, const Params& p, int m0, int n0, int lane, float* slab,
-                                                  int M, int N) {
-    static_assert(COLS == 128 && kSlabBytes == 12288, "EpiResidLn: 128 columns and 12 KB of staging per warp");
-    if (m0 >= M) return;
-    const int nb = boxes(n0, N, COLS);
-    if (nb <= 0) return;
-    if (lane == 0) {
-      bulk_wait_group_read<0>();  // the previous tile's stores have finished reading all three boxes
-      const uint32_t sbase = smem_u32(slab);
-      for (int j = 0; j < 2 && j < nb; ++j) {
-        const uint32_t b = (st.it + j) & 1u;
-        mbar_expect_tx(&st.bars[b], 4096);
-        tma_load_2d(reinterpret_cast<void*>(__cvta_shared_to_generic(sbase + b * 4096u)), &p.resid_map, &st.bars[b],
-                    n0 + 32 * j, m0);
-      }
-    }
-    __syncwarp();
-  }
-
-  template <int COLS, int kSlabBytes>
-  static __device__ __forceinline__ void tile(State& st, const Params& p, int m0, int n0, int lane, uint32_t trow,
-                                              float* slab, int M, int N) {
-    if (m0 >= M) return;
-    const int nb = boxes(n0, N, COLS);
-    if (nb <= 0) return;
-    const uint32_t sbase = smem_u32(slab);
-    const uint32_t hbox = sbase + 8192u;
-    const uint32_t hrow = hbox + lane * 128u;
-    float s1 = 0.f, s2 = 0.f;
-#pragma unroll 1
-    for (int c = 0; c < nb; ++c) {
-      const uint32_t b = st.it & 1u, ph = (st.it >> 1) & 1u;
-      const uint32_t fb = sbase + b * 4096u;
-      const int n = n0 + 32 * c;
-      uint32_t v[32];
-      acc_ld_32(trow + 4 * 32 * c, v);
-      mbar_wait(&st.bars[b], ph);  // old residual box has landed
-      const uint32_t row_addr = fb + lane * 128u;
-      uint32_t h[16];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const uint32_t a = row_addr + ((j ^ (lane & 7)) << 4);
-        const float4 old = lds_v4(a);
-        float4 bz = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (p.bias != nullptr) bz = __ldg(reinterpret_cast<const float4*>(p.bias + n) + j);
-        const float x0 = old.x + (__uint_as_float(v[4 * j]) + bz.x), x1 = old.y + (__uint_as_float(v[4 * j + 1]) + bz.y);
-        const float x2 = old.z + (__uint_as_float(v[4 * j + 2]) + bz.z), x3 = old.w + (__uint_as_float(v[4 * j + 3]) + bz.w);
-        sts_v4(a, __float_as_uint(x0), __float_as_uint(x1), __float_as_uint(x2), __float_as_uint(x3));
-        s1 += (x0 + x1) + (x2 + x3);
-        s2 += (x0 * x0 + x1 * x1) + (x2 * x2 + x3 * x3);
-        h[2 * j] = pack_bf16(x0, x1);
-        h[2 * j + 1] = pack_bf16(x2, x3);
-      }
-      // bf16 copy: these 32 columns are chunks 4 (c & 1) .. + 3 of the row's 128-byte segment in the 64-column box
-#pragma unroll
-      for (int q4 = 0; q4 < 4; ++q4)
-        sts_v4(hrow + (((((c & 1) << 2) + q4) ^ (lane & 7)) << 4), h[4 * q4], h[4 * q4 + 1], h[4 * q4 + 2], h[4 * q4 + 3]);
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) {
-        tma_store_2d(&p.resid_map, reinterpret_cast<const void*>(__cvta_shared_to_generic(fb)), n, m0);
-        if (c & 1) tma_store_2d(&p.xb_map, reinterpret_cast<const void*>(__cvta_shared_to_generic(hbox)), n - 32, m0);
-        bulk_commit_group();
-        if (c + 2 < nb) {
-          bulk_wait_group_read<0>();  // this box (and the bf16 box) may be overwritten now
-          mbar_expect_tx(&st.bars[b], 4096);
-          tma_load_2d(reinterpret_cast<void*>(__cvta_shared_to_generic(fb)), &p.resid_map, &st.bars[b], n + 64, m0);
-        }
-      }
-      __syncwarp();
-      ++st.it;
-    }
-    if (m0 + lane < M) p.stats[static_cast<size_t>(m0 + lane) * p.P + (n0 >> 7)] = make_float2(s1, s2);
-  }
-};
-
 // ---------------------------------------------------------------------------------------------------------------
 // Staged epilogue driver: accumulator -> registers (thread = row) -> smem slab -> (lane = column pair) -> Op::rows()
 // The slab is [32 rows][32 column pairs] of float2 without padding; pair p of row r is stored at p ^ (r & 15), which
@@ -814,7 +574,7 @@ struct EpiStaged {
   using Params = typename Op::Params;
   using State = EpiNoState;
   static constexpr int kEpiWarps = 4;
-  static __device__ __forceinline__ void init(State&, const Params&, int, uint64_t*) {}
+  static __device__ __forceinline__ void init(State&, const Params&) {}
   template <int BN, int kSlabBytes>
   static __device__ __forceinline__ void pre_tile(State&, const Params&, int, int, int, float*, int, int) {}
   static __device__ __forceinline__ void finish(State&, const Params&, int) {}
@@ -1008,7 +768,7 @@ struct EpiFilterRowsT {
   static __device__ __forceinline__ int group_of(const Params& p) {
     return p.group0 + static_cast<int>(blockIdx.x >> p.pair) * 2 + static_cast<int>(threadIdx.x >> 7);
   }
-  static __device__ __forceinline__ void init(State& st, const Params&, int, uint64_t*) { st.cnt = 0; st.cnt_b = 0; }
+  static __device__ __forceinline__ void init(State& st, const Params&) { st.cnt = 0; st.cnt_b = 0; }
   template <int COLS, int kSlabBytes>
   static __device__ __forceinline__ void pre_tile(State& st, const Params& p, int m0, int n0, int lane, float*, int M, int N) {
     static_assert(COLS == 128, "one float4 of document scales per lane covers the warp's half tile");
@@ -1157,9 +917,6 @@ using EpiBiasActBF16 = EpiTma<OpTmaBiasActBF16<kGelu>>;
 using EpiResidualF32 = EpiTma<OpTmaResidAddF32>;
 using EpiResidualBF16 = EpiTma<OpTmaResidAddBF16>;
 using EpiRotaryBF16 = EpiTma<OpTmaRotaryBF16>;
-template <bool kGelu>
-using EpiLnBiasActBF16 = EpiTma<OpTmaLnBiasActBF16<kGelu>>;
-using EpiLnRotaryBF16 = EpiTma<OpTmaLnRotaryBF16>;
 
 // Bring-up / profiling aids (sgpt_linear epilogue codes 100, 101): no epilogue work at all, or accumulator loads only.
 template <bool kLoad>
@@ -1167,7 +924,7 @@ struct EpiDebugNull {
   struct Params { int dummy; };
   using State = EpiNoState;
   static constexpr int kEpiWarps = 4;
-  static __device__ __forceinline__ void init(State&, const Params&, int, uint64_t*) {}
+  static __device__ __forceinline__ void init(State&, const Params&) {}
   template <int BN, int kSlabBytes>
   static __device__ __forceinline__ void pre_tile(State&, const Params&, int, int, int, float*, int, int) {}
   static __device__ __forceinline__ void finish(State&, const Params&, int) {}

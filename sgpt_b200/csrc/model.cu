@@ -9,17 +9,11 @@
 //                                                       bias) -> +res -> post_attention_layernorm -> mlp (tanh gelu) -> +res
 // The handle borrows the caller's weight buffers and owns only its activation workspace, laid out for a ragged batch
 // of at most cfg.max_tokens rows:
-//     resid fp32[T,d] | xb bf16[T,d] | qkv bf16[T,3d] | attn bf16[T,d] | ffn bf16[T,ff] | stats fp32[2T*P+B]
+//     resid fp32[T,d] | xb bf16[T,d] | qkv bf16[T,3d] | attn bf16[T,d] | ffn bf16[T,ff] | stats fp32[2T+B]
 //
-// Two block flows (chosen when the handle is created):
-//   default         LayerNorm as its own HBM pass (fp32 residual -> bf16), GEMMs with bias / gelu / reduce-add epilogues.
-//   SGPT_LN_FOLD=1  no LayerNorm pass inside the blocks: the kernels that WRITE the residual stream (token embedding;
-//                   out-proj / c_proj epilogues, gemm.cuh EpiResidLn) also leave xb = bf16(resid) and per-row partial sums
-//                   (sum x, sum x^2 per 128 columns); the GEMMs that consume LN(resid) (QKV, c_fc) run on xb with gamma folded
-//                   into their weight columns and apply  y = r (xb W'^T) - r mu c + b'  per row in the epilogue
-//                   (OpTmaLnBiasActBF16); ln_f is folded into the pooling kernel the same way.  Parity-tested like the
-//                   default; opt-in (every instruction and byte the GEMM epilogues add can cost as much time as the
-//                   LayerNorm pass it replaces).
+// Each block runs LayerNorm as a pass of its own (residual stream -> bf16 xb), then GEMMs with bias / gelu epilogues for
+// the layers that read xb and reduce-add epilogues for the layers that update the residual stream.  The residual stream is
+// bf16 (SGPT_RESID_BF16=0 at creation: fp32).
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -35,14 +29,8 @@ struct sgpt_model {
   std::vector<sgpt_layer_weights> layers;
   int device = 0;
   float* resid = nullptr;
-  void* xn = nullptr;  // xb: bf16 copy of the residual stream
-  int P = 0;           // statistics groups per row = ceil(d / 128)
-  bool ln_fold = false;  // SGPT_LN_FOLD=1 at creation
-  bool resid_bf16 = true;   // residual stream stored in bf16 (default; SGPT_RESID_BF16=0 at creation: fp32; default flow only)
-  float* sumsq = nullptr;
-  // LayerNorm-folded parameters per layer (library-owned)
-  std::vector<void*> wq_f, wfc_f;
-  std::vector<float*> cq, bq, cfc, bfc;
+  void* xn = nullptr;  // xb: LayerNorm output, the A operand of the QKV / c_fc GEMMs
+  bool resid_bf16 = true;   // residual stream stored in bf16 (default; SGPT_RESID_BF16=0 at creation: fp32)
   void* qkv = nullptr;
   void* attn = nullptr;
   void* ffn = nullptr;
@@ -114,37 +102,12 @@ extern "C" int sgpt_model_create(const sgpt_model_config* cfg, const sgpt_model_
   if (e == cudaSuccess) e = cudaMalloc(&m->qkv, T * d * 3 * 2);
   if (e == cudaSuccess) e = cudaMalloc(&m->attn, T * d * 2);
   if (e == cudaSuccess) e = cudaMalloc(&m->ffn, T * static_cast<size_t>(cfg->d_ff) * 2);
-  m->P = (cfg->d_model + 127) / 128;
   {
-    const char* lf = getenv("SGPT_LN_FOLD");
-    m->ln_fold = (lf != nullptr && lf[0] == '1');
     const char* rb = getenv("SGPT_RESID_BF16");
-    m->resid_bf16 = !(rb != nullptr && rb[0] == '0') && !m->ln_fold;  // default ON; SGPT_RESID_BF16=0 keeps the stream in fp32
+    m->resid_bf16 = !(rb != nullptr && rb[0] == '0');  // default ON; SGPT_RESID_BF16=0 keeps the stream in fp32
   }
-  if (e == cudaSuccess) e = cudaMalloc(&m->stats, (2 * T * m->P + static_cast<size_t>(cfg->max_batch)) * 4);
-  if (e == cudaSuccess) e = cudaMalloc(&m->sumsq, static_cast<size_t>(cfg->max_batch) * 4);
-  // fold ln_1 into the QKV projection and ln_2 (GPT-J: ln_1 again) into the MLP's first layer
-  for (int l = 0; l < cfg->n_layer && e == cudaSuccess && m->ln_fold; ++l) {
-    const sgpt_layer_weights& lw = m->layers[l];
-    const size_t ff = static_cast<size_t>(cfg->d_ff);
-    void *wq = nullptr, *wf = nullptr;
-    float *cq = nullptr, *bq = nullptr, *cf = nullptr, *bf = nullptr;
-    e = cudaMalloc(&wq, 3 * d * d * 2);
-    if (e == cudaSuccess) e = cudaMalloc(&cq, 3 * d * 4);
-    if (e == cudaSuccess) e = cudaMalloc(&bq, 3 * d * 4);
-    if (e == cudaSuccess) e = cudaMalloc(&wf, ff * d * 2);
-    if (e == cudaSuccess) e = cudaMalloc(&cf, ff * 4);
-    if (e == cudaSuccess) e = cudaMalloc(&bf, ff * 4);
-    m->wq_f.push_back(wq); m->cq.push_back(cq); m->bq.push_back(bq);
-    m->wfc_f.push_back(wf); m->cfc.push_back(cf); m->bfc.push_back(bf);
-    if (e != cudaSuccess) break;
-    const bool gptj = cfg->arch == SGPT_ARCH_GPTJ;
-    int rc = sgpt_fold_layernorm(lw.w_qkv, lw.ln1_g, lw.ln1_b, lw.b_qkv, wq, cq, bq, 3 * cfg->d_model, cfg->d_model, nullptr);
-    if (rc == SGPT_OK)
-      rc = sgpt_fold_layernorm(lw.w_fc, gptj ? lw.ln1_g : lw.ln2_g, gptj ? lw.ln1_b : lw.ln2_b, lw.b_fc, wf, cf, bf, cfg->d_ff,
-                               cfg->d_model, nullptr);
-    if (rc != SGPT_OK) e = cudaErrorUnknown;
-  }
+  // (mean, rstd) per row for ln_f, then the per-sequence sums of squares of the normalisation (sgpt_pool_ex2)
+  if (e == cudaSuccess) e = cudaMalloc(&m->stats, (2 * T + static_cast<size_t>(cfg->max_batch)) * 4);
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
   if (e == cudaSuccess && cfg->arch == SGPT_ARCH_GPTJ) {
     // create_sinusoidal_positions, HF:gptj/modeling_gptj.py:45-48: angle(p, i) = p * 10000^(-2i/rotary_dim), fp32
@@ -182,13 +145,6 @@ extern "C" void sgpt_model_destroy(sgpt_model_t m) {
   cudaFree(m->attn);
   cudaFree(m->ffn);
   cudaFree(m->stats);
-  cudaFree(m->sumsq);
-  for (void* p : m->wq_f) cudaFree(p);
-  for (void* p : m->wfc_f) cudaFree(p);
-  for (float* p : m->cq) cudaFree(p);
-  for (float* p : m->bq) cudaFree(p);
-  for (float* p : m->cfc) cudaFree(p);
-  for (float* p : m->bfc) cudaFree(p);
   cudaFree(m->rotary);
   cudaFree(m->alibi);
   delete m;
@@ -241,96 +197,46 @@ extern "C" int sgpt_encode(sgpt_model_t m, const int32_t* ids, const int32_t* po
     else SGPT_TRY(sgpt_layernorm_f32_inplace(m->resid, m->w.emb_ln_g, m->w.emb_ln_b, T, d, c.ln_eps, stream));
   }
   const int n_run = layer_idx;  // hidden_states[i] is the input of block i; hidden_states[L] is ln_f(output of block L-1)
-  if (m->ln_fold) {
-  // bf16 copy + LayerNorm partial sums of the embedded residual stream; inside the blocks the residual epilogues keep
-  // both up to date
-  SGPT_TRY(sgpt_resid_stats(m->resid, m->xn, m->stats, T, d, stream));
-  const int P = m->P;
   for (int l = 0; l < n_run && l < c.n_layer; ++l) {
     const sgpt_layer_weights& lw = m->layers[l];
     if (all_layers)  // hidden_states[l] = the residual stream entering block l (no ln_f)
-      SGPT_TRY(sgpt_pool_accumulate(m->resid, pos, cu_seqlens, nullptr, nullptr, c.ln_eps, out, nullptr, B, T, d,
-                                    base_mode, clamp_denominator, 0, /*accumulate=*/l > 0, layer_scale, stream));
-    if (c.arch == SGPT_ARCH_GPT_NEO || c.arch == SGPT_ARCH_BLOOM) {
-      // ln_1 -> q,k,v   (GPT-Neo: no q/k/v bias, un-scaled logits, local window on odd layers; BLOOM: bias, ALiBi, 1/sqrt(hd))
-      SGPT_TRY(sgpt_linear_lnfold(m->xn, d, m->wq_f[l], d, m->bq[l], m->cq[l], m->stats, P, c.ln_eps, m->qkv, 3 * d, T, 3 * d,
-                                  d, /*gelu=*/0, stream));
-      if (c.arch == SGPT_ARCH_GPT_NEO) {
-        const int window = (lw.local_attention && c.window > 0 && max_seqlen > c.window) ? c.window : 0;
-        SGPT_TRY(sgpt_attention(m->qkv, m->attn, cu_seqlens, B, T, H, hd, /*scale=*/1.0f, window, max_seqlen, nullptr, 0,
-                                stream));
-      } else {
-        SGPT_TRY(sgpt_attention(m->qkv, m->attn, cu_seqlens, B, T, H, hd, inv_sqrt_hd, 0, max_seqlen, m->alibi, 0, stream));
-      }
-      // out-proj + residual; the epilogue also emits xb / partial sums for ln_2
-      SGPT_TRY(sgpt_linear_resid_ln(m->attn, d, lw.w_o, d, lw.b_o, m->resid, m->xn, m->stats, T, d, d, stream));
-      // ln_2 -> c_fc -> gelu
-      SGPT_TRY(sgpt_linear_lnfold(m->xn, d, m->wfc_f[l], d, m->bfc[l], m->cfc[l], m->stats, P, c.ln_eps, m->ffn, ff, T, ff, d,
-                                  /*gelu=*/1, stream));
-      // c_proj + residual; xb / partial sums for the next block's ln_1 (or ln_f)
-      SGPT_TRY(sgpt_linear_resid_ln(m->ffn, ff, lw.w_proj, ff, lw.b_proj, m->resid, m->xn, m->stats, T, d, ff, stream));
-    } else {  // GPT-J: attention and MLP both read ln_1(resid); res + attn + mlp
-      SGPT_TRY(sgpt_linear_qkv_rotary_lnfold(m->xn, d, m->wq_f[l], m->bq[l], m->cq[l], m->stats, P, c.ln_eps, m->qkv, pos,
-                                             m->rotary, T, d, hd, c.rotary_dim, c.max_pos, stream));
+      SGPT_TRY(sgpt_pool_ex2(m->resid, rb, pos, cu_seqlens, nullptr, nullptr, c.ln_eps, nullptr, 0, out, nullptr, B, T, d,
+                             base_mode, clamp_denominator, 0, /*accumulate=*/l > 0, layer_scale, stream));
+    SGPT_TRY(sgpt_layernorm_ex(m->resid, rb, lw.ln1_g, lw.ln1_b, m->xn, T, d, c.ln_eps, stream));
+    if (c.arch == SGPT_ARCH_GPT_NEO) {
+      SGPT_TRY(sgpt_linear(m->xn, d, lw.w_qkv, d, lw.b_qkv, m->qkv, 3 * d, nullptr, T, 3 * d, d, SGPT_EPI_BF16, stream));
+      const int window = (lw.local_attention && c.window > 0 && max_seqlen > c.window) ? c.window : 0;
+      SGPT_TRY(sgpt_attention(m->qkv, m->attn, cu_seqlens, B, T, H, hd, /*scale=*/1.0f, window, max_seqlen, nullptr, 0,
+                              stream));
+      SGPT_TRY(sgpt_linear(m->attn, d, lw.w_o, d, lw.b_o, m->resid, d, m->resid, T, d, d, epi_resid, stream));
+      SGPT_TRY(sgpt_layernorm_ex(m->resid, rb, lw.ln2_g, lw.ln2_b, m->xn, T, d, c.ln_eps, stream));
+      SGPT_TRY(sgpt_linear(m->xn, d, lw.w_fc, d, lw.b_fc, m->ffn, ff, nullptr, T, ff, d, SGPT_EPI_GELU_BF16, stream));
+      SGPT_TRY(sgpt_linear(m->ffn, ff, lw.w_proj, ff, lw.b_proj, m->resid, d, m->resid, T, d, ff, epi_resid,
+                           stream));
+    } else if (c.arch == SGPT_ARCH_GPTJ) {
+      SGPT_TRY(sgpt_linear_qkv_rotary(m->xn, d, lw.w_qkv, m->qkv, pos, m->rotary, T, d, hd, c.rotary_dim, c.max_pos,
+                                      stream));
       SGPT_TRY(sgpt_attention(m->qkv, m->attn, cu_seqlens, B, T, H, hd, inv_sqrt_hd, 0, max_seqlen, nullptr, 0, stream));
-      SGPT_TRY(sgpt_linear_lnfold(m->xn, d, m->wfc_f[l], d, m->bfc[l], m->cfc[l], m->stats, P, c.ln_eps, m->ffn, ff, T, ff, d,
-                                  /*gelu=*/1, stream));
-      // the first of the two residual updates is a plain reduce-add; the second one sees the complete sum and emits xb / stats
-      SGPT_TRY(sgpt_linear(m->attn, d, lw.w_o, d, lw.b_o, m->resid, d, m->resid, T, d, d, SGPT_EPI_RESID_F32, stream));
-      SGPT_TRY(sgpt_linear_resid_ln(m->ffn, ff, lw.w_proj, ff, lw.b_proj, m->resid, m->xn, m->stats, T, d, ff, stream));
-    }
-  }
-  } else {
-    for (int l = 0; l < n_run && l < c.n_layer; ++l) {
-      const sgpt_layer_weights& lw = m->layers[l];
-      if (all_layers)  // hidden_states[l] = the residual stream entering block l (no ln_f)
-        SGPT_TRY(sgpt_pool_ex2(m->resid, rb, pos, cu_seqlens, nullptr, nullptr, c.ln_eps, nullptr, 0, out, nullptr, B, T, d,
-                               base_mode, clamp_denominator, 0, /*accumulate=*/l > 0, layer_scale, stream));
-      SGPT_TRY(sgpt_layernorm_ex(m->resid, rb, lw.ln1_g, lw.ln1_b, m->xn, T, d, c.ln_eps, stream));
-      if (c.arch == SGPT_ARCH_GPT_NEO) {
-        SGPT_TRY(sgpt_linear(m->xn, d, lw.w_qkv, d, lw.b_qkv, m->qkv, 3 * d, nullptr, T, 3 * d, d, SGPT_EPI_BF16, stream));
-        const int window = (lw.local_attention && c.window > 0 && max_seqlen > c.window) ? c.window : 0;
-        SGPT_TRY(sgpt_attention(m->qkv, m->attn, cu_seqlens, B, T, H, hd, /*scale=*/1.0f, window, max_seqlen, nullptr, 0,
-                                stream));
-        SGPT_TRY(sgpt_linear(m->attn, d, lw.w_o, d, lw.b_o, m->resid, d, m->resid, T, d, d, epi_resid, stream));
-        SGPT_TRY(sgpt_layernorm_ex(m->resid, rb, lw.ln2_g, lw.ln2_b, m->xn, T, d, c.ln_eps, stream));
-        SGPT_TRY(sgpt_linear(m->xn, d, lw.w_fc, d, lw.b_fc, m->ffn, ff, nullptr, T, ff, d, SGPT_EPI_GELU_BF16, stream));
-        SGPT_TRY(sgpt_linear(m->ffn, ff, lw.w_proj, ff, lw.b_proj, m->resid, d, m->resid, T, d, ff, epi_resid,
-                             stream));
-      } else if (c.arch == SGPT_ARCH_GPTJ) {
-        SGPT_TRY(sgpt_linear_qkv_rotary(m->xn, d, lw.w_qkv, m->qkv, pos, m->rotary, T, d, hd, c.rotary_dim, c.max_pos,
-                                        stream));
-        SGPT_TRY(sgpt_attention(m->qkv, m->attn, cu_seqlens, B, T, H, hd, inv_sqrt_hd, 0, max_seqlen, nullptr, 0, stream));
-        // both branches read the same ln_1 output and are accumulated into the residual stream (attn + mlp + residual)
-        SGPT_TRY(sgpt_linear(m->xn, d, lw.w_fc, d, lw.b_fc, m->ffn, ff, nullptr, T, ff, d, SGPT_EPI_GELU_BF16, stream));
-        SGPT_TRY(sgpt_linear(m->attn, d, lw.w_o, d, lw.b_o, m->resid, d, m->resid, T, d, d, epi_resid, stream));
-        SGPT_TRY(sgpt_linear(m->ffn, ff, lw.w_proj, ff, lw.b_proj, m->resid, d, m->resid, T, d, ff, epi_resid,
-                             stream));
-      } else {  // BLOOM
-        SGPT_TRY(sgpt_linear(m->xn, d, lw.w_qkv, d, lw.b_qkv, m->qkv, 3 * d, nullptr, T, 3 * d, d, SGPT_EPI_BF16, stream));
-        SGPT_TRY(sgpt_attention(m->qkv, m->attn, cu_seqlens, B, T, H, hd, inv_sqrt_hd, 0, max_seqlen, m->alibi, 0, stream));
-        SGPT_TRY(sgpt_linear(m->attn, d, lw.w_o, d, lw.b_o, m->resid, d, m->resid, T, d, d, epi_resid, stream));
-        SGPT_TRY(sgpt_layernorm_ex(m->resid, rb, lw.ln2_g, lw.ln2_b, m->xn, T, d, c.ln_eps, stream));
-        SGPT_TRY(sgpt_linear(m->xn, d, lw.w_fc, d, lw.b_fc, m->ffn, ff, nullptr, T, ff, d, SGPT_EPI_GELU_BF16, stream));
-        SGPT_TRY(sgpt_linear(m->ffn, ff, lw.w_proj, ff, lw.b_proj, m->resid, d, m->resid, T, d, ff, epi_resid,
-                             stream));
-      }
+      // both branches read the same ln_1 output and are accumulated into the residual stream (attn + mlp + residual)
+      SGPT_TRY(sgpt_linear(m->xn, d, lw.w_fc, d, lw.b_fc, m->ffn, ff, nullptr, T, ff, d, SGPT_EPI_GELU_BF16, stream));
+      SGPT_TRY(sgpt_linear(m->attn, d, lw.w_o, d, lw.b_o, m->resid, d, m->resid, T, d, d, epi_resid, stream));
+      SGPT_TRY(sgpt_linear(m->ffn, ff, lw.w_proj, ff, lw.b_proj, m->resid, d, m->resid, T, d, ff, epi_resid,
+                           stream));
+    } else {  // BLOOM
+      SGPT_TRY(sgpt_linear(m->xn, d, lw.w_qkv, d, lw.b_qkv, m->qkv, 3 * d, nullptr, T, 3 * d, d, SGPT_EPI_BF16, stream));
+      SGPT_TRY(sgpt_attention(m->qkv, m->attn, cu_seqlens, B, T, H, hd, inv_sqrt_hd, 0, max_seqlen, m->alibi, 0, stream));
+      SGPT_TRY(sgpt_linear(m->attn, d, lw.w_o, d, lw.b_o, m->resid, d, m->resid, T, d, d, epi_resid, stream));
+      SGPT_TRY(sgpt_layernorm_ex(m->resid, rb, lw.ln2_g, lw.ln2_b, m->xn, T, d, c.ln_eps, stream));
+      SGPT_TRY(sgpt_linear(m->xn, d, lw.w_fc, d, lw.b_fc, m->ffn, ff, nullptr, T, ff, d, SGPT_EPI_GELU_BF16, stream));
+      SGPT_TRY(sgpt_linear(m->ffn, ff, lw.w_proj, ff, lw.b_proj, m->resid, d, m->resid, T, d, ff, epi_resid,
+                           stream));
     }
   }
   if (pool_mode == kNoPooling) return SGPT_OK;
   const bool final_ln = (layer_idx == c.n_layer);
-  if (final_ln && m->ln_fold) {
-    // ln_f folded into the pooling kernel; its row statistics come from the partial sums the last c_proj (or the
-    // embedding, for a 0-layer run) left behind: ONE pass over the residual stream
-    SGPT_TRY(sgpt_pool_partials(m->resid, pos, cu_seqlens, m->w.lnf_g, m->w.lnf_b, c.ln_eps, pool_w, pool_w ? m->n_pool_w : 0,
-                                out, m->stats, m->P, m->sumsq, B, T, d, base_mode, clamp_denominator, normalize,
-                                /*accumulate=*/all_layers && c.n_layer > 0, layer_scale, stream));
-  } else {
-    // (the partial sums are dead after the last block: the scratch only hosts the normalisation's per-row sums here)
-    SGPT_TRY(sgpt_pool_ex2(m->resid, rb, pos, cu_seqlens, final_ln ? m->w.lnf_g : nullptr, final_ln ? m->w.lnf_b : nullptr, c.ln_eps,
-                          pool_w, pool_w ? m->n_pool_w : 0, out, m->stats, B, T, d, base_mode, clamp_denominator, normalize,
-                          /*accumulate=*/all_layers && c.n_layer > 0, layer_scale, stream));
-  }
+  SGPT_TRY(sgpt_pool_ex2(m->resid, rb, pos, cu_seqlens, final_ln ? m->w.lnf_g : nullptr, final_ln ? m->w.lnf_b : nullptr, c.ln_eps,
+                         pool_w, pool_w ? m->n_pool_w : 0, out, m->stats, B, T, d, base_mode, clamp_denominator, normalize,
+                         /*accumulate=*/all_layers && c.n_layer > 0, layer_scale, stream));
   return SGPT_OK;
 }
 

@@ -68,23 +68,16 @@ class Encoder:
         self._keep = []  # device tensors the C handle borrows
         sd = {(k[len("transformer."):] if k.startswith("transformer.") else k): v for k, v in state_dict.items()}
 
-        # SGPT_LN_FOLD=1 (csrc/model.cu): sgpt_model_create folds LayerNorm parameters, q/k/v and first-MLP-layer weights
-        # and biases into library-owned buffers; those tensors are released as soon as the handle exists
-        import os
-
-        ln_fold = os.environ.get("SGPT_LN_FOLD", "0")[:1] == "1"
-        consumed = []
-
-        def dev(t, dtype, keep=True):
+        def dev(t, dtype):
             x = t.detach().to(device=self.device, dtype=dtype).contiguous()
-            (self._keep if (keep or not ln_fold) else consumed).append(x)
+            self._keep.append(x)
             return x
 
-        def p32(name, keep=True):
-            return dev(sd[name], torch.float32, keep).data_ptr() if name in sd else None
+        def p32(name):
+            return dev(sd[name], torch.float32).data_ptr() if name in sd else None
 
-        def p16(t, keep=True):
-            return dev(t, torch.bfloat16, keep).data_ptr()
+        def p16(t):
+            return dev(t, torch.bfloat16).data_ptr()
 
         with torch.cuda.device(self.device):
             d, H, hd = cfg.d_model, cfg.n_head, cfg.head_dim
@@ -98,15 +91,14 @@ class Encoder:
                 for i in range(cfg.n_layer):
                     p, lw = f"h.{i}.", layers[i]
                     a = p + "attn.attention."
-                    lw.ln1_g, lw.ln1_b = p32(p + "ln_1.weight", False), p32(p + "ln_1.bias", False)
-                    lw.w_qkv = p16(torch.cat([sd[a + "q_proj.weight"], sd[a + "k_proj.weight"], sd[a + "v_proj.weight"]], 0),
-                                   False)
+                    lw.ln1_g, lw.ln1_b = p32(p + "ln_1.weight"), p32(p + "ln_1.bias")
+                    lw.w_qkv = p16(torch.cat([sd[a + "q_proj.weight"], sd[a + "k_proj.weight"], sd[a + "v_proj.weight"]], 0))
                     if (a + "q_proj.bias") in sd:
                         lw.b_qkv = dev(torch.cat([sd[a + "q_proj.bias"], sd[a + "k_proj.bias"], sd[a + "v_proj.bias"]], 0),
-                                       torch.float32, False).data_ptr()
+                                       torch.float32).data_ptr()
                     lw.w_o, lw.b_o = p16(sd[a + "out_proj.weight"]), p32(a + "out_proj.bias")
-                    lw.ln2_g, lw.ln2_b = p32(p + "ln_2.weight", False), p32(p + "ln_2.bias", False)
-                    lw.w_fc, lw.b_fc = p16(sd[p + "mlp.c_fc.weight"], False), p32(p + "mlp.c_fc.bias", False)
+                    lw.ln2_g, lw.ln2_b = p32(p + "ln_2.weight"), p32(p + "ln_2.bias")
+                    lw.w_fc, lw.b_fc = p16(sd[p + "mlp.c_fc.weight"]), p32(p + "mlp.c_fc.bias")
                     lw.w_proj, lw.b_proj = p16(sd[p + "mlp.c_proj.weight"]), p32(p + "mlp.c_proj.bias")
                     lw.local_attention = 1 if cfg.attention_layers[i] == "local" else 0
                 arch_id = _lib.ARCH_GPT_NEO
@@ -114,11 +106,11 @@ class Encoder:
                 mw.wte = p16(sd["wte.weight"])
                 for i in range(cfg.n_layer):
                     p, lw = f"h.{i}.", layers[i]
-                    lw.ln1_g, lw.ln1_b = p32(p + "ln_1.weight", False), p32(p + "ln_1.bias", False)
+                    lw.ln1_g, lw.ln1_b = p32(p + "ln_1.weight"), p32(p + "ln_1.bias")
                     lw.w_qkv = p16(torch.cat([sd[p + "attn.q_proj.weight"], sd[p + "attn.k_proj.weight"],
-                                              sd[p + "attn.v_proj.weight"]], 0), False)
+                                              sd[p + "attn.v_proj.weight"]], 0))
                     lw.w_o = p16(sd[p + "attn.out_proj.weight"])
-                    lw.w_fc, lw.b_fc = p16(sd[p + "mlp.fc_in.weight"], False), p32(p + "mlp.fc_in.bias", False)
+                    lw.w_fc, lw.b_fc = p16(sd[p + "mlp.fc_in.weight"]), p32(p + "mlp.fc_in.bias")
                     lw.w_proj, lw.b_proj = p16(sd[p + "mlp.fc_out.weight"]), p32(p + "mlp.fc_out.bias")
                 arch_id = _lib.ARCH_GPTJ
             else:  # bloom: keys of HF BloomModel.state_dict()
@@ -126,17 +118,17 @@ class Encoder:
                 mw.emb_ln_g, mw.emb_ln_b = p32("word_embeddings_layernorm.weight"), p32("word_embeddings_layernorm.bias")
                 for i in range(cfg.n_layer):
                     p, lw = f"h.{i}.", layers[i]
-                    lw.ln1_g, lw.ln1_b = p32(p + "input_layernorm.weight", False), p32(p + "input_layernorm.bias", False)
+                    lw.ln1_g, lw.ln1_b = p32(p + "input_layernorm.weight"), p32(p + "input_layernorm.bias")
                     # fused query_key_value rows are ordered per head [q(hd) | k(hd) | v(hd)] (HF:bloom:211-215);
                     # regroup to [q_all | k_all | v_all], the layout the attention kernel reads
                     wq = sd[p + "self_attention.query_key_value.weight"].view(H, 3, hd, d)
                     bq = sd[p + "self_attention.query_key_value.bias"].view(H, 3, hd)
-                    lw.w_qkv = p16(wq.permute(1, 0, 2, 3).reshape(3 * d, d), False)
-                    lw.b_qkv = dev(bq.permute(1, 0, 2).reshape(3 * d), torch.float32, False).data_ptr()
+                    lw.w_qkv = p16(wq.permute(1, 0, 2, 3).reshape(3 * d, d))
+                    lw.b_qkv = dev(bq.permute(1, 0, 2).reshape(3 * d), torch.float32).data_ptr()
                     lw.w_o, lw.b_o = p16(sd[p + "self_attention.dense.weight"]), p32(p + "self_attention.dense.bias")
-                    lw.ln2_g, lw.ln2_b = (p32(p + "post_attention_layernorm.weight", False),
-                                          p32(p + "post_attention_layernorm.bias", False))
-                    lw.w_fc, lw.b_fc = p16(sd[p + "mlp.dense_h_to_4h.weight"], False), p32(p + "mlp.dense_h_to_4h.bias", False)
+                    lw.ln2_g, lw.ln2_b = (p32(p + "post_attention_layernorm.weight"),
+                                          p32(p + "post_attention_layernorm.bias"))
+                    lw.w_fc, lw.b_fc = p16(sd[p + "mlp.dense_h_to_4h.weight"]), p32(p + "mlp.dense_h_to_4h.bias")
                     lw.w_proj, lw.b_proj = p16(sd[p + "mlp.dense_4h_to_h.weight"]), p32(p + "mlp.dense_4h_to_h.bias")
                 arch_id = _lib.ARCH_BLOOM
             mw.lnf_g, mw.lnf_b = p32("ln_f.weight"), p32("ln_f.bias")
@@ -148,7 +140,6 @@ class Encoder:
             handle = C.c_void_p()
             _lib.check(self._lib.sgpt_model_create(C.byref(mc), C.byref(mw), C.byref(handle)), "sgpt_model_create")
             self._handle = handle
-            consumed.clear()  # sgpt_model_create synchronises: the folded copies are complete
         # two pinned staging buffers for [ids | pos | cu] and their device twins: one H2D copy per batch, and the
         # host may pack batch i+1 while the GPU still runs batch i
         cap = 2 * self.max_tokens + self.max_batch + 1

@@ -90,6 +90,35 @@ def test_tiny_model_residual_stream_vs_reference_hidden_states(tiny_encoder):
     assert (h - ref).abs().max().item() < 0.08
 
 
+@pytest.mark.parametrize("resid_bf16", ["1", "0"])
+def test_residual_stream_dtype_flows_match_reference_fixture(golden_dir, monkeypatch, resid_bf16):
+    """The residual stream is stored in bf16 by default (what HF does for a bf16 checkpoint) and in fp32 with
+    SGPT_RESID_BF16=0: both against the HF fp32 fixture — pooled embeddings within the 1e-3 cosine bar, per-token residual
+    tap readable."""
+    from sgpt_b200 import Encoder
+
+    z = np.load(os.path.join(golden_dir, "neo_tiny.npz"))
+    spec = _spec_from(z)
+    w = gpt_neo.init_weights(spec, seed=int(z["weight_seed"]))
+    ids, mask = z["input_ids"], z["attention_mask"]
+    monkeypatch.setenv("SGPT_RESID_BF16", resid_bf16)
+    enc = Encoder(_cfg_from_spec(spec), w, device="cuda:0", max_tokens=4096, max_batch=64)
+    for method, key in (("weightedmean", "pooled_weightedmean"), ("mean", "pooled_mean")):
+        got = enc.encode_tokens(ids, mask, method=method).cpu()
+        assert min_row_cosine(got, z[key]) > 1 - 1e-3, method
+    got = enc.encode_tokens(ids, mask, method="weightedmean", layer_idx=int(z["mid_layer"])).cpu()
+    assert min_row_cosine(got, z["pooled_weightedmean_mid"]) > 1 - 1e-3
+    sp = np.load(os.path.join(golden_dir, "script_pooling_neo_tiny.npz"))
+    for method in ("meanmean", "lasttokenmean", "lasttoken"):
+        assert min_row_cosine(enc.encode_tokens(ids, mask, method=method).cpu(), sp["pooled_" + method]) > 1 - 1e-3, method
+    enc.encode_tokens(ids, mask)
+    resid = enc.last_residual().cpu()
+    h = gpt_neo.layer_norm(resid, w["ln_f.weight"], w["ln_f.bias"], spec.ln_eps)
+    ref = torch.from_numpy(z["hidden_states"][-1])[torch.from_numpy(mask).bool()]
+    assert torch.nn.functional.cosine_similarity(h.double(), ref.double(), dim=1).min().item() > 1 - 1e-3
+    enc.close()
+
+
 def test_left_padded_rows_use_padded_positions(tiny_encoder):
     """Pooling weights / position ids follow the PADDED index (Pooling.py:104-112; HF position_ids = arange(S))."""
     z, spec, w, enc = tiny_encoder
