@@ -408,6 +408,35 @@ int sgpt_search_gather_masked(int dtype, sgpt_gather_t g, const void* Q, const v
                               float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * IVF (inverted-file) search: a corpus split into nlist lists (k-means cells), of which each query scans only the
+ * `nprobe` it probes.  The search is exact relative to its lists: it returns exactly what the exact search returns over
+ * the undeleted documents of the probed lists — the same scores (the rows of C as stored: bf16 with c_scale = 1/||row||,
+ * or int8 with per-row scales, see the int8 shard section), the same order (score descending, ties by ascending GLOBAL
+ * id) and the tail (-inf, -1) when fewer than k documents are probed.  Choosing the probes (e.g. the exact top-nprobe of
+ * the centroids) is the caller's part.
+ *   dtype       SGPT_DTYPE_BF16: Q bf16[nq,D], C bf16[n,D] (D % 8 == 0); SGPT_DTYPE_I8: Q int8[nq,D], C int8[n,D]
+ *               (D % 16 == 0, D <= 65536).  q_scale [nq] / c_scale [n] as in sgpt_search (NULL = 1).  Q 16-byte aligned.
+ *   C           the rows in list order: list l is rows [list_offsets[l], list_offsets[l+1]) (int64 [nlist+1], device).
+ *               max_list_len >= every list's length (the workspace and the candidate lists are sized by it).
+ *   doc_ids     int32 [n] (device): the global id of each row; results carry these ids (< 0 = never returned).
+ *   probes      int32 [nq, nprobe] (device): the lists query q scans.  Entries outside [0, nlist) are skipped; the
+ *               entries of one query must be distinct.
+ *   mask        shared bitmap of the ALLOWED rows (row positions, the format of the masked searches, pitch 0) or NULL.
+ *   out_scores  fp32 [nq, k], out_ids int64 [nq, k] (device).
+ * Any nq (blocks of 256 queries reuse ws); no host synchronisation.  The device inputs bound every access: offsets are
+ * clamped to [0, n] and lengths to max_list_len, so inconsistent offsets or probes give wrong results, never an
+ * out-of-bounds access.  SGPT_ERR_INVALID, before any CUDA call, for an unknown dtype, nq < 0, the D rules of the dtype,
+ * nlist < 1, nprobe outside [1, nlist], k outside [1, 4096], n outside [0, 2^31), max_list_len outside [0, n],
+ * nprobe x max_list_len beyond the selection's 2^32 entries, null inputs or outputs, an unaligned Q and a workspace
+ * smaller than sgpt_ivf_search_workspace_bytes (which returns -1 for arguments the search rejects).
+ * ------------------------------------------------------------------------------------------------------------------ */
+int64_t sgpt_ivf_search_workspace_bytes(int dtype, int nq, int nlist, int nprobe, int64_t max_list_len, int D);
+int sgpt_ivf_search(int dtype, const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq,
+                    int64_t n, int D, const int64_t* list_offsets, int nlist, int64_t max_list_len,
+                    const int32_t* doc_ids, const int32_t* probes, int nprobe, int k, const uint32_t* mask,
+                    float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Residual stream in bf16 (SGPT_RESID_BF16=1 when the model handle is created; default fp32).  HF keeps hidden_states in
  * the model dtype, i.e. bf16 for the reference's bf16 configs (BASELINE configs 3-5); the `_ex` entry points take the
  * residual stream as `const void*` + a flag.  sgpt_linear(..., SGPT_EPI_RESID_BF16) adds into it with a bf16 TMA reduce.

@@ -14,7 +14,7 @@ from .config import ModelConfig, preset  # noqa: F401
 
 __all__ = ["ModelConfig", "preset", "Encoder", "CustomEmbedder", "SentenceEncoder", "SentenceBERTBOSEOS",
            "SentenceBERTAsym", "DenseRetrievalExactSearch", "CorpusShard", "merge_topk", "semantic_search",
-           "merge_topk_packed", "unpack_topk", "pack_mask", "sharded_search", "PeerGather", "ShardedDenseRetrievalExactSearch", "DenseHead", "AsymHeads", "load_st_directory", "GenericDataLoader", "EvaluateRetrieval",
+           "merge_topk_packed", "unpack_topk", "pack_mask", "IVFIndex", "sharded_search", "PeerGather", "ShardedDenseRetrievalExactSearch", "DenseHead", "AsymHeads", "load_st_directory", "GenericDataLoader", "EvaluateRetrieval",
            "InformationRetrievalEvaluator", "paraphrase_mining", "paraphrase_mining_embeddings", "community_detection"]
 
 
@@ -43,6 +43,9 @@ def __getattr__(name):  # lazy: torch / CUDA pieces are imported on first use
     if name in ("CorpusShard", "merge_topk", "merge_topk_packed", "unpack_topk", "pack_mask", "semantic_search"):
         from . import index
         return getattr(index, name)
+    if name == "IVFIndex":
+        from .ivf import IVFIndex
+        return IVFIndex
     if name in ("paraphrase_mining", "paraphrase_mining_embeddings", "community_detection"):
         from . import mining
         return getattr(mining, name)

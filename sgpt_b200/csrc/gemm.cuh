@@ -27,6 +27,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "gemm_api.h"
 
 namespace sgpt {
 
@@ -165,7 +166,12 @@ struct TileMap {
 //   row as 64 bf16, so the stage layout, TMA boxes, descriptor steps and ring are unchanged; wgmma k32 accumulates in s32,
 //   exact for |dot| < 2^31, and the accumulator is converted to fp32 where it is parked in shared memory, so every
 //   epilogue runs unchanged.
-template <int BN, class Epi, int CL = 1, bool kS8 = false>
+// kUnits: the work units are read from a table in device memory instead of being derived from (M, N) and the TileMap:
+//   unit u is ep.units[u] = (m0, m_end, n0, n_end), one 128 x BN tile at rows m0 / columns n0 whose epilogue sees only
+//   rows < m_end and columns < n_end (passed to it as M and N), and min(*ep.n_units, ep.max_units) units exist.  The
+//   count is read on the device, so the grid is fixed at launch and nothing waits for the host (the grouped IVF scan,
+//   ivf.cu).  CL = 1 and no split-K; M and N bound the tensor maps only.
+template <int BN, class Epi, int CL = 1, bool kS8 = false, bool kUnits = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, int M,
                     int N, int K, const __grid_constant__ typename Epi::Params ep, TileMap tmap) {
@@ -177,6 +183,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
   static_assert(CL == 1 || CL == 2, "work unit size");
   static_assert(Epi::kEpiWarps == 4 || Epi::kEpiWarps == 8, "4 or 8 epilogue warps");
   static_assert(BN == 128 || BN == 256, "tile width");
+  static_assert(!kUnits || CL == 1, "unit tables name single-CTA tiles");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -195,7 +202,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
   const int m_tiles = ((M + kGemmBM - 1) / kGemmBM + CL - 1) / CL;    // M-tile groups (CL tiles each)
   const int n_tiles = tmap.count((N + BN - 1) / BN);                  // N-tiles this launch visits
   const int ksplit = tmap.ksplit;
-  const int num_tiles = m_tiles * n_tiles * ksplit;  // work units
+  int num_tiles = m_tiles * n_tiles * ksplit;  // work units
   const int num_kb = (K + kBK - 1) / kBK;
   const int kb_per = (num_kb + ksplit - 1) / ksplit;  // k-blocks per slice (the host keeps every slice non-empty)
 
@@ -210,6 +217,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
   }
   __syncthreads();
   pdl_sync();  // everything above overlapped the previous kernel's tail; global memory is touched only below
+  if constexpr (kUnits) num_tiles = min(__ldg(ep.n_units), ep.max_units);
   const bool clock_probe = (blockIdx.x == 0 && threadIdx.x == 0);
   const long long probe_c0 = clock_probe ? clock64() : 0;
   const uint64_t probe_t0 = clock_probe ? global_timer_ns() : 0;
@@ -221,10 +229,17 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
       uint32_t phase = 0;
       for (int unit = cid; unit < num_tiles; unit += ncl) {
         const int tile = unit / ksplit, ks = unit - tile * ksplit;
-        int mg, nt;
-        tmap.coords(tile, m_tiles, n_tiles, mg, nt);
-        const int m0 = (mg * CL + crank) * kGemmBM;
-        const int n0 = tmap.map(nt) * BN;
+        int m0, n0;
+        if constexpr (kUnits) {
+          const int4 u = __ldg(ep.units + unit);
+          m0 = u.x;
+          n0 = u.z;
+        } else {
+          int mg, nt;
+          tmap.coords(tile, m_tiles, n_tiles, mg, nt);
+          m0 = (mg * CL + crank) * kGemmBM;
+          n0 = tmap.map(nt) * BN;
+        }
         const int kb_end = min(num_kb, (ks + 1) * kb_per);
         for (int kb = ks * kb_per; kb < kb_end; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
@@ -255,14 +270,23 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
       const int tile = unit / ksplit;
       const int ks = unit - tile * ksplit;
       if constexpr (StateHasKs<typename Epi::State>::value) st.ks = static_cast<uint32_t>(ks);
-      int mg, ntile;
-      tmap.coords(tile, m_tiles, n_tiles, mg, ntile);
-      const int m0 = (mg * CL + crank) * kGemmBM + ew * 32;  // this warp's 32-row slab
-      const int n0 = tmap.map(ntile) * BN + half * kColsPerWarp;
+      int m0, n0, Me = M, Ne = N;  // this warp's 32-row slab / column half, and the bounds its epilogue sees
+      if constexpr (kUnits) {
+        const int4 u = __ldg(ep.units + unit);
+        m0 = u.x + ew * 32;
+        n0 = u.z + half * kColsPerWarp;
+        Me = u.y;
+        Ne = u.w;
+      } else {
+        int mg, ntile;
+        tmap.coords(tile, m_tiles, n_tiles, mg, ntile);
+        m0 = (mg * CL + crank) * kGemmBM + ew * 32;
+        n0 = tmap.map(ntile) * BN + half * kColsPerWarp;
+      }
       if (epi_warp) {
         // work that does not depend on the accumulator (EpiFilterRows: the document scales and thresholds of the tile)
         // overlaps the mainloop
-        Epi::template pre_tile<kColsPerWarp, kSlabBytes>(st, ep, m0, n0, lane, stage_slab, M, N);
+        Epi::template pre_tile<kColsPerWarp, kSlabBytes>(st, ep, m0, n0, lane, stage_slab, Me, Ne);
       }
 
       Acc acc[BN / 2];
@@ -319,7 +343,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
       named_bar_sync(1, 32 * kGemmMmaWarps);
       if (epi_warp) {
         const uint32_t trow = acc_base + static_cast<uint32_t>(ew * 32 + lane) * (BN * 4) + half * kColsPerWarp * 4;
-        Epi::template tile<kColsPerWarp, kSlabBytes>(st, ep, m0, n0, lane, trow, stage_slab, M, N);
+        Epi::template tile<kColsPerWarp, kSlabBytes>(st, ep, m0, n0, lane, trow, stage_slab, Me, Ne);
       }
     }
     if (epi_warp) {
@@ -910,6 +934,97 @@ struct EpiFilterRowsT {
 };
 using EpiFilterRows = EpiFilterRowsT<false>;
 using EpiFilterRowsMasked = EpiFilterRowsT<true>;
+
+// Grouped scan of the IVF search (ivf.cu), run with kUnits: A row r is one (query, probe) pair of the query block, all
+// rows of a unit probe the same list, and the unit's columns are one 256-document tile of that list (the unit's M / N
+// bounds are the end of its pair block and of the list).  Thread = pair row, as in EpiFilterRows, with the same score
+// arithmetic — fixnan(acc * row_scale * col_scale) on the accumulator of the same mainloop — so every score has the bits
+// the exact search computes for that document.  Nothing is filtered: the thread writes (score bits, int32 global id) of
+// every document of the tile to its pair's candidate list, slot = position - first position of the list, so after all
+// tiles of the list the slots 0 .. len - 1 of the list are filled.  A position the shared bitmap excludes (deletions) is
+// written as an empty slot, id -1.  Slots are written two per 16-byte store (slot 0 is 16-byte aligned: Ls is even).
+// Params: gemm_api.h IvfRowsParams.
+struct EpiIvfRows {
+  using Params = IvfRowsParams;
+  struct State {
+    float4 cs;  // document scales n0 + 4 lane .. + 3 of the warp's half tile (broadcast by shuffles)
+    float rs;   // this row's query scale
+    int list;   // this row's candidate list
+    int begin;  // first position of the probed list
+  };
+  static constexpr int kEpiWarps = 8;
+  static constexpr int kStagingBytes = 1024;  // (none used)
+  static __device__ __forceinline__ void init(State&, const Params&) {}
+  static __device__ __forceinline__ void finish(State&, const Params&, int) {}
+  template <int COLS, int kSlabBytes>
+  static __device__ __forceinline__ void pre_tile(State& st, const Params& p, int m0, int n0, int lane, float*, int M, int N) {
+    static_assert(COLS == 128, "one float4 of document scales per lane covers the warp's half tile");
+    const int r = m0 + lane;
+    const bool rok = r < M;
+    st.rs = rok ? __ldg(p.row_scale + r) : 1.f;
+    const int2 info = rok ? __ldg(p.row_info + r) : make_int2(0, 0);
+    st.list = info.x;
+    st.begin = info.y;
+    st.cs = make_float4(1.f, 1.f, 1.f, 1.f);
+    if (m0 >= M || n0 >= N) return;  // warp-uniform: tile() writes nothing
+    const int c = n0 + 4 * lane;
+    if (p.col_scale != nullptr) {
+      st.cs.x = __ldg(p.col_scale + min(c, N - 1));
+      st.cs.y = __ldg(p.col_scale + min(c + 1, N - 1));
+      st.cs.z = __ldg(p.col_scale + min(c + 2, N - 1));
+      st.cs.w = __ldg(p.col_scale + min(c + 3, N - 1));
+    }
+    // the ids (and mask words) tile() reads once the accumulator is ready
+    if (c < N) asm volatile("prefetch.global.L1 [%0];" ::"l"(p.doc_ids + c));
+    if (p.mask != nullptr && lane < 4 && n0 + 32 * lane < N) {
+      asm volatile("prefetch.global.L1 [%0];" ::"l"(p.mask + ((n0 + 32 * lane) >> 5)));
+    }
+  }
+
+  template <int COLS, int kSlabBytes>
+  static __device__ __forceinline__ void tile(State& st, const Params& p, int m0, int n0, int lane, uint32_t trow,
+                                              float*, int M, int N) {
+    if (m0 >= M) return;  // warp-uniform
+    const bool rok = m0 + lane < M;
+    const float rs = st.rs;
+    const float csv[4] = {st.cs.x, st.cs.y, st.cs.z, st.cs.w};
+    // dst[pos] = the slot of position pos in this row's list
+    uint2* dst = p.cand + static_cast<long long>(rok ? st.list : 0) * p.Ls - st.begin;
+#pragma unroll 1
+    for (int c = 0; c < COLS; c += 32) {
+      const int n = n0 + c;
+      if (n >= N) break;  // warp-uniform
+      uint32_t v[32];
+      acc_ld_32(trow + 4 * c, v);
+      // lane i: global id of position n + i (-1 when excluded or past the list)
+      const int pos = n + lane;
+      int gid = -1;
+      if (pos < N) {
+        gid = __ldg(p.doc_ids + pos);
+        if (p.mask != nullptr && !((__ldg(p.mask + (pos >> 5)) >> (pos & 31)) & 1u)) gid = -1;
+      }
+      float cs[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) cs[i] = __shfl_sync(0xffffffffu, csv[i & 3], (c >> 2) + (i >> 2));
+      const bool full = n + 32 <= N;
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {
+        float x0 = __uint_as_float(v[i]) * rs * cs[i];
+        float x1 = __uint_as_float(v[i + 1]) * rs * cs[i + 1];
+        x0 = (x0 != x0) ? -1.f : x0;
+        x1 = (x1 != x1) ? -1.f : x1;
+        const int g0 = __shfl_sync(0xffffffffu, gid, i), g1 = __shfl_sync(0xffffffffu, gid, i + 1);
+        if (!rok) continue;
+        if (full || n + i + 1 < N) {
+          *reinterpret_cast<uint4*>(dst + n + i) =
+              make_uint4(__float_as_uint(x0), static_cast<uint32_t>(g0), __float_as_uint(x1), static_cast<uint32_t>(g1));
+        } else if (n + i < N) {
+          dst[n + i] = make_uint2(__float_as_uint(x0), static_cast<uint32_t>(g0));
+        }
+      }
+    }
+  }
+};
 
 
 template <bool kGelu>

@@ -50,4 +50,22 @@ int launch_sample_maxima(const void* Q, const void* C, const float* q_scale, con
 int launch_scores(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* scores, long long lds,
                   int nq, int n, int D, DocMask mask, bool s8, cudaStream_t stream);
 
+// Grouped scan of the IVF search (ivf.cu; gemm.cuh EpiIvfRows): the filter GEMM's mainloop (BN = kSimBN, bf16 or s8)
+// over the work units of p.units, A = rows x D gathered query rows, C = the n x D list-ordered corpus.  Launches
+// min(p.max_units, SMs) persistent CTAs; the unit count is read on the device.
+struct IvfRowsParams {
+  const int4* units;        // (m0, m_end, n0, n_end) per work unit
+  const int* n_units;       // [1] number of units (written by the unit-table kernel)
+  int max_units;            // capacity of `units`
+  const float* row_scale;   // [rows] scale of each pair row's query (1 when the scores take none)
+  const float* col_scale;   // [n] or null
+  const int2* row_info;     // [rows] (candidate list of the pair, first position of the probed list)
+  const int32_t* doc_ids;   // [n] global id of each position
+  const uint32_t* mask;     // shared bitmap of allowed positions, or null
+  uint2* cand;              // [pairs of the block][Ls]
+  long long Ls;             // entries per candidate list (even)
+};
+int launch_ivf_scan(const void* A, int rows, const void* C, int n, int D, const IvfRowsParams& p, bool s8,
+                    cudaStream_t stream);
+
 }  // namespace sgpt

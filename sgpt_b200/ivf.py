@@ -1,0 +1,237 @@
+"""Inverted-file (IVF) index over a corpus shard: k-means lists, and a search that scans only each query's nearest lists.
+
+The index splits the documents into ``nlist`` lists around k-means centroids and stores them list by list.  A query
+probes the ``nprobe`` centroids with the highest score (the exact search over the centroids: score descending, ties by
+ascending list id) and scans only the documents of those lists, with one grouped wgmma pass per probed list shared by
+every query that probes it (include/sgpt_b200.h ``sgpt_ivf_search``).
+
+The search is exact relative to its lists: ``IVFIndex.search`` returns exactly what ``CorpusShard.search`` returns over
+the undeleted documents of the probed lists — the same scores of the same stored rows, the same order and tie rule on
+global ids, the tail (-inf, -1) when fewer than k documents are probed.  ``nprobe == nlist`` is the exact search.
+Recall against the full exact search depends on the clustering only.
+"""
+from __future__ import annotations
+
+import json
+import os
+from typing import Optional, Tuple, Union
+
+import numpy as np
+import torch
+
+from . import _lib
+from .index import CorpusShard, _bit_slice, _check_score_function, unpack_mask
+
+FORMAT = "sgpt_b200.IVFIndex/1"
+_ASSIGN_BYTES = 256 << 20  # score matrix of one assignment batch (dense search over the centroids)
+
+
+def _rows_f32(shard: CorpusShard, pos: torch.Tensor) -> torch.Tensor:
+    """fp32 rows of the shard at positions `pos` as stored (int8: dequantized with the per-row scale)."""
+    v = shard.vectors.index_select(0, pos).float()
+    if shard.dtype == "int8":
+        v.mul_(shard.scales.index_select(0, pos)[:, None])
+    return v
+
+
+def _assign(cshard: CorpusShard, x: torch.Tensor, score_function: str) -> torch.Tensor:
+    """Best centroid of every row of x (exact search, k = 1), int64 [m] on the device."""
+    step = max(1, min(65536, _ASSIGN_BYTES // (4 * max(cshard.n, 1))))
+    out = [cshard.search(x[i:i + step], 1, score_function)[1][:, 0] for i in range(0, x.shape[0], step)]
+    return torch.cat(out) if out else torch.empty(0, dtype=torch.int64, device=x.device)
+
+
+class IVFIndex:
+    """IVF index on one GPU.  Built by ``IVFIndex.build`` or ``IVFIndex.load``.
+
+    ``shard`` is a ``CorpusShard`` of the rows in list order whose ids are the positions (0 .. n-1); list l is positions
+    ``offsets[l] .. offsets[l+1]`` and ``ids[pos]`` (int32) the global id of position pos.  ``centroids`` fp32
+    [nlist, D] are searched as a bf16 shard to choose the probes.  Deletions live in the inner shard's bitmap."""
+
+    def __init__(self, shard: CorpusShard, centroids: torch.Tensor, offsets: torch.Tensor, ids: torch.Tensor,
+                 id_base: int, score_function: str):
+        _check_score_function(score_function)
+        self.shard, self.score_function, self.id_base = shard, score_function, int(id_base)
+        self.device = shard.device
+        self.centroids = centroids.to(self.device, torch.float32).contiguous()
+        self.offsets = offsets.to(self.device, torch.int64).contiguous()
+        self.ids = ids.to(self.device, torch.int32).contiguous()
+        self.nlist, self.dim, self.n, self.dtype = self.centroids.shape[0], shard.dim, shard.n, shard.dtype
+        self.list_sizes = (self.offsets[1:] - self.offsets[:-1]).cpu()
+        self.max_list_len = int(self.list_sizes.max()) if self.nlist else 0
+        self._cshard = CorpusShard.from_embeddings(self.centroids, device=self.device)
+        # position of every global id (ids are a permutation of id_base .. id_base + n - 1)
+        self._pos = torch.empty(self.n, dtype=torch.int64, device=self.device)
+        self._pos[self.ids.long() - self.id_base] = torch.arange(self.n, device=self.device)
+        self._ws: Optional[torch.Tensor] = None
+
+    # ---- construction -------------------------------------------------------------------------------------------
+    @classmethod
+    def build(cls, source: Union[CorpusShard, torch.Tensor], nlist: int, score_function: str = "cos_sim",
+              dtype: Optional[str] = None, n_iter: int = 10, train_size: Optional[int] = None, seed: int = 0,
+              device=None) -> "IVFIndex":
+        """k-means lists over ``source`` (a ``CorpusShard``, or fp32/bf16 embeddings [n, D] stored as a ``dtype`` shard
+        first, "bf16" by default; a shard's own dtype is kept) and a list-ordered copy of its stored rows.
+
+        k-means runs on ``train_size`` rows (default min(n, 64 nlist)) drawn with ``seed``: assignment is the library's
+        exact search (k = 1) against the centroids as a bf16 shard, the update is the mean of the assigned rows summed in
+        fp64 on the host in row order (no atomics), and an empty list is re-seeded with a row drawn from the same seeded
+        generator.  For cos_sim the training rows are normalized first (spherical k-means).  The same inputs and seed give
+        bit-identical centroids, offsets and ids on the same device.  Every row then goes to its best centroid; the rows
+        keep their stored bits (a source shard's rows and scales are copied, not re-quantized), so scores equal the
+        source's.  A source shard's deletions carry over.
+
+        Peak device memory: the source plus the index (rows, scales, int32 ids, centroids), plus one batch of dequantized
+        rows and its centroid scores (~256 MB) during the assignment."""
+        _check_score_function(score_function)
+        if isinstance(source, CorpusShard):
+            if dtype is not None and dtype != source.dtype:
+                raise ValueError(f"dtype {dtype!r} differs from the source shard's {source.dtype!r}")
+            src = source
+        else:
+            src = CorpusShard.from_embeddings(torch.as_tensor(source), device=device, dtype=dtype or "bf16")
+        n, D, dev = src.n, src.dim, src.device
+        nlist = int(nlist)
+        if not 1 <= nlist <= n:
+            raise ValueError(f"nlist={nlist} must lie in [1, n={n}]")
+        if src.id_base < 0 or src.id_base + n >= 2 ** 31:
+            raise ValueError("global ids must fit in int32 (id_base + n < 2^31)")
+        cos = score_function == "cos_sim"
+        g = torch.Generator().manual_seed(int(seed))
+        T = min(n, int(train_size) if train_size is not None else 64 * nlist)
+        if T < nlist:
+            raise ValueError(f"train_size={T} is below nlist={nlist}")
+        sample = torch.randperm(n, generator=g)[:T].to(dev)
+        x = _rows_f32(src, sample)
+        if cos:
+            x = torch.nn.functional.normalize(x, dim=1)
+        cent = x[:nlist].clone()
+        step = max(1, (64 << 20) // (8 * D))  # rows per host transfer of the update
+        for _ in range(int(n_iter)):
+            a = _assign(CorpusShard.from_embeddings(cent, device=dev), x, score_function).cpu()
+            sums = torch.zeros(nlist, D, dtype=torch.float64)
+            for i in range(0, T, step):  # index_add_ on the host adds the rows in order: reproducible bits
+                sums.index_add_(0, a[i:i + step], x[i:i + step].cpu().double())
+            counts = torch.bincount(a, minlength=nlist)
+            new = sums / counts.clamp(min=1)[:, None].double()
+            empty = (counts == 0).nonzero().flatten()
+            if len(empty):
+                new[empty] = x[torch.randint(T, (len(empty),), generator=g).to(dev)].double().cpu()
+            if cos:
+                new = torch.nn.functional.normalize(new, dim=1)
+            cent = new.float().to(dev)
+        del x
+        cshard = CorpusShard.from_embeddings(cent, device=dev)
+        bs = max(1, min(65536, _ASSIGN_BYTES // (4 * D)))
+        assign = torch.cat([_assign(cshard, _rows_f32(src, torch.arange(i, min(i + bs, n), device=dev)), score_function)
+                            for i in range(0, n, bs)])
+        perm = torch.sort(assign, stable=True).indices
+        offsets = torch.zeros(nlist + 1, dtype=torch.int64, device=dev)
+        torch.cumsum(torch.bincount(assign, minlength=nlist), 0, out=offsets[1:])
+        inner = CorpusShard(D, n, device=dev, dtype=src.dtype)
+        torch.index_select(src.vectors[:n], 0, perm, out=inner.vectors[:n])
+        if src.dtype == "int8":
+            torch.index_select(src.scales[:n], 0, perm, out=inner.scales[:n])
+            torch.index_select(src.cos_scales[:n], 0, perm, out=inner.cos_scales[:n])
+        else:
+            torch.index_select(src.inv_norms[:n], 0, perm, out=inner.inv_norms[:n])
+        inner.n = n
+        if src._deleted["any"]:
+            deleted = unpack_mask(_bit_slice(src._deleted["words"], src._deleted_at, n), n)
+            inner.remove(deleted[perm].nonzero().flatten())
+        return cls(inner, cent, offsets, (perm + src.id_base).to(torch.int32), src.id_base, score_function)
+
+    # ---- search -------------------------------------------------------------------------------------------------
+    def probe(self, queries: torch.Tensor, nprobe: int) -> torch.Tensor:
+        """The ``nprobe`` lists each query scans: int32 [Q, nprobe], best centroid first (score descending, ties by
+        ascending list id), from the exact search over the centroids."""
+        if not 1 <= int(nprobe) <= self.nlist:
+            raise ValueError(f"nprobe={nprobe} must lie in [1, nlist={self.nlist}]")
+        return self._cshard.search(queries.to(self.device), int(nprobe), self.score_function)[1].to(torch.int32)
+
+    def search(self, queries: torch.Tensor, k: int, nprobe: int) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Top-k of the undeleted documents in each query's ``nprobe`` probed lists, for fp32/bf16 queries [Q, D]:
+        (scores fp32 [Q, k] descending, global ids int64 [Q, k]), tail (-inf, -1) when fewer than k are probed.  Scores,
+        order and ties are those of ``CorpusShard.search`` on the same stored rows."""
+        if not 1 <= int(k) <= 4096:
+            raise ValueError(f"k={k} must lie in [1, 4096]")
+        probes = self.probe(queries, nprobe)
+        qb, q_scale, c_scale = self.shard._queries(queries, self.score_function)
+        nq = qb.shape[0]
+        mask, _ = self.shard._mask(None, nq)
+        dt = self.shard._dtype_id()
+        lib = _lib.lib()
+        need = lib.sgpt_ivf_search_workspace_bytes(dt, nq, self.nlist, int(nprobe), self.max_list_len, self.dim)
+        if need < 0:
+            raise ValueError(f"sgpt_ivf_search rejects nq={nq} nprobe={nprobe}: {lib.sgpt_last_error().decode()}")
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+        out_s = torch.empty((nq, k), dtype=torch.float32, device=self.device)
+        out_i = torch.empty((nq, k), dtype=torch.int64, device=self.device)
+        with torch.cuda.device(self.device):
+            rc = lib.sgpt_ivf_search(dt, qb.data_ptr(), self.shard.vectors.data_ptr(), _lib.ptr(q_scale), c_scale, nq,
+                                     self.n, self.dim, self.offsets.data_ptr(), self.nlist, self.max_list_len,
+                                     self.ids.data_ptr(), probes.data_ptr(), int(nprobe), int(k), _lib.ptr(mask),
+                                     out_s.data_ptr(), out_i.data_ptr(), self._ws.data_ptr(), self._ws.numel(),
+                                     _lib.current_stream())
+        _lib.check(rc, "sgpt_ivf_search")
+        return out_s, out_i
+
+    def remove(self, ids) -> None:
+        """Delete documents by global id: no search returns them afterwards."""
+        ids = torch.as_tensor(ids, dtype=torch.int64).to(self.device).reshape(-1)
+        if ids.numel() == 0:
+            return
+        local = ids - self.id_base
+        if bool(((local < 0) | (local >= self.n)).any()):
+            raise ValueError(f"remove: ids must lie in [{self.id_base}, {self.id_base + self.n})")
+        self.shard.remove(self._pos[local])
+
+    @property
+    def n_deleted(self) -> int:
+        return self.shard.n_deleted
+
+    # ---- persistence --------------------------------------------------------------------------------------------
+    def save(self, path: str) -> None:
+        """One directory: the inner shard (``shard/``, deletions included) plus centroids.npy (fp32 [nlist, D]),
+        offsets.npy (int64 [nlist + 1]), ids.npy (int32 [n]) and meta.json."""
+        os.makedirs(path, exist_ok=True)
+        self.shard.save(os.path.join(path, "shard"))
+        np.save(os.path.join(path, "centroids.npy"), self.centroids.cpu().numpy())
+        np.save(os.path.join(path, "offsets.npy"), self.offsets.cpu().numpy())
+        np.save(os.path.join(path, "ids.npy"), self.ids.cpu().numpy())
+        with open(os.path.join(path, "meta.json"), "w") as f:
+            json.dump({"format": FORMAT, "dtype": self.dtype, "dim": self.dim, "n": self.n, "nlist": self.nlist,
+                       "id_base": self.id_base, "score_function": self.score_function, "shard": "shard"}, f)
+
+    @classmethod
+    def load(cls, path: str, device="cuda:0") -> "IVFIndex":
+        """Reload an index written by ``save`` (identical search bits).  Shapes, offset monotonicity and the id range
+        are checked on the host before anything is allocated on the device."""
+        with open(os.path.join(path, "meta.json")) as f:
+            meta = json.load(f)
+        if meta.get("format") != FORMAT:
+            raise ValueError(f"{path}: not an IVFIndex directory ({meta})")
+        n, dim, nlist, id_base = int(meta["n"]), int(meta["dim"]), int(meta["nlist"]), int(meta["id_base"])
+        _check_score_function(meta["score_function"])
+        cent = np.load(os.path.join(path, "centroids.npy"))
+        offsets = np.load(os.path.join(path, "offsets.npy"))
+        ids = np.load(os.path.join(path, "ids.npy"))
+        if nlist < 1 or cent.shape != (nlist, dim) or cent.dtype != np.float32:
+            raise ValueError(f"{path}: centroids {cent.shape}/{cent.dtype} do not match meta {meta}")
+        if offsets.shape != (nlist + 1,) or offsets.dtype != np.int64:
+            raise ValueError(f"{path}: offsets {offsets.shape}/{offsets.dtype} do not match meta {meta}")
+        if offsets[0] != 0 or offsets[-1] != n or bool((np.diff(offsets) < 0).any()):
+            raise ValueError(f"{path}: offsets must rise monotonically from 0 to n={n}")
+        if ids.shape != (n,) or ids.dtype != np.int32:
+            raise ValueError(f"{path}: ids {ids.shape}/{ids.dtype} do not match meta {meta}")
+        if n and (int(ids.min()) < id_base or int(ids.max()) >= id_base + n or len(np.unique(ids)) != n):
+            raise ValueError(f"{path}: ids must be a permutation of [{id_base}, {id_base + n})")
+        shard_dir = os.path.join(path, meta.get("shard", "shard"))
+        with open(os.path.join(shard_dir, "meta.json")) as f:
+            smeta = json.load(f)
+        if (int(smeta.get("n", -1)), int(smeta.get("dim", -1)), smeta.get("dtype")) != (n, dim, meta["dtype"]):
+            raise ValueError(f"{path}: inner shard {smeta} does not match meta {meta}")
+        shard = CorpusShard.load(shard_dir, device=device)
+        return cls(shard, torch.from_numpy(cent), torch.from_numpy(offsets), torch.from_numpy(ids), id_base,
+                   meta["score_function"])
