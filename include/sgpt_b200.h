@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define SGPT_ABI_VERSION 3  /* 3: sgpt_topk_merge_packed requires sorted input lists; sgpt_debug_topk_timeline added */
+#define SGPT_ABI_VERSION 4  /* 4: the embed / layernorm / pool entry points changed signature (one per operation) */
 
 #define SGPT_OK 0
 #define SGPT_ERR_INVALID 1     /* bad argument / unsupported shape */
@@ -40,38 +40,38 @@ const char* sgpt_last_error(void);
  * are packed back to back into T = sum(len_b) rows ("tokens"); padding never exists on the device.
  * ------------------------------------------------------------------------------------------------------------------ */
 
-/* F1. resid[t,:] = wte[ids[t],:] (+ wpe[pos[t],:] if wpe != NULL)       HF:gpt_neo/modeling_gpt_neo.py:462-463
- *     ids,pos int32[T]; wte bf16[vocab,d]; wpe bf16[max_pos,d] or NULL (GPT-J / BLOOM); resid fp32[T,d]. */
-int sgpt_embed_tokens(const int32_t* ids, const int32_t* pos, const void* wte, const void* wpe, float* resid,
-                      int T, int d, int vocab, int max_pos, sgpt_stream_t stream);
+/* The residual stream is bf16: HF keeps hidden_states in the model dtype, i.e. bf16 for the reference's bf16 configs
+ * (BASELINE configs 3-5).  The embedding writes it, LayerNorm reads it, and sgpt_linear(..., SGPT_EPI_RESID_BF16) adds
+ * into it with a bf16 TMA reduce.  Sums and statistics are fp32. */
+
+/* F1. resid[t,:] = bf16(wte[ids[t],:] (+ wpe[pos[t],:] if wpe != NULL))       HF:gpt_neo/modeling_gpt_neo.py:462-463
+ *     ids,pos int32[T]; wte bf16[vocab,d]; wpe bf16[max_pos,d] or NULL (GPT-J / BLOOM); resid bf16[T,d]. */
+int sgpt_embed_tokens(const int32_t* ids, const int32_t* pos, const void* wte, const void* wpe, void* resid, int T,
+                      int d, int vocab, int max_pos, sgpt_stream_t stream);
 
 /* F2/F7. y = LayerNorm(x; gamma, beta, eps) row-wise, fp32 statistics, bf16 output.   HF:gpt_neo/...:332,345,492
- *     x fp32[T,d]; gamma,beta fp32[d]; y bf16[T,d]. */
-int sgpt_layernorm(const float* x, const float* gamma, const float* beta, void* y, int T, int d, float eps,
+ *     x bf16[T,d]; gamma,beta fp32[d]; y bf16[T,d]; y may alias x (BLOOM word_embeddings_layernorm runs in place,
+ *     HF:bloom/modeling_bloom.py:496). */
+int sgpt_layernorm(const void* x, const float* gamma, const float* beta, void* y, int T, int d, float eps,
                    sgpt_stream_t stream);
 
 /* F3/F5/F6. y = epilogue(x @ w^T + bias).   torch.nn.Linear call sites HF:gpt_neo/...:84-87,153,295-309
  *     x bf16[M,K] (row pitch ldx), w bf16[N,K] (nn.Linear weight layout, row pitch ldw), bias fp32[N] or NULL.
  *     epilogue: SGPT_EPI_BF16       out bf16[M,N]  = acc + bias
  *               SGPT_EPI_GELU_BF16  out bf16[M,N]  = gelu_new(acc + bias)       (HF activations.py NewGELUActivation)
- *               SGPT_EPI_RESID_F32  out fp32[M,N]  = resid + acc + bias         (resid fp32[M,N] with row pitch ldo,
- *                                                                                may alias out; unchanged if it does not)
+ *               SGPT_EPI_RESID_BF16 out bf16[M,N] += acc + bias                 (in place: resid == out, the residual
+ *                                                                                stream)
  *     Runs on the wgmma tensor cores (TMA-staged tiles, register accumulators). */
 #define SGPT_EPI_BF16 0
 #define SGPT_EPI_GELU_BF16 1
-#define SGPT_EPI_RESID_F32 2
-#define SGPT_EPI_RESID_BF16 3 /* out bf16[M,N] += acc + bias, in place (resid == out): bf16 residual stream */
+#define SGPT_EPI_RESID_BF16 3
 int sgpt_linear(const void* x, int64_t ldx, const void* w, int64_t ldw, const float* bias, void* out, int64_t ldo,
-                const float* resid, int M, int N, int K, int epilogue, sgpt_stream_t stream);
+                const void* resid, int M, int N, int K, int epilogue, sgpt_stream_t stream);
 
 /* F7'. y[m,:] = LayerNorm(x[rows[m],:]) for a gathered subset of rows (bf16 out): the LM-head input of
- *      sgpt_lm_logprobs.  x fp32[T,d]; rows int32[M] (values in [0,T)); y bf16[M,d]. */
-int sgpt_layernorm_gather(const float* x, const int32_t* rows, const float* gamma, const float* beta, void* y, int M,
+ *      sgpt_lm_logprobs.  x bf16[T,d]; rows int32[M] (values in [0,T)); y bf16[M,d]. */
+int sgpt_layernorm_gather(const void* x, const int32_t* rows, const float* gamma, const float* beta, void* y, int M,
                           int d, float eps, sgpt_stream_t stream);
-
-/* F2'. In-place fp32 LayerNorm (BLOOM word_embeddings_layernorm, HF:bloom/modeling_bloom.py:496): x fp32[T,d]. */
-int sgpt_layernorm_f32_inplace(float* x, const float* gamma, const float* beta, int T, int d, float eps,
-                               sgpt_stream_t stream);
 
 /* F3'. GPT-J fused q/k/v projection with rotary position embedding in the epilogue
  *     (HF:gptj/modeling_gptj.py:98-101 bias-free projections, :55-67 + :196-207 rotary on the first rotary_dim dims of
@@ -95,11 +95,20 @@ int sgpt_attention(const void* qkv, void* out, const int32_t* cu_seqlens, int B,
 /* ------------------------------------------------------------------------------------------------------------------
  * P1/P2. Pooling over the ragged sequence dimension, fp32 accumulate.
  *     BDR:258-270 == ST/models/Pooling.py:99-125 (weightedmean), BDR:238-242 (mean), BDR:271-282 (lasttoken)
- *     x fp32[T,d] (residual stream or hidden state); pos int32[T] = index of the token in its *padded* row
- *     (weight of token t is pos[t]+1 for weightedmean); out fp32[B,d].
+ *     x bf16[T,d] (x_bf16 = 1: the residual stream) or fp32[T,d] (x_bf16 = 0: a hidden state); pos int32[T] = index
+ *     of the token in its *padded* row (weight of token t is pos[t]+1 for weightedmean); out fp32[B,d].
  *     If gamma != NULL the final LayerNorm (ln_f, F7) is applied to every row on the fly before it is pooled.
  *     clamp_denominator != 0 reproduces ST's clamp(min=1e-9) (Pooling.py:122); 0 reproduces the script (no clamp).
  *     normalize != 0 additionally L2-normalises each output row (ST/models/Normalize.py:13-14).
+ *     row_stats_ws: fp32[2*T + B] scratch, needed with gamma or normalize (else may be NULL).
+ *     pos_weights: fp32[n_pos_weights] or NULL.  With a table (mode must be WEIGHTEDMEAN) the weight of token t is
+ *     pos_weights[pos[t]] instead of pos[t]+1 — the learnt per-position weights of ST/models/WeightedMeanPooling.py:21-37
+ *     (`position_weights[:positions]`, indexed by the position in the padded row; that module always clamps the
+ *     denominator, :34).  pos[t] >= n_pos_weights is the caller's error (the reference asserts, :30); the kernel clamps
+ *     the index instead of reading out of bounds.
+ *     out = (accumulate ? out : 0) + out_scale * pool(x): the building block of the all-hidden-state modes below; mode
+ *     is one of MEAN / WEIGHTEDMEAN / LASTTOKEN; normalize (if set) acts on the accumulated rows, so pass it with the
+ *     last state.
  * ------------------------------------------------------------------------------------------------------------------ */
 #define SGPT_POOL_MEAN 0
 #define SGPT_POOL_WEIGHTEDMEAN 1
@@ -110,24 +119,10 @@ int sgpt_attention(const void* qkv, void* out, const int32_t* cu_seqlens, int B,
  * the reference. */
 #define SGPT_POOL_MEANMEAN 3
 #define SGPT_POOL_LASTTOKENMEAN 4
-int sgpt_pool(const float* x, const int32_t* pos, const int32_t* cu_seqlens, const float* gamma, const float* beta,
-              float eps, float* out, float* row_stats_ws /* fp32[2*T] scratch */, int B, int T, int d, int mode,
-              int clamp_denominator, int normalize, sgpt_stream_t stream);
-/* Building block of the all-hidden-state modes: out = (accumulate ? out : 0) + out_scale * pool(x); mode is one of
- * MEAN / WEIGHTEDMEAN / LASTTOKEN; normalize (if set) acts on the accumulated rows, so pass it with the last state. */
-int sgpt_pool_accumulate(const float* x, const int32_t* pos, const int32_t* cu_seqlens, const float* gamma,
-                         const float* beta, float eps, float* out, float* row_stats_ws, int B, int T, int d, int mode,
-                         int clamp_denominator, int normalize, int accumulate, float out_scale, sgpt_stream_t stream);
-
-/* General form: pos_weights fp32[n_pos_weights] or NULL.  With a table (mode must be WEIGHTEDMEAN) the weight of token t
- * is pos_weights[pos[t]] instead of pos[t]+1 — the learnt per-position weights of
- * ST/models/WeightedMeanPooling.py:21-37 (`position_weights[:positions]`, indexed by the position in the padded row;
- * that module always clamps the denominator, :34).  pos[t] >= n_pos_weights is the caller's error (the reference
- * asserts, :30); the kernel clamps the index instead of reading out of bounds. */
-int sgpt_pool_ex(const float* x, const int32_t* pos, const int32_t* cu_seqlens, const float* gamma, const float* beta,
-                 float eps, const float* pos_weights, int n_pos_weights, float* out, float* row_stats_ws, int B, int T,
-                 int d, int mode, int clamp_denominator, int normalize, int accumulate, float out_scale,
-                 sgpt_stream_t stream);
+int sgpt_pool(const void* x, int x_bf16, const int32_t* pos, const int32_t* cu_seqlens, const float* gamma,
+              const float* beta, float eps, const float* pos_weights, int n_pos_weights, float* out, float* row_stats_ws,
+              int B, int T, int d, int mode, int clamp_denominator, int normalize, int accumulate, float out_scale,
+              sgpt_stream_t stream);
 
 /* Sentence-embedding head applied after pooling: y = act(x @ w^T + bias), all fp32 (ST/models/Dense.py:40-43 with
  * key_name "sentence_embedding"; nn.Linear weight layout).  x fp32[B,in], w fp32[out,in], bias fp32[out] or NULL,
@@ -208,7 +203,7 @@ int sgpt_encode(sgpt_model_t m, const int32_t* ids, const int32_t* pos, const in
  * ------------------------------------------------------------------------------------------------------------------ */
 
 /* The GPT forward pass alone (F1..F6 of every block): replaces `model(inps)` at sgptce.py:76-83 up to the final
- * LayerNorm.  Leaves the fp32 residual stream [T,d] in the handle for sgpt_lm_logprobs / sgpt_model_read_residual. */
+ * LayerNorm.  Leaves the bf16 residual stream [T,d] in the handle for sgpt_lm_logprobs / sgpt_model_read_residual. */
 int sgpt_forward(sgpt_model_t m, const int32_t* ids, const int32_t* pos, const int32_t* cu_seqlens, int B, int T,
                  int max_seqlen, sgpt_stream_t stream);
 
@@ -235,8 +230,8 @@ int sgpt_segment_sum(const float* x, const int32_t* offsets, int R, float* out, 
  * SGPT_ERR_INVALID when max_seqlen > n, like the reference's shape assert (:30). */
 int sgpt_model_set_position_weights(sgpt_model_t m, const float* w, int n);
 
-/* Debug/parity tap: copies the fp32 residual stream (hidden_states[layer] before ln_f) left by the LAST sgpt_encode
- * into dst (device, capacity_elems floats) and reports its shape. */
+/* Debug/parity tap: copies the residual stream (hidden_states[layer] before ln_f) left by the LAST sgpt_encode, widened
+ * to fp32, into dst (device, capacity_elems floats) and reports its shape. */
 int sgpt_model_read_residual(sgpt_model_t m, float* dst, int64_t capacity_elems, int* T, int* d, sgpt_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
@@ -436,21 +431,7 @@ int sgpt_ivf_search(int dtype, const void* Q, const void* C, const float* q_scal
                     const int32_t* doc_ids, const int32_t* probes, int nprobe, int k, const uint32_t* mask,
                     float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
 
-/* ------------------------------------------------------------------------------------------------------------------
- * Residual stream in bf16 (SGPT_RESID_BF16=1 when the model handle is created; default fp32).  HF keeps hidden_states in
- * the model dtype, i.e. bf16 for the reference's bf16 configs (BASELINE configs 3-5); the `_ex` entry points take the
- * residual stream as `const void*` + a flag.  sgpt_linear(..., SGPT_EPI_RESID_BF16) adds into it with a bf16 TMA reduce.
- * ------------------------------------------------------------------------------------------------------------------ */
-int sgpt_embed_tokens_ex(const int32_t* ids, const int32_t* pos, const void* wte, const void* wpe, void* resid, int T,
-                         int d, int vocab, int max_pos, int resid_bf16, sgpt_stream_t stream);
-int sgpt_layernorm_ex(const void* x, int x_bf16, const float* gamma, const float* beta, void* y, int T, int d, float eps,
-                      sgpt_stream_t stream);
-int sgpt_layernorm_gather_ex(const void* x, int x_bf16, const int32_t* row_idx, const float* gamma, const float* beta,
-                             void* y, int M, int d, float eps, sgpt_stream_t stream);
-int sgpt_pool_ex2(const void* x, int x_bf16, const int32_t* pos, const int32_t* cu_seqlens, const float* gamma,
-                  const float* beta, float eps, const float* pos_weights, int n_pos_weights, float* out,
-                  float* row_stats_ws, int B, int T, int d, int mode, int clamp_denominator, int normalize,
-                  int accumulate, float out_scale, sgpt_stream_t stream);
+/* bf16 -> fp32 conversion of count elements (count % 4 == 0), e.g. of the residual stream. */
 int sgpt_bf16_to_f32(const void* x, float* y, int64_t count, sgpt_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------

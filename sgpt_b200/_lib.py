@@ -14,7 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SGPT_B200_LIB") or os.path.join(_HERE, "libsgpt_b200.so")
 
 SGPT_OK = 0
-EPI_BF16, EPI_GELU_BF16, EPI_RESID_F32, EPI_RESID_BF16 = 0, 1, 2, 3
+EPI_BF16, EPI_GELU_BF16, EPI_RESID_BF16 = 0, 1, 3
 POOL_MEAN, POOL_WEIGHTEDMEAN, POOL_LASTTOKEN, POOL_MEANMEAN, POOL_LASTTOKENMEAN = 0, 1, 2, 3, 4
 ARCH_GPT_NEO, ARCH_GPTJ, ARCH_BLOOM = 0, 1, 2
 ACT_IDENTITY, ACT_TANH, ACT_RELU, ACT_SIGMOID = 0, 1, 2, 3
@@ -44,13 +44,10 @@ _SIGNATURES = {
     "sgpt_last_error": (C.c_char_p, []),
     "sgpt_embed_tokens": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]),
     "sgpt_layernorm": (i32, [vp, vp, vp, vp, i32, i32, f32, vp]),
-    "sgpt_layernorm_f32_inplace": (i32, [vp, vp, vp, i32, i32, f32, vp]),
     "sgpt_linear_qkv_rotary": (i32, [vp, i64, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
     "sgpt_linear": (i32, [vp, i64, vp, i64, vp, vp, i64, vp, i32, i32, i32, i32, vp]),
     "sgpt_attention": (i32, [vp, vp, vp, i32, i32, i32, i32, f32, i32, i32, vp, i32, vp]),
-    "sgpt_pool": (i32, [vp, vp, vp, vp, vp, f32, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
-    "sgpt_pool_accumulate": (i32, [vp, vp, vp, vp, vp, f32, vp, vp, i32, i32, i32, i32, i32, i32, i32, f32, vp]),
-    "sgpt_pool_ex": (i32, [vp, vp, vp, vp, vp, f32, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32, f32, vp]),
+    "sgpt_pool": (i32, [vp, i32, vp, vp, vp, vp, f32, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32, f32, vp]),
     "sgpt_normalize_rows": (i32, [vp, i32, i32, vp]),
     "sgpt_dense": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, vp]),
     "sgpt_model_set_position_weights": (i32, [vp, vp, i32]),
@@ -76,10 +73,6 @@ _SIGNATURES = {
     "sgpt_profile_gemm_clock": (i32, [vp, vp]),
     "sgpt_debug_topk_timeline": (i32, [vp, i32]),
     "sgpt_search": (i32, [vp, vp, vp, vp, i32, i64, i32, i32, i64, vp, vp, vp, i64, vp]),
-    "sgpt_embed_tokens_ex": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
-    "sgpt_layernorm_ex": (i32, [vp, i32, vp, vp, vp, i32, i32, f32, vp]),
-    "sgpt_layernorm_gather_ex": (i32, [vp, i32, vp, vp, vp, vp, i32, i32, f32, vp]),
-    "sgpt_pool_ex2": (i32, [vp, i32, vp, vp, vp, vp, f32, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32, f32, vp]),
     "sgpt_bf16_to_f32": (i32, [vp, vp, i64, vp]),
     "sgpt_search_packed": (i32, [vp, vp, vp, vp, i32, i64, i32, i32, i64, vp, vp, i64, vp]),
     "sgpt_topk_merge_packed": (i32, [vp, i32, i32, i32, vp, vp, vp, vp]),
@@ -107,7 +100,7 @@ _SIGNATURES = {
 }
 DTYPE_BF16, DTYPE_I8 = 0, 1
 
-ABI_VERSION = 3  # include/sgpt_b200.h SGPT_ABI_VERSION these signatures / struct layouts were written for
+ABI_VERSION = 4  # include/sgpt_b200.h SGPT_ABI_VERSION these signatures / struct layouts were written for
 IPC_HANDLE_BYTES = 64
 
 _lib: Optional[C.CDLL] = None

@@ -2,7 +2,6 @@
 // position-weighted masked pooling with ln_f fused in (P1/P2).  All reductions accumulate in fp32; all global
 // accesses are 16-byte vectorised and coalesced along d.
 #include <math.h>
-#include <stdlib.h>
 
 #include "../../include/sgpt_b200.h"
 #include "common.cuh"
@@ -10,23 +9,25 @@
 
 namespace sgpt {
 
-// Four consecutive elements of a residual-stream row: the stream is fp32 (default) or bf16 (SGPT_RESID_BF16=1, the storage
-// the reference's own bf16 checkpoints use: HF keeps hidden_states in the model dtype).  idx4 counts groups of 4 elements.
+// Four consecutive elements of a bf16 row (the residual stream), widened to fp32.  idx4 counts groups of 4 elements.
+__device__ __forceinline__ float4 ld_bf16x4(const uint2* x, size_t idx4) {
+  const uint2 u = x[idx4];
+  return make_float4(bf16_lo(u.x), bf16_hi(u.x), bf16_lo(u.y), bf16_hi(u.y));
+}
+
+// The same for the pooling input, which is the bf16 residual stream or an fp32 hidden state.
 __device__ __forceinline__ float4 ld_row4(const void* x, size_t idx4, int is_bf16) {
-  if (is_bf16) {
-    const uint2 u = reinterpret_cast<const uint2*>(x)[idx4];
-    return make_float4(bf16_lo(u.x), bf16_hi(u.x), bf16_lo(u.y), bf16_hi(u.y));
-  }
+  if (is_bf16) return ld_bf16x4(static_cast<const uint2*>(x), idx4);
   return reinterpret_cast<const float4*>(x)[idx4];
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// F1: resid[t, :] = wte[ids[t], :] (+ wpe[pos[t], :])        one warp-wide 16-B vector per thread-iteration
+// F1: resid[t, :] = bf16(wte[ids[t], :] (+ wpe[pos[t], :]))        one warp-wide 16-B vector per thread-iteration
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) embed_kernel(const int32_t* __restrict__ ids, const int32_t* __restrict__ pos,
                                                     const uint4* __restrict__ wte, const uint4* __restrict__ wpe,
-                                                    float4* __restrict__ resid, int T, int d8, int vocab,
-                                                    int max_pos, int out_bf16) {
+                                                    uint4* __restrict__ resid, int T, int d8, int vocab,
+                                                    int max_pos) {
   pdl_sync();  // programmatic dependent launch: see common.cuh
   // d8 = d / 8: number of 16-B bf16 vectors per row.  Grid-stride over (token, vector).
   const long long total = static_cast<long long>(T) * d8;
@@ -46,19 +47,13 @@ __global__ void __launch_bounds__(256) embed_kernel(const int32_t* __restrict__ 
       f[0] += bf16_lo(q.x); f[1] += bf16_hi(q.x); f[2] += bf16_lo(q.y); f[3] += bf16_hi(q.y);
       f[4] += bf16_lo(q.z); f[5] += bf16_hi(q.z); f[6] += bf16_lo(q.w); f[7] += bf16_hi(q.w);
     }
-    if (out_bf16) {
-      reinterpret_cast<uint4*>(resid)[static_cast<size_t>(t) * d8 + v] =
-          make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7]));
-    } else {
-      float4* dst = resid + (static_cast<size_t>(t) * d8 + v) * 2;
-      dst[0] = make_float4(f[0], f[1], f[2], f[3]);
-      dst[1] = make_float4(f[4], f[5], f[6], f[7]);
-    }
+    resid[static_cast<size_t>(t) * d8 + v] =
+        make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7]));
   }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// F2/F7: LayerNorm, fp32 in, bf16 out.  TPR threads cooperate on one row; each holds V float4 (row in registers,
+// F2/F7: LayerNorm, bf16 in, bf16 out.  TPR threads cooperate on one row; each holds V float4 (row in registers,
 // exact two-pass mean/variance like torch's CPU kernel).
 // ---------------------------------------------------------------------------------------------------------------
 template <int TPR>
@@ -76,16 +71,9 @@ __device__ __forceinline__ float group_sum(float v, float* scratch /* [rows_per_
   return s;
 }
 
-__device__ __forceinline__ void ln_store(uint2* y, size_t idx, float o0, float o1, float o2, float o3) {
-  y[idx] = make_uint2(pack_bf16(o0, o1), pack_bf16(o2, o3));
-}
-__device__ __forceinline__ void ln_store(float4* y, size_t idx, float o0, float o1, float o2, float o3) {
-  y[idx] = make_float4(o0, o1, o2, o3);
-}
-
-template <int TPR, int V, class OutT>
-__device__ __forceinline__ void layernorm_body(const void* x, int x_bf16, const float4* __restrict__ g,
-                                               const float4* __restrict__ b, OutT* y, int T, int d4, float eps,
+template <int TPR, int V>
+__device__ __forceinline__ void layernorm_body(const uint2* x, const float4* __restrict__ g, const float4* __restrict__ b,
+                                               uint2* y, int T, int d4, float eps,
                                                const int32_t* __restrict__ src_rows = nullptr) {
   constexpr int ROWS = 256 / TPR;
   __shared__ float scratch[ROWS * (TPR / 32) + 1];
@@ -100,7 +88,7 @@ __device__ __forceinline__ void layernorm_body(const void* x, int x_bf16, const 
 #pragma unroll
   for (int i = 0; i < V; ++i) {
     const int c = l + i * TPR;
-    v[i] = (active && c < d4) ? ld_row4(x, static_cast<size_t>(src) * d4 + c, x_bf16) : make_float4(0.f, 0.f, 0.f, 0.f);
+    v[i] = (active && c < d4) ? ld_bf16x4(x, static_cast<size_t>(src) * d4 + c) : make_float4(0.f, 0.f, 0.f, 0.f);
     s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
   }
   const float inv_d = 1.0f / static_cast<float>(d4 * 4);
@@ -126,25 +114,26 @@ __device__ __forceinline__ void layernorm_body(const void* x, int x_bf16, const 
       const float o1 = (v[i].y - mean) * rstd * gg.y + bb.y;
       const float o2 = (v[i].z - mean) * rstd * gg.z + bb.z;
       const float o3 = (v[i].w - mean) * rstd * gg.w + bb.w;
-      ln_store(y, static_cast<size_t>(row) * d4 + c, o0, o1, o2, o3);
+      y[static_cast<size_t>(row) * d4 + c] = make_uint2(pack_bf16(o0, o1), pack_bf16(o2, o3));
     }
   }
 }
 
+// (min. 1 CTA per SM: without it ptxas caps the <128, 8> instance at 48 registers and spills)
 template <int TPR, int V>
-__global__ void __launch_bounds__(256) layernorm_kernel(const void* x, const float4* __restrict__ g,
-                                                        const float4* __restrict__ b, uint2* y, int T,
-                                                        int d4, float eps, int x_bf16) {
+__global__ void __launch_bounds__(256, 1) layernorm_kernel(const uint2* x, const float4* __restrict__ g,
+                                                           const float4* __restrict__ b, uint2* y, int T, int d4,
+                                                           float eps) {
   pdl_sync();  // programmatic dependent launch: see common.cuh
-  layernorm_body<TPR, V>(x, x_bf16, g, b, y, T, d4, eps);  // (bf16 in: y may alias x — a thread rewrites only what it read)
+  layernorm_body<TPR, V>(x, g, b, y, T, d4, eps);  // y may alias x: a thread rewrites only what it read
 }
 
 // bf16 residual stream -> bf16 normalised row with 16-byte accesses (8 elements per load / store; the generic kernel above
 // would read a bf16 row with 8-byte loads and write with 8-byte stores).  May run in place (a thread rewrites only the chunks it read).
-template <int TPR, int V8, int MINB = 1>
-__global__ void __launch_bounds__(256, MINB) layernorm_bf16_kernel(const uint4* x, const float4* __restrict__ g,
-                                                             const float4* __restrict__ b, uint4* y, int T, int d8,
-                                                             float eps) {
+template <int TPR, int V8>
+__global__ void __launch_bounds__(256, 1) layernorm_bf16_kernel(const uint4* x, const float4* __restrict__ g,
+                                                                const float4* __restrict__ b, uint4* y, int T, int d8,
+                                                                float eps) {
   pdl_sync();  // programmatic dependent launch: see common.cuh
   constexpr int ROWS = 256 / TPR;
   __shared__ float scratch[ROWS * (TPR / 32) + 1];
@@ -195,7 +184,7 @@ __global__ void __launch_bounds__(256, MINB) layernorm_bf16_kernel(const uint4* 
   }
 }
 
-// Persistent form of the kernel above (the default for d <= 768 and 1024 < d <= 4096).  In the one-row-per-group kernel every
+// Persistent form of the kernel above (used for d <= 768 and 1024 < d <= 4096).  In the one-row-per-group kernel every
 // row re-reads 8 bytes of gamma / beta per element through the L1 against 2 bytes of x (tools/ln_bench.cu times both).  Here a thread group keeps its gamma / beta
 // chunks in registers and walks over rows (grid = MINB CTAs per SM), with the next row's loads issued as soon as the
 // current row is unpacked.  May run in place (a group rewrites only rows it has already read, and
@@ -297,109 +286,15 @@ __global__ void __launch_bounds__(256, MINB) layernorm_bf16_persist_kernel(const
   }
 }
 
-// bf16 -> bf16 LayerNorm with the rows staged through shared memory by bulk async copies (UBLKCP): a CTA owns 8 * NS
-// consecutive rows and issues the copies of ALL its stages (8 rows = one contiguous 8 * d * 2-byte chunk each) before it
-// touches the first one, so every SM has ~190 KB of reads in flight regardless of register pressure.  One warp per row:
-// sum, centred sum of squares and the normalised output are three sweeps over the row IN SHARED MEMORY (16-byte, conflict-
-// free), the output leaves with 16-byte global stores.  The register-resident kernels above are latency x occupancy
-// bound at 3.4 TB/s (32 rows in flight per SM).  May run in place (a stage is read completely before its rows are written;
-// stages of different CTAs are disjoint).
-template <int NS>
-__global__ void __launch_bounds__(256) layernorm_bf16_bulk_kernel(const uint4* x, const float4* __restrict__ g,
-                                                                  const float4* __restrict__ b, uint4* y, int T, int d8,
-                                                                  float eps) {
-  extern __shared__ uint8_t ln_smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(ln_smem_raw) + 127) & ~uintptr_t(127));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem);          // NS barriers (128 bytes reserved)
-  uint4* rows = reinterpret_cast<uint4*>(smem + 128);          // [NS][8][d8]
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int row_base = blockIdx.x * 8 * NS;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < NS; ++s) mbar_init(&bars[s], 1);
-    fence_mbar_init();
-  }
-  __syncthreads();
-  pdl_sync();  // programmatic dependent launch: the residual stream is read only below this line
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < NS; ++s) {
-      const int r0 = row_base + 8 * s;
-      if (r0 >= T) break;
-      const int nr = min(8, T - r0);
-      const uint32_t bytes = static_cast<uint32_t>(nr) * static_cast<uint32_t>(d8) * 16u;
-      mbar_expect_tx(&bars[s], bytes);
-      bulk_load_1d(rows + static_cast<size_t>(s) * 8 * d8, x + static_cast<size_t>(r0) * d8, bytes, &bars[s]);
-    }
-  }
-  const float inv_d = 1.0f / static_cast<float>(d8 * 8);
-#pragma unroll 1
-  for (int s = 0; s < NS; ++s) {
-    const int row = row_base + 8 * s + warp;
-    if (row_base + 8 * s >= T) break;  // CTA-uniform
-    mbar_wait(&bars[s], 0);
-    if (row >= T) continue;            // warp-uniform
-    const uint4* r = rows + (static_cast<size_t>(s) * 8 + warp) * d8;
-    float sum = 0.f;
-    for (int c = lane; c < d8; c += 32) {
-      const uint4 u = r[c];
-      sum += ((bf16_lo(u.x) + bf16_hi(u.x)) + (bf16_lo(u.y) + bf16_hi(u.y))) +
-             ((bf16_lo(u.z) + bf16_hi(u.z)) + (bf16_lo(u.w) + bf16_hi(u.w)));
-    }
-    const float mean = warp_sum(sum) * inv_d;
-    float q = 0.f;
-    for (int c = lane; c < d8; c += 32) {
-      const uint4 u = r[c];
-      const float e[8] = {bf16_lo(u.x), bf16_hi(u.x), bf16_lo(u.y), bf16_hi(u.y), bf16_lo(u.z), bf16_hi(u.z), bf16_lo(u.w), bf16_hi(u.w)};
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float a = e[i] - mean;
-        q = fmaf(a, a, q);
-      }
-    }
-    const float rstd = rsqrtf(warp_sum(q) * inv_d + eps);
-    uint4* yo = y + static_cast<size_t>(row) * d8;
-    for (int c = lane; c < d8; c += 32) {
-      const uint4 u = r[c];
-      const float e[8] = {bf16_lo(u.x), bf16_hi(u.x), bf16_lo(u.y), bf16_hi(u.y), bf16_lo(u.z), bf16_hi(u.z), bf16_lo(u.w), bf16_hi(u.w)};
-      const float4 g0 = __ldg(g + 2 * c), g1 = __ldg(g + 2 * c + 1), b0 = __ldg(b + 2 * c), b1 = __ldg(b + 2 * c + 1);
-      const float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-      const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-      float o[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) o[i] = (e[i] - mean) * rstd * gg[i] + bb[i];
-      yo[c] = make_uint4(pack_bf16(o[0], o[1]), pack_bf16(o[2], o[3]), pack_bf16(o[4], o[5]), pack_bf16(o[6], o[7]));
-    }
-  }
-}
-
-template <int NS>
-static int launch_layernorm_bulk(const uint4* x, const float4* g, const float4* b, uint4* y, int T, int d8, float eps,
-                                 cudaStream_t stream) {
-  const size_t smem = 128 + 128 + static_cast<size_t>(NS) * 8 * d8 * 16;
-  auto kern = layernorm_bf16_bulk_kernel<NS>;
-  static PerDeviceOnce attr_once;
-  if (attr_once.first()) SGPT_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  SGPT_CHECK_CUDA(launch_kernel(kern, dim3((T + 8 * NS - 1) / (8 * NS)), dim3(256), smem, stream, x, g, b, y, T, d8, eps));
-  return SGPT_OK;
-}
-
 // LayerNorm of a gathered subset of rows: y[m,:] = LN(x[rows[m],:]) (the LM-head input of the cross-encoder scorer)
 template <int TPR, int V>
-__global__ void __launch_bounds__(256) layernorm_gather_kernel(const void* __restrict__ x,
+__global__ void __launch_bounds__(256) layernorm_gather_kernel(const uint2* __restrict__ x,
                                                                const float4* __restrict__ g,
                                                                const float4* __restrict__ b, uint2* __restrict__ y,
                                                                int M, int d4, float eps,
-                                                               const int32_t* __restrict__ rows, int x_bf16) {
+                                                               const int32_t* __restrict__ rows) {
   pdl_sync();  // programmatic dependent launch: see common.cuh
-  layernorm_body<TPR, V>(x, x_bf16, g, b, y, M, d4, eps, rows);
-}
-
-// fp32 output, may run in place (each thread rewrites exactly the elements it read)
-template <int TPR, int V>
-__global__ void __launch_bounds__(256) layernorm_f32_kernel(const float4* x, const float4* __restrict__ g,
-                                                            const float4* __restrict__ b, float4* y, int T, int d4,
-                                                            float eps) {
-  pdl_sync();  // programmatic dependent launch: see common.cuh
-  layernorm_body<TPR, V>(x, 0, g, b, y, T, d4, eps);
+  layernorm_body<TPR, V>(x, g, b, y, M, d4, eps, rows);
 }
 
 // Row statistics only (mean, rstd) -> stats[2*t], used by the pooling kernel to apply ln_f on the fly.
@@ -779,14 +674,8 @@ static inline int grid_for(long long work_items, int threads) {
 
 using namespace sgpt;
 
-extern "C" int sgpt_embed_tokens(const int32_t* ids, const int32_t* pos, const void* wte, const void* wpe,
-                                 float* resid, int T, int d, int vocab, int max_pos, sgpt_stream_t stream_) {
-  return sgpt_embed_tokens_ex(ids, pos, wte, wpe, resid, T, d, vocab, max_pos, 0, stream_);
-}
-
-extern "C" int sgpt_embed_tokens_ex(const int32_t* ids, const int32_t* pos, const void* wte, const void* wpe,
-                                    void* resid, int T, int d, int vocab, int max_pos, int resid_bf16,
-                                    sgpt_stream_t stream_) {
+extern "C" int sgpt_embed_tokens(const int32_t* ids, const int32_t* pos, const void* wte, const void* wpe, void* resid,
+                                 int T, int d, int vocab, int max_pos, sgpt_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   SGPT_REQUIRE(T >= 0 && d > 0 && d % 8 == 0, "sgpt_embed_tokens: d=%d must be a positive multiple of 8", d);
   SGPT_REQUIRE(wpe == nullptr || pos != nullptr, "sgpt_embed_tokens: pos required when wpe is given");
@@ -795,97 +684,59 @@ extern "C" int sgpt_embed_tokens_ex(const int32_t* ids, const int32_t* pos, cons
   LaunchScope _ls(kCatEmbed, stream);
   SGPT_CHECK_CUDA(launch_kernel(embed_kernel, dim3(grid_for(static_cast<long long>(T) * d8, 256)), dim3(256), 0, stream,
                                 ids, pos, static_cast<const uint4*>(wte), static_cast<const uint4*>(wpe),
-                                reinterpret_cast<float4*>(resid), T, d8, vocab, max_pos, resid_bf16));
+                                static_cast<uint4*>(resid), T, d8, vocab, max_pos));
   return SGPT_OK;
 }
 
-extern "C" int sgpt_layernorm(const float* x, const float* gamma, const float* beta, void* y, int T, int d,
-                              float eps, sgpt_stream_t stream_) {
-  return sgpt_layernorm_ex(x, 0, gamma, beta, y, T, d, eps, stream_);
-}
-
-extern "C" int sgpt_layernorm_ex(const void* x, int x_bf16, const float* gamma, const float* beta, void* y, int T, int d,
-                                 float eps, sgpt_stream_t stream_) {
+extern "C" int sgpt_layernorm(const void* x, const float* gamma, const float* beta, void* y, int T, int d, float eps,
+                              sgpt_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   SGPT_REQUIRE(T >= 0 && d > 0 && d % 4 == 0, "sgpt_layernorm: d=%d must be a positive multiple of 4", d);
   if (T == 0) return SGPT_OK;
   const int d4 = d / 4;
   LaunchScope _ls(kCatLayerNorm, stream);
-  if (x_bf16 && d % 8 == 0 && d <= 8192) {
+  if (d % 8 == 0 && d <= 8192) {
     const int d8 = d / 8;
     const uint4* xi = static_cast<const uint4*>(x);
     const float4 *gi = reinterpret_cast<const float4*>(gamma), *bi = reinterpret_cast<const float4*>(beta);
     uint4* yo = static_cast<uint4*>(y);
-    // SGPT_LN_BULK=1: rows staged through shared memory by bulk async copies, off by default
-    static const bool bulk = [] { const char* e = getenv("SGPT_LN_BULK"); return e != nullptr && e[0] == '1'; }();
-    if (bulk) {
-      // stages of 8 rows; as many per CTA as ~48 KB hold (d 768: 4, d 2048: 1, d 4096: 1)
-      const size_t stage = static_cast<size_t>(8) * d8 * 16;
-      if (4 * stage <= 56 * 1024) return launch_layernorm_bulk<4>(xi, gi, bi, yo, T, d8, eps, stream);
-      if (2 * stage <= 56 * 1024) return launch_layernorm_bulk<2>(xi, gi, bi, yo, T, d8, eps, stream);
-      return launch_layernorm_bulk<1>(xi, gi, bi, yo, T, d8, eps, stream);
-    }
-    // Persistent groups with gamma / beta in registers (see layernorm_bf16_persist_kernel); SGPT_LN_PERSIST=0 selects the
-    // one-row-per-group kernels.  Widths without a persistent instance (768 < d <= 1024, d > 4096) use those as well.
-    static const bool persist = [] { const char* e = getenv("SGPT_LN_PERSIST"); return !(e != nullptr && e[0] == '0'); }();
+    // Persistent groups with gamma / beta in registers (see layernorm_bf16_persist_kernel) where an instance exists; the
+    // one-row-per-group kernels for the other widths (768 < d <= 1024, d > 4096).
     const int sms = sm_count();
     auto grid_for_rows = [&](int rows_per_cta, int ctas_per_sm) {
       const int need = (T + rows_per_cta - 1) / rows_per_cta;
       return dim3(static_cast<unsigned>(need < sms * ctas_per_sm ? need : sms * ctas_per_sm));
     };
-    if (persist && d8 <= 32 * 3)
+    if (d8 <= 32 * 3)
       SGPT_CHECK_CUDA(launch_kernel(layernorm_bf16_persist_kernel<32, 3, 2>, grid_for_rows(8, 2), dim3(256), 0, stream, xi, gi, bi, yo, T, d8, eps));
-    else if (persist && d8 > 32 * 4 && d8 <= 128 * 2)
-      SGPT_CHECK_CUDA(launch_kernel(layernorm_bf16_persist_kernel<128, 2, 3>, grid_for_rows(2, 3), dim3(256), 0, stream, xi, gi, bi, yo, T, d8, eps));
-    else if (persist && d8 > 128 * 2 && d8 <= 256 * 2)
-      SGPT_CHECK_CUDA(launch_kernel(layernorm_bf16_persist_kernel<256, 2, 3>, grid_for_rows(1, 3), dim3(256), 0, stream, xi, gi, bi, yo, T, d8, eps));
-    else if (d8 <= 32 * 3)
-      SGPT_CHECK_CUDA(launch_kernel(layernorm_bf16_kernel<32, 3, 6>, dim3((T + 7) / 8), dim3(256), 0, stream, xi, gi, bi, yo, T, d8, eps));
     else if (d8 <= 32 * 4)
       SGPT_CHECK_CUDA(launch_kernel(layernorm_bf16_kernel<32, 4>, dim3((T + 7) / 8), dim3(256), 0, stream, xi, gi, bi, yo, T, d8, eps));
-    else if (d8 <= 128 * 4)
-      SGPT_CHECK_CUDA(launch_kernel(layernorm_bf16_kernel<128, 4>, dim3((T + 1) / 2), dim3(256), 0, stream, xi, gi, bi, yo, T, d8, eps));
+    else if (d8 <= 128 * 2)
+      SGPT_CHECK_CUDA(launch_kernel(layernorm_bf16_persist_kernel<128, 2, 3>, grid_for_rows(2, 3), dim3(256), 0, stream, xi, gi, bi, yo, T, d8, eps));
+    else if (d8 <= 256 * 2)
+      SGPT_CHECK_CUDA(launch_kernel(layernorm_bf16_persist_kernel<256, 2, 3>, grid_for_rows(1, 3), dim3(256), 0, stream, xi, gi, bi, yo, T, d8, eps));
     else
       SGPT_CHECK_CUDA(launch_kernel(layernorm_bf16_kernel<256, 4>, dim3(T), dim3(256), 0, stream, xi, gi, bi, yo, T, d8, eps));
     return SGPT_OK;
   }
-  SGPT_ROW_DISPATCH(layernorm_kernel, d4, T, stream, x,
+  SGPT_ROW_DISPATCH(layernorm_kernel, d4, T, stream, static_cast<const uint2*>(x),
                     reinterpret_cast<const float4*>(gamma), reinterpret_cast<const float4*>(beta),
-                    static_cast<uint2*>(y), T, d4, eps, x_bf16);
+                    static_cast<uint2*>(y), T, d4, eps);
   SGPT_CHECK_CUDA(cudaGetLastError());
   return SGPT_OK;
 }
 
-extern "C" int sgpt_layernorm_gather(const float* x, const int32_t* row_idx, const float* gamma, const float* beta, void* y,
-                                     int M, int d, float eps, sgpt_stream_t stream_) {
-  return sgpt_layernorm_gather_ex(x, 0, row_idx, gamma, beta, y, M, d, eps, stream_);
-}
-
-extern "C" int sgpt_layernorm_gather_ex(const void* x, int x_bf16, const int32_t* row_idx, const float* gamma,
-                                        const float* beta, void* y, int M, int d, float eps, sgpt_stream_t stream_) {
+extern "C" int sgpt_layernorm_gather(const void* x, const int32_t* row_idx, const float* gamma, const float* beta,
+                                     void* y, int M, int d, float eps, sgpt_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   SGPT_REQUIRE(M >= 0 && d > 0 && d % 4 == 0, "sgpt_layernorm_gather: d=%d must be a positive multiple of 4", d);
   SGPT_REQUIRE(row_idx != nullptr, "sgpt_layernorm_gather: rows required");  // (`rows` is a local of the macro below)
   if (M == 0) return SGPT_OK;
   const int d4 = d / 4;
   LaunchScope _ls(kCatLayerNorm, stream);
-  SGPT_ROW_DISPATCH(layernorm_gather_kernel, d4, M, stream, x,
+  SGPT_ROW_DISPATCH(layernorm_gather_kernel, d4, M, stream, static_cast<const uint2*>(x),
                     reinterpret_cast<const float4*>(gamma), reinterpret_cast<const float4*>(beta),
-                    static_cast<uint2*>(y), M, d4, eps, row_idx, x_bf16);
-  SGPT_CHECK_CUDA(cudaGetLastError());
-  return SGPT_OK;
-}
-
-extern "C" int sgpt_layernorm_f32_inplace(float* x, const float* gamma, const float* beta, int T, int d, float eps,
-                                          sgpt_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SGPT_REQUIRE(T >= 0 && d > 0 && d % 4 == 0, "sgpt_layernorm_f32_inplace: d=%d must be a positive multiple of 4", d);
-  if (T == 0) return SGPT_OK;
-  const int d4 = d / 4;
-  LaunchScope _ls(kCatLayerNorm, stream);
-  SGPT_ROW_DISPATCH(layernorm_f32_kernel, d4, T, stream, reinterpret_cast<const float4*>(x),
-                    reinterpret_cast<const float4*>(gamma), reinterpret_cast<const float4*>(beta),
-                    reinterpret_cast<float4*>(x), T, d4, eps);
+                    static_cast<uint2*>(y), M, d4, eps, row_idx);
   SGPT_CHECK_CUDA(cudaGetLastError());
   return SGPT_OK;
 }
@@ -922,18 +773,10 @@ static int pool_check(const int32_t* pos, const float* gamma, const float* beta,
   return SGPT_OK;
 }
 
-extern "C" int sgpt_pool_ex(const float* x, const int32_t* pos, const int32_t* cu_seqlens, const float* gamma,
-                            const float* beta, float eps, const float* pos_weights, int n_pos_weights, float* out,
-                            float* row_stats_ws, int B, int T, int d, int mode, int clamp_denominator, int normalize,
-                            int accumulate, float out_scale, sgpt_stream_t stream_) {
-  return sgpt_pool_ex2(x, 0, pos, cu_seqlens, gamma, beta, eps, pos_weights, n_pos_weights, out, row_stats_ws, B, T, d, mode,
-                       clamp_denominator, normalize, accumulate, out_scale, stream_);
-}
-
-extern "C" int sgpt_pool_ex2(const void* x, int x_bf16, const int32_t* pos, const int32_t* cu_seqlens, const float* gamma,
-                             const float* beta, float eps, const float* pos_weights, int n_pos_weights, float* out,
-                             float* row_stats_ws, int B, int T, int d, int mode, int clamp_denominator, int normalize,
-                             int accumulate, float out_scale, sgpt_stream_t stream_) {
+extern "C" int sgpt_pool(const void* x, int x_bf16, const int32_t* pos, const int32_t* cu_seqlens, const float* gamma,
+                         const float* beta, float eps, const float* pos_weights, int n_pos_weights, float* out,
+                         float* row_stats_ws, int B, int T, int d, int mode, int clamp_denominator, int normalize,
+                         int accumulate, float out_scale, sgpt_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   int rc = pool_check(pos, gamma, beta, pos_weights, n_pos_weights, d, mode);
   if (rc != SGPT_OK) return rc;
@@ -960,21 +803,6 @@ extern "C" int sgpt_pool_ex2(const void* x, int x_bf16, const int32_t* pos, cons
   return pool_launch(x, x_bf16, pos, cu_seqlens, gamma, beta, pos_weights, n_pos_weights, out, stats,
                      normalize ? row_stats_ws + 2 * static_cast<size_t>(T) : nullptr, B, d, mode, clamp_denominator,
                      normalize, accumulate, out_scale, stream);
-}
-
-extern "C" int sgpt_pool_accumulate(const float* x, const int32_t* pos, const int32_t* cu_seqlens, const float* gamma,
-                                    const float* beta, float eps, float* out, float* row_stats_ws, int B, int T, int d,
-                                    int mode, int clamp_denominator, int normalize, int accumulate, float out_scale,
-                                    sgpt_stream_t stream_) {
-  return sgpt_pool_ex(x, pos, cu_seqlens, gamma, beta, eps, nullptr, 0, out, row_stats_ws, B, T, d, mode,
-                      clamp_denominator, normalize, accumulate, out_scale, stream_);
-}
-
-extern "C" int sgpt_pool(const float* x, const int32_t* pos, const int32_t* cu_seqlens, const float* gamma,
-                         const float* beta, float eps, float* out, float* row_stats_ws, int B, int T, int d, int mode,
-                         int clamp_denominator, int normalize, sgpt_stream_t stream_) {
-  return sgpt_pool_ex(x, pos, cu_seqlens, gamma, beta, eps, nullptr, 0, out, row_stats_ws, B, T, d, mode,
-                      clamp_denominator, normalize, /*accumulate=*/0, /*out_scale=*/1.0f, stream_);
 }
 
 extern "C" int sgpt_normalize_rows(float* x, int B, int d, sgpt_stream_t stream_) {

@@ -210,7 +210,7 @@ extern "C" int sgpt_profile_gemm_clock(double* sm_cycles, double* nanoseconds) {
 }
 
 extern "C" int sgpt_linear(const void* x, int64_t ldx, const void* w, int64_t ldw, const float* bias, void* out,
-                           int64_t ldo, const float* resid, int M, int N, int K, int epilogue,
+                           int64_t ldo, const void* resid, int M, int N, int K, int epilogue,
                            sgpt_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   SGPT_REQUIRE(M >= 0 && N > 0 && K > 0, "sgpt_linear: bad sizes M=%d N=%d K=%d", M, N, K);
@@ -233,24 +233,8 @@ extern "C" int sgpt_linear(const void* x, int64_t ldx, const void* w, int64_t ld
       EpiBiasActBF16<true>::Params p{om, bias, out, static_cast<int>(ldo)};
       return launch_linear<EpiBiasActBF16<true>>(x, ldx, w, ldw, M, N, K, p, stream);
     }
-    case SGPT_EPI_RESID_F32: {
-      SGPT_REQUIRE(resid != nullptr, "sgpt_linear: SGPT_EPI_RESID_F32 needs resid");
-      SGPT_REQUIRE(ldo % 4 == 0, "sgpt_linear: ldo must be a multiple of 4 for fp32 output");
-      if (resid != static_cast<const float*>(out)) {
-        // not in place: seed the output with the residual, the epilogue then adds acc + bias into it
-        SGPT_CHECK_CUDA(cudaMemcpy2DAsync(out, static_cast<size_t>(ldo) * 4, resid, static_cast<size_t>(ldo) * 4,
-                                          static_cast<size_t>(N) * 4, static_cast<size_t>(M),
-                                          cudaMemcpyDeviceToDevice, stream));
-      }
-      CUtensorMap om;
-      int rc = make_tma_2d_f32(&om, out, static_cast<uint64_t>(M), static_cast<uint64_t>(N),
-                               static_cast<uint64_t>(ldo), 32, 32);
-      if (rc != SGPT_OK) return rc;
-      EpiResidualF32::Params p{om, bias, out, static_cast<int>(ldo)};
-      return launch_linear<EpiResidualF32>(x, ldx, w, ldw, M, N, K, p, stream, pick_ksplit(K));
-    }
     case SGPT_EPI_RESID_BF16: {
-      SGPT_REQUIRE(resid != nullptr && static_cast<const void*>(resid) == out,
+      SGPT_REQUIRE(resid != nullptr && resid == out,
                    "sgpt_linear: SGPT_EPI_RESID_BF16 updates the bf16 residual stream in place (resid must alias out)");
       SGPT_REQUIRE(ldo % 8 == 0, "sgpt_linear: ldo must be a multiple of 8 for bf16 output");
       CUtensorMap om;

@@ -375,8 +375,8 @@ template <class Op, int kDebug = 0>  // kDebug: 1 = skip the TMA store (timing e
 struct EpiTma {
   using Params = typename Op::Params;
   using State = EpiTmaState;
-  static constexpr int kEpiWarps = 8;                 // 2 warps per 32-row slab; each owns ONE 4 KB smem box
-  static constexpr int kCols = 128 / Op::kElemBytes;  // columns per 128-byte row segment: 64 (bf16) or 32 (fp32)
+  static constexpr int kEpiWarps = 8;  // 2 warps per 32-row slab; each owns ONE 4 KB smem box
+  static constexpr int kCols = 64;     // bf16 columns per 128-byte row segment
   static __device__ __forceinline__ void init(State& st, const Params&) { st.it = 0; st.ks = 0; }
   template <int BN, int kSlabBytes>
   static __device__ __forceinline__ void pre_tile(State&, const Params&, int, int, int, float*, int, int) {}
@@ -404,7 +404,7 @@ struct EpiTma {
       }
       uint32_t v[kCols];
       acc_ld_32(trow + 4 * c, *reinterpret_cast<uint32_t(*)[32]>(&v[0]));
-      if (kCols == 64) acc_ld_32(trow + 4 * (c + 32), *reinterpret_cast<uint32_t(*)[32]>(&v[kCols - 32]));
+      acc_ld_32(trow + 4 * (c + 32), *reinterpret_cast<uint32_t(*)[32]>(&v[32]));
       // 8 chunks of 16 bytes; chunk j of row r lives at position j ^ (r & 7) of the row (SWIZZLE_128B)
       // All 8 chunks are computed before any of them is stored: the bias / rotary-table loads inside Op::chunk are then
       // independent ordinary loads the compiler batches up front (one exposed latency per box instead of one per chunk;
@@ -414,14 +414,14 @@ struct EpiTma {
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         if constexpr (OpSplitK<Op>::value)
-          Op::chunk(p, &v[j * (kCols / 8)], n + j * (kCols / 8), N, m0 + lane, o[j], st.ks == 0);
+          Op::chunk(p, &v[8 * j], n + 8 * j, N, m0 + lane, o[j], st.ks == 0);
         else
-          Op::chunk(p, &v[j * (kCols / 8)], n + j * (kCols / 8), N, m0 + lane, o[j]);
+          Op::chunk(p, &v[8 * j], n + 8 * j, N, m0 + lane, o[j]);
       }
       if (kDebug == 4) {  // experiment: straight 16-byte global stores from the thread = row layout (no smem, no TMA)
         if (m0 + lane < M) {
           uint4* g = reinterpret_cast<uint4*>(static_cast<uint8_t*>(p.out_ptr) +
-                                              (static_cast<size_t>(m0 + lane) * p.ldc + n) * Op::kElemBytes);
+                                              (static_cast<size_t>(m0 + lane) * p.ldc + n) * 2);
 #pragma unroll
           for (int j = 0; j < 8; ++j) g[j] = make_uint4(o[j][0], o[j][1], o[j][2], o[j][3]);
         }
@@ -449,7 +449,6 @@ __device__ __forceinline__ float bias_at(const float* bias, int col, int N) {
 // out_bf16[m, n] = act(acc + bias[n])          act = identity | gelu_new
 template <bool kGelu>
 struct OpTmaBiasActBF16 {
-  static constexpr int kElemBytes = 2;
   struct Params {
     CUtensorMap out_map;  // bf16 [M, N], box 32 rows x 64 cols, SWIZZLE_128B
     const float* bias;    // may be null
@@ -486,7 +485,6 @@ struct OpTmaBiasActBF16 {
 // (HF:gptj/modeling_gptj.py:55-67, 196-207: interleaved pairs (x[2i], x[2i+1]) -> (x[2i] c - x[2i+1] s, x[2i+1] c + x[2i] s)
 // with angle pos[m] * 10000^(-2i/rotary_dim)); v columns and the non-rotary dims pass through.  No bias (:98-101).
 struct OpTmaRotaryBF16 {
-  static constexpr int kElemBytes = 2;
   struct Params {
     CUtensorMap out_map;     // bf16 [M, 3d]
     const int32_t* pos;      // [M] position of each token row
@@ -523,40 +521,9 @@ struct OpTmaRotaryBF16 {
   }
 };
 
-// resid_f32[m, n] += acc + bias[n]      (fp32 residual stream updated in place by a TMA reduce-add)
-struct OpTmaResidAddF32 {
-  static constexpr int kElemBytes = 4;
-  struct Params {
-    CUtensorMap out_map;  // fp32 [M, N], box 32 rows x 32 cols, SWIZZLE_128B
-    const float* bias;    // may be null
-    void* out_ptr;
-    int ldc;
-  };
-  // 4 consecutive columns -> 16 bytes
-  static constexpr bool kSplitK = true;
-  static __device__ __forceinline__ void chunk(const Params& p, const uint32_t* acc, int col, int N,
-                                               int /*row*/, uint32_t (&o)[4], bool add_bias) {
-    const float* bias = add_bias ? p.bias : nullptr;
-    if (bias && col + 4 <= N) {
-      const float4 b = __ldg(reinterpret_cast<const float4*>(bias + col));
-      o[0] = __float_as_uint(__uint_as_float(acc[0]) + b.x);
-      o[1] = __float_as_uint(__uint_as_float(acc[1]) + b.y);
-      o[2] = __float_as_uint(__uint_as_float(acc[2]) + b.z);
-      o[3] = __float_as_uint(__uint_as_float(acc[3]) + b.w);
-    } else {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) o[i] = __float_as_uint(__uint_as_float(acc[i]) + bias_at(bias, col + i, N));
-    }
-  }
-  static __device__ __forceinline__ void issue(const Params& p, const void* box, int n, int m0) {
-    tma_reduce_add_2d(&p.out_map, box, n, m0);
-  }
-};
-
-// resid_bf16[m, n] += acc + bias[n]     (bf16 residual stream, SGPT_RESID_BF16=1: the add is a bf16 TMA reduce-add
-// performed by the L2 — half the epilogue's shared-memory and HBM traffic of the fp32 stream)
+// resid_bf16[m, n] += acc + bias[n]     (the residual stream updated in place by a bf16 TMA reduce-add performed by
+// the L2: no residual load in the SM)
 struct OpTmaResidAddBF16 {
-  static constexpr int kElemBytes = 2;
   struct Params {
     CUtensorMap out_map;  // bf16 [M, N], box 32 rows x 64 cols, SWIZZLE_128B
     const float* bias;    // may be null
@@ -1029,7 +996,6 @@ struct EpiIvfRows {
 
 template <bool kGelu>
 using EpiBiasActBF16 = EpiTma<OpTmaBiasActBF16<kGelu>>;
-using EpiResidualF32 = EpiTma<OpTmaResidAddF32>;
 using EpiResidualBF16 = EpiTma<OpTmaResidAddBF16>;
 using EpiRotaryBF16 = EpiTma<OpTmaRotaryBF16>;
 

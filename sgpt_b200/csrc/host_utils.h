@@ -32,9 +32,6 @@ const char* get_error();
 // 128-byte swizzle (box_cols must be 64 bf16 = 128 B).  Returns 0 on success.
 int make_tma_2d_bf16(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
                      uint32_t box_rows, uint32_t box_cols);
-// Same for fp32 elements (box_cols = 32 floats = 128 B).
-int make_tma_2d_f32(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
-                    uint32_t box_cols);
 // Same for int8 elements (box_cols = 128 bytes); out-of-bounds elements of a box read as zero, which covers the K tail.
 int make_tma_2d_u8(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
                    uint32_t box_cols);

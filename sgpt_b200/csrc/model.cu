@@ -9,13 +9,11 @@
 //                                                       bias) -> +res -> post_attention_layernorm -> mlp (tanh gelu) -> +res
 // The handle borrows the caller's weight buffers and owns only its activation workspace, laid out for a ragged batch
 // of at most cfg.max_tokens rows:
-//     resid fp32[T,d] | xb bf16[T,d] | qkv bf16[T,3d] | attn bf16[T,d] | ffn bf16[T,ff] | stats fp32[2T+B]
+//     resid bf16[T,d] | xb bf16[T,d] | qkv bf16[T,3d] | attn bf16[T,d] | ffn bf16[T,ff] | stats fp32[2T+B]
 //
 // Each block runs LayerNorm as a pass of its own (residual stream -> bf16 xb), then GEMMs with bias / gelu epilogues for
-// the layers that read xb and reduce-add epilogues for the layers that update the residual stream.  The residual stream is
-// bf16 (SGPT_RESID_BF16=0 at creation: fp32).
+// the layers that read xb and bf16 reduce-add epilogues for the layers that update the bf16 residual stream.
 #include <math.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include <vector>
@@ -28,9 +26,8 @@ struct sgpt_model {
   sgpt_model_weights w;
   std::vector<sgpt_layer_weights> layers;
   int device = 0;
-  float* resid = nullptr;
-  void* xn = nullptr;  // xb: LayerNorm output, the A operand of the QKV / c_fc GEMMs
-  bool resid_bf16 = true;   // residual stream stored in bf16 (default; SGPT_RESID_BF16=0 at creation: fp32)
+  void* resid = nullptr;  // the residual stream, bf16
+  void* xn = nullptr;     // xb: LayerNorm output, the A operand of the QKV / c_fc GEMMs
   void* qkv = nullptr;
   void* attn = nullptr;
   void* ffn = nullptr;
@@ -97,16 +94,12 @@ extern "C" int sgpt_model_create(const sgpt_model_config* cfg, const sgpt_model_
   }
   cudaError_t e = cudaGetDevice(&m->device);
   const size_t T = static_cast<size_t>(cfg->max_tokens), d = static_cast<size_t>(cfg->d_model);
-  if (e == cudaSuccess) e = cudaMalloc(&m->resid, T * d * 4);
+  if (e == cudaSuccess) e = cudaMalloc(&m->resid, T * d * 2);
   if (e == cudaSuccess) e = cudaMalloc(&m->xn, T * d * 2);
   if (e == cudaSuccess) e = cudaMalloc(&m->qkv, T * d * 3 * 2);
   if (e == cudaSuccess) e = cudaMalloc(&m->attn, T * d * 2);
   if (e == cudaSuccess) e = cudaMalloc(&m->ffn, T * static_cast<size_t>(cfg->d_ff) * 2);
-  {
-    const char* rb = getenv("SGPT_RESID_BF16");
-    m->resid_bf16 = !(rb != nullptr && rb[0] == '0');  // default ON; SGPT_RESID_BF16=0 keeps the stream in fp32
-  }
-  // (mean, rstd) per row for ln_f, then the per-sequence sums of squares of the normalisation (sgpt_pool_ex2)
+  // (mean, rstd) per row for ln_f, then the per-sequence sums of squares of the normalisation (sgpt_pool)
   if (e == cudaSuccess) e = cudaMalloc(&m->stats, (2 * T + static_cast<size_t>(cfg->max_batch)) * 4);
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
   if (e == cudaSuccess && cfg->arch == SGPT_ARCH_GPTJ) {
@@ -188,55 +181,51 @@ extern "C" int sgpt_encode(sgpt_model_t m, const int32_t* ids, const int32_t* po
   const float inv_sqrt_hd = 1.0f / sqrtf(static_cast<float>(hd));
   m->last_T = T;
 
-  const int rb = m->resid_bf16 ? 1 : 0;  // residual stream dtype: 0 fp32, 1 bf16 (same buffer, half of it used)
-  const int epi_resid = rb ? SGPT_EPI_RESID_BF16 : SGPT_EPI_RESID_F32;
-  SGPT_TRY(sgpt_embed_tokens_ex(ids, pos, m->w.wte, c.arch == SGPT_ARCH_GPT_NEO ? m->w.wpe : nullptr, m->resid, T, d,
-                                c.vocab, c.max_pos, rb, stream));
-  if (c.arch == SGPT_ARCH_BLOOM) {
-    if (rb) SGPT_TRY(sgpt_layernorm_ex(m->resid, 1, m->w.emb_ln_g, m->w.emb_ln_b, m->resid, T, d, c.ln_eps, stream));
-    else SGPT_TRY(sgpt_layernorm_f32_inplace(m->resid, m->w.emb_ln_g, m->w.emb_ln_b, T, d, c.ln_eps, stream));
-  }
+  SGPT_TRY(sgpt_embed_tokens(ids, pos, m->w.wte, c.arch == SGPT_ARCH_GPT_NEO ? m->w.wpe : nullptr, m->resid, T, d,
+                             c.vocab, c.max_pos, stream));
+  if (c.arch == SGPT_ARCH_BLOOM)
+    SGPT_TRY(sgpt_layernorm(m->resid, m->w.emb_ln_g, m->w.emb_ln_b, m->resid, T, d, c.ln_eps, stream));
   const int n_run = layer_idx;  // hidden_states[i] is the input of block i; hidden_states[L] is ln_f(output of block L-1)
   for (int l = 0; l < n_run && l < c.n_layer; ++l) {
     const sgpt_layer_weights& lw = m->layers[l];
     if (all_layers)  // hidden_states[l] = the residual stream entering block l (no ln_f)
-      SGPT_TRY(sgpt_pool_ex2(m->resid, rb, pos, cu_seqlens, nullptr, nullptr, c.ln_eps, nullptr, 0, out, nullptr, B, T, d,
-                             base_mode, clamp_denominator, 0, /*accumulate=*/l > 0, layer_scale, stream));
-    SGPT_TRY(sgpt_layernorm_ex(m->resid, rb, lw.ln1_g, lw.ln1_b, m->xn, T, d, c.ln_eps, stream));
+      SGPT_TRY(sgpt_pool(m->resid, 1, pos, cu_seqlens, nullptr, nullptr, c.ln_eps, nullptr, 0, out, nullptr, B, T, d,
+                         base_mode, clamp_denominator, 0, /*accumulate=*/l > 0, layer_scale, stream));
+    SGPT_TRY(sgpt_layernorm(m->resid, lw.ln1_g, lw.ln1_b, m->xn, T, d, c.ln_eps, stream));
     if (c.arch == SGPT_ARCH_GPT_NEO) {
       SGPT_TRY(sgpt_linear(m->xn, d, lw.w_qkv, d, lw.b_qkv, m->qkv, 3 * d, nullptr, T, 3 * d, d, SGPT_EPI_BF16, stream));
       const int window = (lw.local_attention && c.window > 0 && max_seqlen > c.window) ? c.window : 0;
       SGPT_TRY(sgpt_attention(m->qkv, m->attn, cu_seqlens, B, T, H, hd, /*scale=*/1.0f, window, max_seqlen, nullptr, 0,
                               stream));
-      SGPT_TRY(sgpt_linear(m->attn, d, lw.w_o, d, lw.b_o, m->resid, d, m->resid, T, d, d, epi_resid, stream));
-      SGPT_TRY(sgpt_layernorm_ex(m->resid, rb, lw.ln2_g, lw.ln2_b, m->xn, T, d, c.ln_eps, stream));
+      SGPT_TRY(sgpt_linear(m->attn, d, lw.w_o, d, lw.b_o, m->resid, d, m->resid, T, d, d, SGPT_EPI_RESID_BF16, stream));
+      SGPT_TRY(sgpt_layernorm(m->resid, lw.ln2_g, lw.ln2_b, m->xn, T, d, c.ln_eps, stream));
       SGPT_TRY(sgpt_linear(m->xn, d, lw.w_fc, d, lw.b_fc, m->ffn, ff, nullptr, T, ff, d, SGPT_EPI_GELU_BF16, stream));
-      SGPT_TRY(sgpt_linear(m->ffn, ff, lw.w_proj, ff, lw.b_proj, m->resid, d, m->resid, T, d, ff, epi_resid,
-                           stream));
+      SGPT_TRY(sgpt_linear(m->ffn, ff, lw.w_proj, ff, lw.b_proj, m->resid, d, m->resid, T, d, ff,
+                           SGPT_EPI_RESID_BF16, stream));
     } else if (c.arch == SGPT_ARCH_GPTJ) {
       SGPT_TRY(sgpt_linear_qkv_rotary(m->xn, d, lw.w_qkv, m->qkv, pos, m->rotary, T, d, hd, c.rotary_dim, c.max_pos,
                                       stream));
       SGPT_TRY(sgpt_attention(m->qkv, m->attn, cu_seqlens, B, T, H, hd, inv_sqrt_hd, 0, max_seqlen, nullptr, 0, stream));
       // both branches read the same ln_1 output and are accumulated into the residual stream (attn + mlp + residual)
       SGPT_TRY(sgpt_linear(m->xn, d, lw.w_fc, d, lw.b_fc, m->ffn, ff, nullptr, T, ff, d, SGPT_EPI_GELU_BF16, stream));
-      SGPT_TRY(sgpt_linear(m->attn, d, lw.w_o, d, lw.b_o, m->resid, d, m->resid, T, d, d, epi_resid, stream));
-      SGPT_TRY(sgpt_linear(m->ffn, ff, lw.w_proj, ff, lw.b_proj, m->resid, d, m->resid, T, d, ff, epi_resid,
-                           stream));
+      SGPT_TRY(sgpt_linear(m->attn, d, lw.w_o, d, lw.b_o, m->resid, d, m->resid, T, d, d, SGPT_EPI_RESID_BF16, stream));
+      SGPT_TRY(sgpt_linear(m->ffn, ff, lw.w_proj, ff, lw.b_proj, m->resid, d, m->resid, T, d, ff,
+                           SGPT_EPI_RESID_BF16, stream));
     } else {  // BLOOM
       SGPT_TRY(sgpt_linear(m->xn, d, lw.w_qkv, d, lw.b_qkv, m->qkv, 3 * d, nullptr, T, 3 * d, d, SGPT_EPI_BF16, stream));
       SGPT_TRY(sgpt_attention(m->qkv, m->attn, cu_seqlens, B, T, H, hd, inv_sqrt_hd, 0, max_seqlen, m->alibi, 0, stream));
-      SGPT_TRY(sgpt_linear(m->attn, d, lw.w_o, d, lw.b_o, m->resid, d, m->resid, T, d, d, epi_resid, stream));
-      SGPT_TRY(sgpt_layernorm_ex(m->resid, rb, lw.ln2_g, lw.ln2_b, m->xn, T, d, c.ln_eps, stream));
+      SGPT_TRY(sgpt_linear(m->attn, d, lw.w_o, d, lw.b_o, m->resid, d, m->resid, T, d, d, SGPT_EPI_RESID_BF16, stream));
+      SGPT_TRY(sgpt_layernorm(m->resid, lw.ln2_g, lw.ln2_b, m->xn, T, d, c.ln_eps, stream));
       SGPT_TRY(sgpt_linear(m->xn, d, lw.w_fc, d, lw.b_fc, m->ffn, ff, nullptr, T, ff, d, SGPT_EPI_GELU_BF16, stream));
-      SGPT_TRY(sgpt_linear(m->ffn, ff, lw.w_proj, ff, lw.b_proj, m->resid, d, m->resid, T, d, ff, epi_resid,
-                           stream));
+      SGPT_TRY(sgpt_linear(m->ffn, ff, lw.w_proj, ff, lw.b_proj, m->resid, d, m->resid, T, d, ff,
+                           SGPT_EPI_RESID_BF16, stream));
     }
   }
   if (pool_mode == kNoPooling) return SGPT_OK;
   const bool final_ln = (layer_idx == c.n_layer);
-  SGPT_TRY(sgpt_pool_ex2(m->resid, rb, pos, cu_seqlens, final_ln ? m->w.lnf_g : nullptr, final_ln ? m->w.lnf_b : nullptr, c.ln_eps,
-                         pool_w, pool_w ? m->n_pool_w : 0, out, m->stats, B, T, d, base_mode, clamp_denominator, normalize,
-                         /*accumulate=*/all_layers && c.n_layer > 0, layer_scale, stream));
+  SGPT_TRY(sgpt_pool(m->resid, 1, pos, cu_seqlens, final_ln ? m->w.lnf_g : nullptr, final_ln ? m->w.lnf_b : nullptr, c.ln_eps,
+                     pool_w, pool_w ? m->n_pool_w : 0, out, m->stats, B, T, d, base_mode, clamp_denominator, normalize,
+                     /*accumulate=*/all_layers && c.n_layer > 0, layer_scale, stream));
   return SGPT_OK;
 }
 
@@ -272,8 +261,7 @@ extern "C" int sgpt_lm_logprobs(sgpt_model_t m, const void* lm_head_w, const flo
   for (int m0 = 0; m0 < M; m0 += rows_per_chunk) {
     const int mc = (M - m0 < rows_per_chunk) ? M - m0 : rows_per_chunk;
     // hidden_states[-1] of the selected positions: ln_f of the residual stream the last sgpt_forward left behind
-    SGPT_TRY(sgpt_layernorm_gather_ex(m->resid, m->resid_bf16 ? 1 : 0, rows + m0, m->w.lnf_g, m->w.lnf_b, xsel, mc, d,
-                                      m->cfg.ln_eps, stream));
+    SGPT_TRY(sgpt_layernorm_gather(m->resid, rows + m0, m->w.lnf_g, m->w.lnf_b, xsel, mc, d, m->cfg.ln_eps, stream));
     SGPT_TRY(sgpt_scores(xsel, lm_head_w, nullptr, nullptr, logits, lds, mc, vocab, d, stream));
     SGPT_TRY(sgpt_token_logprobs(logits, lds, mc, vocab, lm_head_bias, targets + m0, token_logprobs + m0,
                                  greedy ? greedy + m0 : nullptr, stream));
@@ -296,8 +284,5 @@ extern "C" int sgpt_model_read_residual(sgpt_model_t m, float* dst, int64_t capa
   *d = m->cfg.d_model;
   const int64_t n = static_cast<int64_t>(m->last_T) * m->cfg.d_model;
   SGPT_REQUIRE(capacity_elems >= n, "sgpt_model_read_residual: destination too small");
-  if (m->resid_bf16) return sgpt_bf16_to_f32(m->resid, dst, n, stream);
-  SGPT_CHECK_CUDA(cudaMemcpyAsync(dst, m->resid, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToDevice,
-                                  static_cast<cudaStream_t>(stream)));
-  return SGPT_OK;
+  return sgpt_bf16_to_f32(m->resid, dst, n, stream);
 }

@@ -231,7 +231,7 @@ class Encoder:
                                   normalize)
 
     def last_residual(self) -> torch.Tensor:
-        """fp32 [T, d] residual stream of the last encode call (parity/debug tap), copied out of the workspace."""
+        """Residual stream of the last encode call widened to fp32 [T, d] (parity/debug tap), copied out of the workspace."""
         T, d = C.c_int32(), C.c_int32()
         buf = torch.empty(self.max_tokens * self.cfg.d_model, dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):

@@ -35,8 +35,6 @@
 static int g_fail = 0;
 static std::mt19937 rng(1234);
 
-static float bf16r(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
-
 template <class T>
 static T* dalloc(size_t n) {
   T* p;
@@ -85,36 +83,35 @@ static float gelu_ref(float x) { return 0.5f * x * (1.f + tanhf(0.79788456080286
 
 // ---------------------------------------------------------------------------------------------------------------
 static void test_linear(int M, int N, int K, int epi, int check_rows) {
+  const bool resid_add = epi == SGPT_EPI_RESID_BF16;  // out += acc + bias in place: out starts as the residual
   auto x = randn((size_t)M * K, 1.0f), w = randn((size_t)N * K, 0.05f), bias = randn(N, 0.5f);
   auto resid = randn((size_t)M * N, 1.0f);
-  auto xb = to_bf16(x), wb = to_bf16(w);
+  auto xb = to_bf16(x), wb = to_bf16(w), rb = to_bf16(resid);
   auto *dx = to_dev(xb), *dw = to_dev(wb);
   float* dbias = to_dev(bias);
-  float* dres = to_dev(resid);
-  void* dout = (epi == SGPT_EPI_RESID_F32) ? (void*)dres : (void*)dalloc<__nv_bfloat16>((size_t)M * N);
+  __nv_bfloat16* dout = resid_add ? to_dev(rb) : dalloc<__nv_bfloat16>((size_t)M * N);
   cudaEvent_t e0, e1;
   CK(cudaEventCreate(&e0));
   CK(cudaEventCreate(&e1));
   // timing: 1 warm-up + 5 timed launches into a scratch output (the checked launch below runs once, on fresh data)
   float ms = 0.f;
   {
-    void* scratch = (epi == SGPT_EPI_RESID_F32) ? (void*)dalloc<float>((size_t)M * N) : dout;
-    const float* rsrc = (epi == SGPT_EPI_RESID_F32) ? (const float*)scratch : dres;
-    if (epi == SGPT_EPI_RESID_F32) CK(cudaMemset(scratch, 0, (size_t)M * N * 4));
-    SG(sgpt_linear(dx, K, dw, K, dbias, scratch, N, rsrc, M, N, K, epi, 0));
+    __nv_bfloat16* scratch = resid_add ? dalloc<__nv_bfloat16>((size_t)M * N) : dout;
+    if (resid_add) CK(cudaMemset(scratch, 0, (size_t)M * N * 2));
+    SG(sgpt_linear(dx, K, dw, K, dbias, scratch, N, resid_add ? scratch : nullptr, M, N, K, epi, 0));
     CK(cudaEventRecord(e0));
-    for (int it = 0; it < 5; ++it) SG(sgpt_linear(dx, K, dw, K, dbias, scratch, N, rsrc, M, N, K, epi, 0));
+    for (int it = 0; it < 5; ++it)
+      SG(sgpt_linear(dx, K, dw, K, dbias, scratch, N, resid_add ? scratch : nullptr, M, N, K, epi, 0));
     CK(cudaEventRecord(e1));
     CK(cudaDeviceSynchronize());
     ms = time_ms(e0, e1) / 5.f;
-    if (epi == SGPT_EPI_RESID_F32) cudaFree(scratch);
+    if (resid_add) cudaFree(scratch);
   }
-  SG(sgpt_linear(dx, K, dw, K, dbias, dout, N, dres, M, N, K, epi, 0));
+  SG(sgpt_linear(dx, K, dw, K, dbias, dout, N, resid_add ? dout : nullptr, M, N, K, epi, 0));
   CK(cudaDeviceSynchronize());
   std::vector<float> got((size_t)M * N);
-  if (epi == SGPT_EPI_RESID_F32) got = to_host((float*)dout, (size_t)M * N);
-  else {
-    auto gb = to_host((__nv_bfloat16*)dout, (size_t)M * N);
+  {
+    auto gb = to_host(dout, (size_t)M * N);
     for (size_t i = 0; i < gb.size(); ++i) got[i] = __bfloat162float(gb[i]);
   }
   double maxerr = 0;
@@ -131,22 +128,24 @@ static void test_linear(int M, int N, int K, int epi, int check_rows) {
       const float* wr = &w[(size_t)n * K];
       for (int k = 0; k < K; ++k) acc += (double)xr[k] * wr[k];
       float ref = (float)acc + bias[n];
-      float tol_scale = 1.f;
       if (epi == SGPT_EPI_GELU_BF16) ref = gelu_ref(ref);
-      if (epi == SGPT_EPI_RESID_F32) ref += resid[(size_t)m * N + n];
-      else tol_scale = fmaxf(1.f, fabsf(ref));  // bf16 output rounding is relative
+      // bf16 output rounding is relative; the residual add rounds acc + bias and then the sum, so it scales with both
+      float tol_scale = fmaxf(1.f, fabsf(ref));
+      if (resid_add) {
+        tol_scale = fmaxf(1.f, fabsf(ref) + fabsf(resid[(size_t)m * N + n]));
+        ref += resid[(size_t)m * N + n];
+      }
       const double err = fabs((double)got[(size_t)m * N + n] - ref) / tol_scale;
       maxerr = std::max(maxerr, err);
     }
   }
   char name[128];
-  const char* en[] = {"bf16", "gelu_bf16", "resid_f32"};
-  snprintf(name, sizeof name, "linear M=%d N=%d K=%d epi=%s (%.1f TFLOP/s)", M, N, K, epi < 3 ? en[epi] : "stub",
+  const char* en[] = {"bf16", "gelu_bf16", "", "resid_bf16"};
+  snprintf(name, sizeof name, "linear M=%d N=%d K=%d epi=%s (%.1f TFLOP/s)", M, N, K, epi <= 3 ? en[epi] : "stub",
            2.0 * M * N * K / (ms * 1e9));
   if (epi >= 100) maxerr = 0;  // profiling stubs write nothing meaningful: timing only
-  report(name, maxerr, epi == SGPT_EPI_RESID_F32 ? 2e-3 : 1.2e-2, ms);
-  cudaFree(dx); cudaFree(dw); cudaFree(dbias); cudaFree(dres);
-  if (epi != SGPT_EPI_RESID_F32) cudaFree(dout);
+  report(name, maxerr, 1.2e-2, ms);
+  cudaFree(dx); cudaFree(dw); cudaFree(dbias); cudaFree(dout);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -229,7 +228,7 @@ static void test_attention(const std::vector<int>& lens, int H, int hd, float sc
 
 // ---------------------------------------------------------------------------------------------------------------
 static void test_rows(int T, int d) {
-  // embed + layernorm + pool(ln_f fused) on a ragged batch
+  // embed + layernorm + pool(ln_f fused) on a ragged batch, through a bf16 residual stream
   const int vocab = 1000, max_pos = 512;
   std::vector<int> lens = {1, 37, 64, 5, 128, 2};
   while ((int)lens.size() < 8) lens.push_back(16);
@@ -247,25 +246,29 @@ static void test_rows(int T, int d) {
   auto *dwte = to_dev(wteb), *dwpe = to_dev(wpeb);
   int *dids = to_dev(ids), *dpos = to_dev(pos), *dcu = to_dev(cu);
   float *dg = to_dev(g), *db = to_dev(bt);
-  float* dres = dalloc<float>((size_t)T * d);
+  auto* dres = dalloc<__nv_bfloat16>((size_t)T * d);
   auto* dy = dalloc<__nv_bfloat16>((size_t)T * d);
   float* dpool = dalloc<float>((size_t)B * d);
   float* dstats = dalloc<float>(2 * (size_t)T + B);
   SG(sgpt_embed_tokens(dids, dpos, dwte, dwpe, dres, T, d, vocab, max_pos, 0));
   SG(sgpt_layernorm(dres, dg, db, dy, T, d, 1e-5f, 0));
-  SG(sgpt_pool(dres, dpos, dcu, dg, db, 1e-5f, dpool, dstats, B, T, d, SGPT_POOL_WEIGHTEDMEAN, 0, 0, 0));
+  SG(sgpt_pool(dres, 1, dpos, dcu, dg, db, 1e-5f, nullptr, 0, dpool, dstats, B, T, d, SGPT_POOL_WEIGHTEDMEAN, 0, 0, 0,
+               1.f, 0));
   CK(cudaDeviceSynchronize());
-  auto res = to_host(dres, (size_t)T * d);
+  auto resb = to_host(dres, (size_t)T * d);
   auto y = to_host(dy, (size_t)T * d);
   auto pool = to_host(dpool, (size_t)B * d);
-  double e_emb = 0, e_ln = 0, e_pool = 0;
+  std::vector<float> res((size_t)T * d);
+  for (size_t i = 0; i < res.size(); ++i) res[i] = __bfloat162float(resb[i]);
+  int emb_bits = 0;  // the embedding is the fp32 sum rounded to nearest even: bit for bit
+  double e_ln = 0, e_pool = 0;
   std::vector<double> ln((size_t)T * d);
   for (int t = 0; t < T; ++t) {
     double mean = 0, var = 0;
     for (int c = 0; c < d; ++c) {
-      const float r = wte[(size_t)ids[t] * d + c] + wpe[(size_t)pos[t] * d + c];
-      e_emb = std::max(e_emb, (double)fabsf(r - res[(size_t)t * d + c]));
-      mean += r;
+      const __nv_bfloat16 r = __float2bfloat16_rn(wte[(size_t)ids[t] * d + c] + wpe[(size_t)pos[t] * d + c]);
+      emb_bits += memcmp(&r, &resb[(size_t)t * d + c], sizeof r) != 0;
+      mean += res[(size_t)t * d + c];
     }
     mean /= d;
     for (int c = 0; c < d; ++c) { double dv = res[(size_t)t * d + c] - mean; var += dv * dv; }
@@ -284,11 +287,12 @@ static void test_rows(int T, int d) {
       e_pool = std::max(e_pool, fabs(num / den - pool[(size_t)b * d + c]));
     }
   char name[96];
-  snprintf(name, sizeof name, "embed d=%d", d); report(name, e_emb, 1e-6);
+  snprintf(name, sizeof name, "embed d=%d bf16 mismatches", d); report(name, emb_bits, 0);
   snprintf(name, sizeof name, "layernorm d=%d", d); report(name, e_ln, 8e-3);
   snprintf(name, sizeof name, "pool weightedmean + ln_f d=%d", d); report(name, e_pool, 2e-5);
   // mean / lasttoken without LN, with normalize
-  SG(sgpt_pool(dres, dpos, dcu, nullptr, nullptr, 0.f, dpool, dstats, B, T, d, SGPT_POOL_LASTTOKEN, 1, 1, 0));
+  SG(sgpt_pool(dres, 1, dpos, dcu, nullptr, nullptr, 0.f, nullptr, 0, dpool, dstats, B, T, d, SGPT_POOL_LASTTOKEN, 1, 1,
+               0, 1.f, 0));
   CK(cudaDeviceSynchronize());
   pool = to_host(dpool, (size_t)B * d);
   double e_last = 0;
@@ -478,20 +482,20 @@ int main(int argc, char** argv) {
     test_linear(300, 768, 768, SGPT_EPI_BF16, 1 << 30);
     test_linear(257, 2304, 768, SGPT_EPI_BF16, 1 << 30);
     test_linear(200, 3072, 768, SGPT_EPI_GELU_BF16, 1 << 30);
-    test_linear(333, 768, 3072, SGPT_EPI_RESID_F32, 1 << 30);
+    test_linear(333, 768, 3072, SGPT_EPI_RESID_BF16, 1 << 30);
     test_linear(77, 200, 72, SGPT_EPI_BF16, 1 << 30);   // ragged N and K tails
-    test_linear(77, 200, 72, SGPT_EPI_RESID_F32, 1 << 30);
+    test_linear(77, 200, 72, SGPT_EPI_RESID_BF16, 1 << 30);
     test_linear(32768, 2304, 768, SGPT_EPI_BF16, 24);
-    test_linear(32768, 768, 768, SGPT_EPI_RESID_F32, 24);
+    test_linear(32768, 768, 768, SGPT_EPI_RESID_BF16, 24);
     test_linear(32768, 3072, 768, SGPT_EPI_GELU_BF16, 24);
-    test_linear(32768, 768, 3072, SGPT_EPI_RESID_F32, 24);
+    test_linear(32768, 768, 3072, SGPT_EPI_RESID_BF16, 24);
     test_linear(16384, 8192, 2048, SGPT_EPI_GELU_BF16, 16);
   }
   if (!strcmp(only, "linperf")) {  // the four per-layer GEMMs of SGPT-125M at batch 256 x 128 (ncu target)
     test_linear(32768, 2304, 768, SGPT_EPI_BF16, 4);
-    test_linear(32768, 768, 768, SGPT_EPI_RESID_F32, 4);
+    test_linear(32768, 768, 768, SGPT_EPI_RESID_BF16, 4);
     test_linear(32768, 3072, 768, SGPT_EPI_GELU_BF16, 4);
-    test_linear(32768, 768, 3072, SGPT_EPI_RESID_F32, 4);
+    test_linear(32768, 768, 3072, SGPT_EPI_RESID_BF16, 4);
   }
   if (!strcmp(only, "nullepi")) {  // timing only: mainloop without / with accumulator loads in the epilogue
     for (int epi = 100; epi <= 105; ++epi)
@@ -538,12 +542,12 @@ int main(int argc, char** argv) {
           cudaFree(dx); cudaFree(dw); cudaFree(dout);
         }
   }
-  if (!strcmp(only, "resid")) {  // is the fp32 reduce-add epilogue what bounds the d x d out-projection?
+  if (!strcmp(only, "resid")) {  // is the reduce-add epilogue what bounds the d x d out-projection?
     test_linear(32768, 768, 768, SGPT_EPI_BF16, 2);
-    test_linear(32768, 768, 768, SGPT_EPI_RESID_F32, 2);
+    test_linear(32768, 768, 768, SGPT_EPI_RESID_BF16, 2);
     test_linear(32768, 768, 768, 100, 0);
     test_linear(32768, 768, 3072, SGPT_EPI_BF16, 2);
-    test_linear(32768, 768, 3072, SGPT_EPI_RESID_F32, 2);
+    test_linear(32768, 768, 3072, SGPT_EPI_RESID_BF16, 2);
     test_linear(32768, 768, 3072, 100, 0);
   }
   if (!strcmp(only, "sweep")) {  // which dimension limits the GEMM rate?

@@ -23,7 +23,7 @@ def _check(enc, fwd, spec, lw, ids, mask, rows):
     want = pooling.weighted_mean(hs, mask[rows])
     cos = min_row_cosine(out[rows], want)
     print(f"[full depth] {type(spec).__name__} {spec.n_layer} layers d={spec.d_model}: min pooled-embedding cosine vs fp32 oracle "
-          f"= {cos:.7f} (SGPT_RESID_BF16={__import__('os').environ.get('SGPT_RESID_BF16', 'default')})")
+          f"= {cos:.7f}")
     assert cos > 1 - COS_TOL, f"pooled-embedding cosine {cos:.6f} through {spec.n_layer} layers"
     again = enc.encode_tokens(ids.numpy(), mask.numpy(), method="weightedmean").cpu()
     assert torch.equal(again, out), "non-deterministic"

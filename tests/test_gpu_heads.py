@@ -41,7 +41,7 @@ def _sentences(ref):
 
 
 def test_pool_ex_learnt_position_weights_bit_level(ref):
-    """sgpt_pool_ex on the reference's fp32 token embeddings (no LayerNorm): same arithmetic as
+    """sgpt_pool on the reference's fp32 token embeddings (x_bf16 = 0, no LayerNorm): same arithmetic as
     WeightedMeanPooling.forward, so fp32 agreement to rounding (1e-5), not just cosine."""
     from sgpt_b200 import _lib
     from sgpt_b200.encoder import pack_ragged
@@ -55,14 +55,14 @@ def test_pool_ex_learnt_position_weights_bit_level(ref):
     out = torch.empty((B, d), dtype=torch.float32, device="cuda")
     ws = torch.empty(2 * T + B, dtype=torch.float32, device="cuda")
     pos_d, cu_d = torch.from_numpy(pos).cuda(), torch.from_numpy(cu).cuda()  # keep alive: raw pointers below
-    rc = _lib.lib().sgpt_pool_ex(x.data_ptr(), pos_d.data_ptr(), cu_d.data_ptr(),
-                                 None, None, 1e-5, pw.data_ptr(), pw.numel(), out.data_ptr(), ws.data_ptr(), B, T, d,
-                                 _lib.POOL_WEIGHTEDMEAN, 1, 0, 0, 1.0, _lib.current_stream())
-    _lib.check(rc, "sgpt_pool_ex")
+    rc = _lib.lib().sgpt_pool(x.data_ptr(), 0, pos_d.data_ptr(), cu_d.data_ptr(),
+                              None, None, 1e-5, pw.data_ptr(), pw.numel(), out.data_ptr(), ws.data_ptr(), B, T, d,
+                              _lib.POOL_WEIGHTEDMEAN, 1, 0, 0, 1.0, _lib.current_stream())
+    _lib.check(rc, "sgpt_pool")
     assert np.abs(out.cpu().numpy() - ref["pooled_learnt"]).max() < 1e-5
     # a table needs the weightedmean mode
-    rc = _lib.lib().sgpt_pool_ex(x.data_ptr(), None, None, None, None, 1e-5, pw.data_ptr(), pw.numel(), out.data_ptr(),
-                                 ws.data_ptr(), B, T, d, _lib.POOL_MEAN, 1, 0, 0, 1.0, _lib.current_stream())
+    rc = _lib.lib().sgpt_pool(x.data_ptr(), 0, None, None, None, None, 1e-5, pw.data_ptr(), pw.numel(), out.data_ptr(),
+                              ws.data_ptr(), B, T, d, _lib.POOL_MEAN, 1, 0, 0, 1.0, _lib.current_stream())
     assert rc == 1
 
 

@@ -42,32 +42,25 @@ def _check_linear(epi, M, K, N, with_bias, padded, seed):
     bias = torch.randn(N, generator=g) * 0.5 if with_bias else None
     ldx, ldw, ldo = (K + 24, K + 8, N + 40) if padded else (K, K, N)
     sentinel = -12352.0  # exact in bf16 and fp32
-    out_f32 = epi in ("resid_f32", "resid_f32_copy")
-    odt = torch.float32 if out_f32 else torch.bfloat16
     resid = None
-    if epi in ("resid_f32", "resid_f32_copy", "resid_bf16"):
-        resid = (torch.randn(M, N, generator=g) * 2).to(odt)
-    if epi in ("resid_f32", "resid_bf16"):  # in place: out starts as the residual
+    if epi == "resid_bf16":  # in place: out starts as the residual
+        resid = (torch.randn(M, N, generator=g) * 2).to(torch.bfloat16)
         out0 = _padded(resid, ldo, sentinel)
     else:  # every element the call must write starts as NaN
-        out0 = _padded(torch.full((M, N), float("nan"), dtype=odt), ldo, sentinel)
+        out0 = _padded(torch.full((M, N), float("nan"), dtype=torch.bfloat16), ldo, sentinel)
     dev = "cuda"
     xd, wd = _padded(x, ldx, float("nan")).to(dev), _padded(w, ldw, float("nan")).to(dev)
     bd = bias.to(dev) if with_bias else None
     od = out0.to(dev)
-    rd = _padded(resid, ldo, -sentinel).to(dev) if epi == "resid_f32_copy" else (od if resid is not None else None)
-    code = {"bf16": L.EPI_BF16, "gelu": L.EPI_GELU_BF16, "resid_f32": L.EPI_RESID_F32, "resid_f32_copy": L.EPI_RESID_F32,
-            "resid_bf16": L.EPI_RESID_BF16}[epi]
+    rd = od if resid is not None else None
+    code = {"bf16": L.EPI_BF16, "gelu": L.EPI_GELU_BF16, "resid_bf16": L.EPI_RESID_BF16}[epi]
     L.check(lib.sgpt_linear(xd.data_ptr(), ldx, wd.data_ptr(), ldw, L.ptr(bd), od.data_ptr(), ldo, L.ptr(rd), M, N, K,
                             code, L.current_stream()), f"sgpt_linear {epi} M={M} K={K} N={N}")
     torch.cuda.synchronize()
     what = f"{epi} M={M} K={K} N={N} bias={with_bias} padded={padded}"
     got_full = od.cpu()
-    bits = torch.int32 if out_f32 else torch.int16
-    assert torch.equal(got_full[:, N:].view(bits), out0[:, N:].view(bits)), f"{what}: pad columns of out were written"
-    if epi == "resid_f32_copy":
-        assert torch.equal(rd.cpu().view(torch.int32), _padded(resid, ldo, -sentinel).view(torch.int32)), \
-            f"{what}: resid was modified"
+    assert torch.equal(got_full[:, N:].view(torch.int16), out0[:, N:].view(torch.int16)), \
+        f"{what}: pad columns of out were written"
     got = got_full[:, :N].double()
     assert bool(torch.isfinite(got).all()), f"{what}: output not written or not finite"
 
@@ -85,26 +78,21 @@ def _check_linear(epi, M, K, N, with_bias, padded, seed):
         # fp32 ulps of |pre| (1 + pre^2)
         want = _gelu_new(pre)
         tol = U * want.abs() + (1 + U) * (1.13 * e_pre + 2.0 ** -11 * pre.abs() + 8 * F32 * pre.abs() * (1 + pre * pre))
-    elif epi == "resid_bf16":
-        # acc + bias is rounded to bf16, then added to the bf16 residual by the TMA reduce (rounded to bf16 again)
+    else:  # resid_bf16: acc + bias is rounded to bf16, then added to the bf16 residual by the TMA reduce (rounded again)
         want = resid.double() + pre
         tol = U * want.abs() + (1 + U) * (e_pre + U * pre.abs())
-    else:  # fp32 residual: acc + bias added into out by an fp32 TMA reduce
-        want = resid.double() + pre
-        tol = e_pre + F32 * want.abs()
     err = (got - want).abs()
     if bool((err > tol).any()):
         m, n = (err > tol).nonzero()[0].tolist()
         raise AssertionError(f"{what}: out[{m},{n}] = {float(got[m, n])}, want {float(want[m, n])} (tol {float(tol[m, n])})")
 
 
-@pytest.mark.parametrize("epi", ["bf16", "gelu", "resid_f32", "resid_f32_copy", "resid_bf16"])
+@pytest.mark.parametrize("epi", ["bf16", "gelu", "resid_bf16"])
 @pytest.mark.parametrize("M", [1, 2, 127, 129])
 def test_linear_edge_shapes_vs_fp64(epi, M):
     """M around one 128-row tile, K tails below the 64-wide k-block (8, 72 = 64 + 8, 136 = 128 + 8), N column tails inside
     a 64-column output box (8, 136, 200: 200 also takes the per-element bias path for its last chunk), with and without
-    bias, tight and padded row pitches.  resid_f32_copy is SGPT_EPI_RESID_F32 with resid != out (resid has the row pitch
-    ldo of out): out must become resid + x w^T + b and resid must keep its bits."""
+    bias, tight and padded row pitches."""
     for K in (8, 72, 136):
         for N in (8, 136, 200):
             for with_bias in (True, False):

@@ -29,10 +29,12 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(handle, name), f"{name} declared in include/sgpt_b200.h but not exported"
     assert sorted(_lib.exported_symbols()) == declared, "ctypes signature table out of sync with the header"
     lib = _lib.lib()
-    assert lib.sgpt_abi_version() == _lib.ABI_VERSION == 3
+    assert lib.sgpt_abi_version() == _lib.ABI_VERSION == 4
     # argument validation happens before any CUDA call, so it is checkable without a GPU
     assert lib.sgpt_linear(None, 8, None, 8, None, None, 8, None, 4, 4, 7, 0, None) == 1  # K % 8 != 0
     assert b"multiples of 8" in lib.sgpt_last_error()
+    assert lib.sgpt_linear(None, 8, None, 8, None, None, 8, None, 4, 4, 8, 2, None) == 1  # no epilogue 2 (fp32 residual)
+    assert b"unknown epilogue 2" in lib.sgpt_last_error()
     assert lib.sgpt_topk(None, 4, 1, 8, 3, 0, None, None, None, None) == 1  # lds < n
 
 

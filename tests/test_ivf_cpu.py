@@ -59,7 +59,15 @@ REJECTIONS = [
 ]
 
 
-@pytest.mark.parametrize("bad,msg", REJECTIONS, ids=[",".join(f"{k}={v}" for k, v in b.items()) for b, _ in REJECTIONS])
+PTR_ARGS = {"Q", "C", "offsets", "ids", "probes", "out_s", "out_i", "ws"}
+
+
+def _case_id(bad):
+    """Test id of a rejection.  A pointer is named by its offset from P: the address itself changes from run to run."""
+    return ",".join(f"{k}=P+{v - P}" if k in PTR_ARGS and v is not None else f"{k}={v}" for k, v in bad.items())
+
+
+@pytest.mark.parametrize("bad,msg", REJECTIONS, ids=[_case_id(b) for b, _ in REJECTIONS])
 def test_ivf_search_rejects_bad_arguments(bad, msg):
     """Each rejection returns SGPT_ERR_INVALID with its message, before any CUDA call (no GPU needed)."""
     assert _call(**bad) == 1

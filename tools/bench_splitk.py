@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Residual (reduce-add) GEMMs of every config with SGPT_GEMM_SPLITK forced to 0 / 2 / 3 / 4 and automatic, isolated
-launches with the L2 flushed, bf16 and fp32 residual streams.  Usage: python tools/bench_splitk.py [--iters 20]"""
+launches with the L2 flushed.  Usage: python tools/bench_splitk.py [--iters 20]"""
 import argparse
 import json
 import os
@@ -47,20 +47,18 @@ def main():
         x = torch.randn(M, K, generator=g, device=dev).to(bf)
         w = (torch.randn(N, K, generator=g, device=dev) * 0.02).to(bf)
         bias = torch.randn(N, generator=g, device=dev) * 0.1
-        for code, name in ((L.EPI_RESID_BF16, "bf16"), (L.EPI_RESID_F32, "f32")):
-            r = torch.zeros(M, N, device=dev, dtype=bf if name == "bf16" else torch.float32)
-            res = {"gemm": label, "M": M, "N": N, "K": K, "resid": name}
-            for setting in ("0", "2", "3", "4", None):
-                if setting is None:
-                    os.environ.pop("SGPT_GEMM_SPLITK", None)
-                else:
-                    os.environ["SGPT_GEMM_SPLITK"] = setting
-                t = timeit(lambda: L.check(lib.sgpt_linear(x.data_ptr(), K, w.data_ptr(), K, bias.data_ptr(), r.data_ptr(), N,
-                                                           r.data_ptr(), M, N, K, code, st)))
-                res["auto" if setting is None else "split" + setting] = {"us": round(1e3 * t, 1),
-                                                                       "tflops": round(2.0 * M * N * K / t / 1e9, 1)}
-            print(json.dumps(res), flush=True)
-            r.zero_()
+        r = torch.zeros(M, N, device=dev, dtype=bf)
+        res = {"gemm": label, "M": M, "N": N, "K": K}
+        for setting in ("0", "2", "3", "4", None):
+            if setting is None:
+                os.environ.pop("SGPT_GEMM_SPLITK", None)
+            else:
+                os.environ["SGPT_GEMM_SPLITK"] = setting
+            t = timeit(lambda: L.check(lib.sgpt_linear(x.data_ptr(), K, w.data_ptr(), K, bias.data_ptr(), r.data_ptr(), N,
+                                                       r.data_ptr(), M, N, K, L.EPI_RESID_BF16, st)))
+            res["auto" if setting is None else "split" + setting] = {"us": round(1e3 * t, 1),
+                                                                   "tflops": round(2.0 * M * N * K / t / 1e9, 1)}
+        print(json.dumps(res), flush=True)
 
 
 if __name__ == "__main__":
