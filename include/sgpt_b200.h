@@ -424,12 +424,26 @@ int sgpt_search_gather_masked(int dtype, sgpt_gather_t g, const void* Q, const v
  * nlist < 1, nprobe outside [1, nlist], k outside [1, 4096], n outside [0, 2^31), max_list_len outside [0, n],
  * nprobe x max_list_len beyond the selection's 2^32 entries, null inputs or outputs, an unaligned Q and a workspace
  * smaller than sgpt_ivf_search_workspace_bytes (which returns -1 for arguments the search rejects).
+ *
+ * sgpt_ivf_search_masked: the same search with a filter, shared or per query, in the mask format of the masked searches
+ * above, indexed by row position of C (list order): mask_pitch_words = 0: one bitmap [ceil(n/32)] shared by all queries
+ * (sgpt_ivf_search's `mask`); mask_pitch_words >= ceil(n/32): one bitmap per query, [nq][pitch]; NULL with pitch 0:
+ * every row allowed.  Bits at or past n are ignored.  The result is exactly sgpt_ivf_search's over the allowed rows of
+ * each query's probed lists (same scores, order and tie rule, tail (-inf, -1)); a masked row never appears.  The probes
+ * are the caller's and do not see the mask.  sgpt_ivf_search(..., mask, ...) is this call with pitch 0, and the workspace
+ * is the same.  SGPT_ERR_INVALID, before any CUDA call, for sgpt_ivf_search's rejections and, as in the masked searches,
+ * a negative pitch, 0 < pitch < ceil(n/32) and a non-zero pitch with a NULL mask.
  * ------------------------------------------------------------------------------------------------------------------ */
 int64_t sgpt_ivf_search_workspace_bytes(int dtype, int nq, int nlist, int nprobe, int64_t max_list_len, int D);
 int sgpt_ivf_search(int dtype, const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq,
                     int64_t n, int D, const int64_t* list_offsets, int nlist, int64_t max_list_len,
                     const int32_t* doc_ids, const int32_t* probes, int nprobe, int k, const uint32_t* mask,
                     float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
+int sgpt_ivf_search_masked(int dtype, const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq,
+                           int64_t n, int D, const int64_t* list_offsets, int nlist, int64_t max_list_len,
+                           const int32_t* doc_ids, const int32_t* probes, int nprobe, int k, const uint32_t* mask,
+                           int64_t mask_pitch_words, float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes,
+                           sgpt_stream_t stream);
 
 /* bf16 -> fp32 conversion of count elements (count % 4 == 0), e.g. of the residual stream. */
 int sgpt_bf16_to_f32(const void* x, float* y, int64_t count, sgpt_stream_t stream);

@@ -150,26 +150,16 @@ int launch_sample_maxima(const void* Q, const void* C, const float* q_scale, con
   return launch_filter_any(Q, C, nq, n, D, p, mask, stream, tm, s8);
 }
 
-int launch_ivf_scan(const void* A, int rows, const void* C, int n, int D, const IvfRowsParams& p, bool s8,
-                    cudaStream_t stream) {
-  SGPT_REQUIRE(rows > 0 && n > 0 && p.max_units > 0, "IVF scan: empty launch (rows=%d n=%d units=%d)", rows, n,
-               p.max_units);
-  using Cfg = GemmCfg<kSimBN, EpiStaging<EpiIvfRows>::value>;
-  auto make_map = s8 ? make_tma_2d_u8 : make_tma_2d_bf16;
-  const uint32_t box_k = s8 ? 2 * kGemmBK : kGemmBK;
-  CUtensorMap ta, tb;
-  int rc = make_map(&ta, A, static_cast<uint64_t>(rows), static_cast<uint64_t>(D), static_cast<uint64_t>(D), kGemmBM,
-                    box_k);
-  if (rc != SGPT_OK) return rc;
-  rc = make_map(&tb, C, static_cast<uint64_t>(n), static_cast<uint64_t>(D), static_cast<uint64_t>(D), kSimBN, box_k);
-  if (rc != SGPT_OK) return rc;
-  auto kern = s8 ? gemm_bf16_tn_kernel<kSimBN, EpiIvfRows, 1, true, true>
-                 : gemm_bf16_tn_kernel<kSimBN, EpiIvfRows, 1, false, true>;
+template <class Epi>
+static int launch_ivf_units(const CUtensorMap& ta, const CUtensorMap& tb, int rows, int n, int D,
+                            const typename Epi::Params& p, bool s8, cudaStream_t stream) {
+  using Cfg = GemmCfg<kSimBN, EpiStaging<Epi>::value>;
+  auto kern = s8 ? gemm_bf16_tn_kernel<kSimBN, Epi, 1, true, true> : gemm_bf16_tn_kernel<kSimBN, Epi, 1, false, true>;
   static PerDeviceOnce attr_once;
   if (attr_once.first()) {
-    SGPT_CHECK_CUDA(cudaFuncSetAttribute(gemm_bf16_tn_kernel<kSimBN, EpiIvfRows, 1, true, true>,
+    SGPT_CHECK_CUDA(cudaFuncSetAttribute(gemm_bf16_tn_kernel<kSimBN, Epi, 1, true, true>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    SGPT_CHECK_CUDA(cudaFuncSetAttribute(gemm_bf16_tn_kernel<kSimBN, EpiIvfRows, 1, false, true>,
+    SGPT_CHECK_CUDA(cudaFuncSetAttribute(gemm_bf16_tn_kernel<kSimBN, Epi, 1, false, true>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
   }
   // the unit count is only known on the device: one persistent CTA per SM, at most one per possible unit
@@ -178,6 +168,27 @@ int launch_ivf_scan(const void* A, int rows, const void* C, int n, int D, const 
   SGPT_CHECK_CUDA(launch_kernel(kern, dim3(static_cast<unsigned>(ctas)), dim3(kGemmThreads), Cfg::kSmemBytes, stream, ta,
                                 tb, rows, n, D, p, TileMap()));
   return SGPT_OK;
+}
+
+int launch_ivf_scan(const void* A, int rows, const void* C, int n, int D, const IvfRowsParams& p, long long mask_pitch,
+                    int nprobe, bool s8, cudaStream_t stream) {
+  SGPT_REQUIRE(rows > 0 && n > 0 && p.max_units > 0, "IVF scan: empty launch (rows=%d n=%d units=%d)", rows, n,
+               p.max_units);
+  SGPT_REQUIRE(mask_pitch == 0 || (p.mask != nullptr && nprobe > 0), "IVF scan: per-query masks need a bitmap");
+  auto make_map = s8 ? make_tma_2d_u8 : make_tma_2d_bf16;
+  const uint32_t box_k = s8 ? 2 * kGemmBK : kGemmBK;
+  CUtensorMap ta, tb;
+  int rc = make_map(&ta, A, static_cast<uint64_t>(rows), static_cast<uint64_t>(D), static_cast<uint64_t>(D), kGemmBM,
+                    box_k);
+  if (rc != SGPT_OK) return rc;
+  rc = make_map(&tb, C, static_cast<uint64_t>(n), static_cast<uint64_t>(D), static_cast<uint64_t>(D), kSimBN, box_k);
+  if (rc != SGPT_OK) return rc;
+  if (mask_pitch == 0) return launch_ivf_units<EpiIvfRows>(ta, tb, rows, n, D, p, s8, stream);
+  IvfRowsMaskedParams pm;
+  static_cast<IvfRowsParams&>(pm) = p;
+  pm.mask_pitch = mask_pitch;
+  pm.nprobe = nprobe;
+  return launch_ivf_units<EpiIvfRowsMasked>(ta, tb, rows, n, D, pm, s8, stream);
 }
 
 int launch_scores(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* scores, long long lds,

@@ -911,8 +911,16 @@ using EpiFilterRowsMasked = EpiFilterRowsT<true>;
 // tiles of the list the slots 0 .. len - 1 of the list are filled.  A position the shared bitmap excludes (deletions) is
 // written as an empty slot, id -1.  Slots are written two per 16-byte store (slot 0 is 16-byte aligned: Ls is even).
 // Params: gemm_api.h IvfRowsParams.
-struct EpiIvfRows {
-  using Params = IvfRowsParams;
+//
+// kPerQuery (sgpt_ivf_search_masked with a pitch): every pair row reads its own query's bitmap (query = row_info.x /
+// nprobe inside the block) instead of the shared one.  List starts are not multiples of 32, so the row's 32 positions
+// n .. n + 31 of a chunk straddle two mask words: both are loaded and the row's 32 bits taken with a funnel shift; a
+// position whose bit is 0 becomes an empty slot, as a deletion does.  pre_tile only prefetches the row's words into L1
+// (words held in registers across the mainloop would spill it).  The shared instantiation compiles to the code it had
+// before the per-query mask existed.
+template <bool kPerQuery>
+struct EpiIvfRowsT {
+  using Params = typename std::conditional<kPerQuery, IvfRowsMaskedParams, IvfRowsParams>::type;
   struct State {
     float4 cs;  // document scales n0 + 4 lane .. + 3 of the warp's half tile (broadcast by shuffles)
     float rs;   // this row's query scale
@@ -943,7 +951,13 @@ struct EpiIvfRows {
     }
     // the ids (and mask words) tile() reads once the accumulator is ready
     if (c < N) asm volatile("prefetch.global.L1 [%0];" ::"l"(p.doc_ids + c));
-    if (p.mask != nullptr && lane < 4 && n0 + 32 * lane < N) {
+    if constexpr (kPerQuery) {
+      if (rok) {  // the row's words of positions n0 .. min(n0 + 128, N) - 1 (at most 5 words, at most two L1 lines)
+        const uint32_t* w = p.mask + static_cast<long long>(info.x / p.nprobe) * p.mask_pitch;
+        asm volatile("prefetch.global.L1 [%0];" ::"l"(w + (n0 >> 5)));
+        asm volatile("prefetch.global.L1 [%0];" ::"l"(w + ((min(n0 + COLS, N) - 1) >> 5)));
+      }
+    } else if (p.mask != nullptr && lane < 4 && n0 + 32 * lane < N) {
       asm volatile("prefetch.global.L1 [%0];" ::"l"(p.mask + ((n0 + 32 * lane) >> 5)));
     }
   }
@@ -957,6 +971,8 @@ struct EpiIvfRows {
     const float csv[4] = {st.cs.x, st.cs.y, st.cs.z, st.cs.w};
     // dst[pos] = the slot of position pos in this row's list
     uint2* dst = p.cand + static_cast<long long>(rok ? st.list : 0) * p.Ls - st.begin;
+    const uint32_t* qmask = nullptr;  // kPerQuery: this row's query's bitmap
+    if constexpr (kPerQuery) qmask = p.mask + static_cast<long long>(rok ? st.list / p.nprobe : 0) * p.mask_pitch;
 #pragma unroll 1
     for (int c = 0; c < COLS; c += 32) {
       const int n = n0 + c;
@@ -968,7 +984,16 @@ struct EpiIvfRows {
       int gid = -1;
       if (pos < N) {
         gid = __ldg(p.doc_ids + pos);
-        if (p.mask != nullptr && !((__ldg(p.mask + (pos >> 5)) >> (pos & 31)) & 1u)) gid = -1;
+        if (!kPerQuery && p.mask != nullptr && !((__ldg(p.mask + (pos >> 5)) >> (pos & 31)) & 1u)) gid = -1;
+      }
+      // kPerQuery: bit i = position n + i allowed for this row's query.  n < N <= the corpus size, so word n / 32 exists;
+      // the next word is read only when it holds a position below N
+      uint32_t allow = 0xffffffffu;
+      if constexpr (kPerQuery) {
+        const int w = n >> 5, s = n & 31;
+        const uint32_t lo = rok ? __ldg(qmask + w) : 0u;
+        const uint32_t hi = (rok && s != 0 && (w + 1) * 32 < N) ? __ldg(qmask + w + 1) : 0u;
+        allow = __funnelshift_r(lo, hi, s);
       }
       float cs[32];
 #pragma unroll
@@ -980,7 +1005,11 @@ struct EpiIvfRows {
         float x1 = __uint_as_float(v[i + 1]) * rs * cs[i + 1];
         x0 = (x0 != x0) ? -1.f : x0;
         x1 = (x1 != x1) ? -1.f : x1;
-        const int g0 = __shfl_sync(0xffffffffu, gid, i), g1 = __shfl_sync(0xffffffffu, gid, i + 1);
+        int g0 = __shfl_sync(0xffffffffu, gid, i), g1 = __shfl_sync(0xffffffffu, gid, i + 1);
+        if constexpr (kPerQuery) {
+          g0 = ((allow >> i) & 1u) ? g0 : -1;
+          g1 = ((allow >> (i + 1)) & 1u) ? g1 : -1;
+        }
         if (!rok) continue;
         if (full || n + i + 1 < N) {
           *reinterpret_cast<uint4*>(dst + n + i) =
@@ -992,6 +1021,8 @@ struct EpiIvfRows {
     }
   }
 };
+using EpiIvfRows = EpiIvfRowsT<false>;
+using EpiIvfRowsMasked = EpiIvfRowsT<true>;
 
 
 template <bool kGelu>

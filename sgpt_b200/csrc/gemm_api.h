@@ -65,7 +65,15 @@ struct IvfRowsParams {
   uint2* cand;              // [pairs of the block][Ls]
   long long Ls;             // entries per candidate list (even)
 };
-int launch_ivf_scan(const void* A, int rows, const void* C, int n, int D, const IvfRowsParams& p, bool s8,
-                    cudaStream_t stream);
+// The scan with one bitmap per query (gemm.cuh EpiIvfRowsT<true>): `mask` is the bitmap of the block's first query, and
+// pair row r reads the bitmap at mask + (row_info[r].x / nprobe) * mask_pitch.
+struct IvfRowsMaskedParams : IvfRowsParams {
+  long long mask_pitch;  // words between consecutive queries' bitmaps (> 0)
+  int nprobe;            // pairs per query: row_info.x / nprobe is the pair's query inside the block
+};
+// mask_pitch == 0: p.mask is null or one shared bitmap (EpiIvfRows); mask_pitch > 0: one bitmap per query of the block,
+// p.mask + q * mask_pitch for query q of the block (EpiIvfRowsMasked).
+int launch_ivf_scan(const void* A, int rows, const void* C, int n, int D, const IvfRowsParams& p, long long mask_pitch,
+                    int nprobe, bool s8, cudaStream_t stream);
 
 }  // namespace sgpt

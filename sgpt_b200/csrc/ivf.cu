@@ -12,7 +12,8 @@
 //   units    one warp per list: (block of <= 128 pair rows) x (256-document tile) work units, tile-major, so that the pair
 //            blocks of one tile run back to back on neighbouring CTAs and share the tile in L2.
 //   scan     the filter GEMM's mainloop over the unit table (gemm.cuh kUnits + EpiIvfRows): (score, global id) of every
-//            probed document into its pair's candidate list, deleted positions as empty slots.
+//            probed document into its pair's candidate list, positions the shared or the query's own bitmap excludes
+//            as empty slots (sgpt_ivf_search_masked; sgpt_ivf_search is its pitch-0 case).
 //   select   launch_topk_select over G = nprobe packed lists per query (global ids) with per-pair counts.
 // The list offsets and probes are device data: every read and write above is bounded by the clamped list ranges and
 // the workspace layout, so inconsistent inputs give wrong results, never an out-of-bounds access.
@@ -258,11 +259,13 @@ extern "C" int64_t sgpt_ivf_search_workspace_bytes(int dtype, int nq, int nlist,
   return make_layout(nq, nlist, nprobe, max_list_len, D, dtype == SGPT_DTYPE_I8 ? 1 : 2).total;
 }
 
-extern "C" int sgpt_ivf_search(int dtype, const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq,
-                               int64_t n, int D, const int64_t* list_offsets, int nlist, int64_t max_list_len,
-                               const int32_t* doc_ids, const int32_t* probes, int nprobe, int k, const uint32_t* mask,
-                               float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream_) {
-  const char* fn = "sgpt_ivf_search";
+namespace {
+
+// both entry points: `fn` names the one called in error messages
+int ivf_search(const char* fn, int dtype, const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq,
+               int64_t n, int D, const int64_t* list_offsets, int nlist, int64_t max_list_len, const int32_t* doc_ids,
+               const int32_t* probes, int nprobe, int k, const uint32_t* mask, int64_t mask_pitch, float* out_scores,
+               int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (check_sizes(fn, dtype, nq, nlist, nprobe, max_list_len, D) != SGPT_OK) return SGPT_ERR_INVALID;
   SGPT_REQUIRE(n >= 0 && n < (1ll << 31), "%s: corpus size n=%lld outside [0, 2^31)", fn, (long long)n);
@@ -276,6 +279,7 @@ extern "C" int sgpt_ivf_search(int dtype, const void* Q, const void* C, const fl
   const Layout w = make_layout(nq, nlist, nprobe, max_list_len, D, elem);
   SGPT_REQUIRE(ws != nullptr && ws_bytes >= w.total, "%s: workspace too small (%lld < %lld bytes)", fn,
                (long long)ws_bytes, (long long)w.total);
+  if (check_doc_mask(fn, n, DocMask{mask, mask_pitch}) != SGPT_OK) return SGPT_ERR_INVALID;
   if (nq == 0) return SGPT_OK;
   const bool s8 = dtype == SGPT_DTYPE_I8;
   const long long row_bytes = static_cast<long long>(D) * elem;
@@ -326,9 +330,11 @@ extern "C" int sgpt_ivf_search(int dtype, const void* Q, const void* C, const fl
                                       dim3(kThreads), 0, stream, hist, pair_off, unit_off, list_offsets, nlist, N, max_len,
                                       pairs, static_cast<int>(w.max_units), units));
       }
-      IvfRowsParams p{units, n_units, static_cast<int>(w.max_units), row_scale, c_scale, row_info, doc_ids, mask, cand,
-                      static_cast<long long>(w.Ls)};
-      const int rc = launch_ivf_scan(rows, static_cast<int>(pairs), C, N, D, p, s8, stream);
+      // per-query bitmaps: the block's queries start at query q0
+      const uint32_t* block_mask = mask != nullptr ? mask + q0 * mask_pitch : nullptr;
+      IvfRowsParams p{units, n_units, static_cast<int>(w.max_units), row_scale, c_scale, row_info, doc_ids, block_mask,
+                      cand, static_cast<long long>(w.Ls)};
+      const int rc = launch_ivf_scan(rows, static_cast<int>(pairs), C, N, D, p, mask_pitch, nprobe, s8, stream);
       if (rc != SGPT_OK) return rc;
     }
     TopkSrc src{};
@@ -345,4 +351,25 @@ extern "C" int sgpt_ivf_search(int dtype, const void* Q, const void* C, const fl
     if (rc != SGPT_OK) return rc;
   }
   return SGPT_OK;
+}
+
+}  // namespace
+
+extern "C" int sgpt_ivf_search(int dtype, const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq,
+                               int64_t n, int D, const int64_t* list_offsets, int nlist, int64_t max_list_len,
+                               const int32_t* doc_ids, const int32_t* probes, int nprobe, int k, const uint32_t* mask,
+                               float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream) {
+  return ivf_search("sgpt_ivf_search", dtype, Q, C, q_scale, c_scale, nq, n, D, list_offsets, nlist, max_list_len,
+                    doc_ids, probes, nprobe, k, mask, 0, out_scores, out_ids, ws, ws_bytes, stream);
+}
+
+extern "C" int sgpt_ivf_search_masked(int dtype, const void* Q, const void* C, const float* q_scale,
+                                      const float* c_scale, int nq, int64_t n, int D, const int64_t* list_offsets,
+                                      int nlist, int64_t max_list_len, const int32_t* doc_ids, const int32_t* probes,
+                                      int nprobe, int k, const uint32_t* mask, int64_t mask_pitch_words,
+                                      float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes,
+                                      sgpt_stream_t stream) {
+  return ivf_search("sgpt_ivf_search_masked", dtype, Q, C, q_scale, c_scale, nq, n, D, list_offsets, nlist,
+                    max_list_len, doc_ids, probes, nprobe, k, mask, mask_pitch_words, out_scores, out_ids, ws, ws_bytes,
+                    stream);
 }

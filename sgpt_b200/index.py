@@ -108,6 +108,14 @@ def _bit_slice(words: torch.Tensor, start: int, n: int) -> torch.Tensor:
     return torch.where(s >= 2 ** 31, s - 2 ** 32, s).to(torch.int32)
 
 
+def _check_allow(allow, device, n: int, nq: int) -> torch.Tensor:
+    """`allow` of a search of nq queries over n documents as a device tensor: boolean [n] or [nq, n], else ValueError."""
+    allow = torch.as_tensor(allow, device=device)
+    if allow.dtype != torch.bool or allow.shape not in ((n,), (nq, n)):
+        raise ValueError(f"allow must be a boolean tensor [{n}] or [{nq}, {n}], got {allow.dtype} {tuple(allow.shape)}")
+    return allow
+
+
 def _check_dtype(dtype: str, dim: int) -> None:
     if dtype not in SHARD_DTYPES:
         raise ValueError(f"shard dtype {dtype!r} must be one of {SHARD_DTYPES}")
@@ -267,11 +275,7 @@ class CorpusShard:
         deleted = _bit_slice(self._deleted["words"], self._deleted_at, self.n) if self._deleted["any"] else None
         if allow is None:
             return (None, 0) if deleted is None else (torch.bitwise_not(deleted).contiguous(), 0)
-        allow = torch.as_tensor(allow, device=self.device)
-        if allow.dtype != torch.bool or allow.shape not in ((self.n,), (nq, self.n)):
-            raise ValueError(f"allow must be a boolean tensor [{self.n}] or [{nq}, {self.n}], got {allow.dtype} "
-                             f"{tuple(allow.shape)}")
-        m = pack_mask(allow)
+        m = pack_mask(_check_allow(allow, self.device, self.n, nq))
         if deleted is not None:
             m = m & torch.bitwise_not(deleted)
         return m.contiguous(), (m.shape[1] if m.dim() == 2 and self.n > 0 else 0)

@@ -20,7 +20,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .index import CorpusShard, _bit_slice, _check_score_function, unpack_mask
+from .index import CorpusShard, _bit_slice, _check_allow, _check_score_function, unpack_mask
 
 FORMAT = "sgpt_b200.IVFIndex/1"
 _ASSIGN_BYTES = 256 << 20  # score matrix of one assignment batch (dense search over the centroids)
@@ -41,6 +41,14 @@ def _assign(cshard: CorpusShard, x: torch.Tensor, score_function: str) -> torch.
     return torch.cat(out) if out else torch.empty(0, dtype=torch.int64, device=x.device)
 
 
+def _assign_rows(cshard: CorpusShard, shard: CorpusShard, score_function: str) -> torch.Tensor:
+    """Best centroid of every stored row of `shard` (dequantized), in batches of ~256 MB of fp32 rows: int64 [n]."""
+    n, D, dev = shard.n, shard.dim, shard.device
+    bs = max(1, min(65536, _ASSIGN_BYTES // (4 * D)))
+    return torch.cat([_assign(cshard, _rows_f32(shard, torch.arange(i, min(i + bs, n), device=dev)), score_function)
+                      for i in range(0, n, bs)])
+
+
 class IVFIndex:
     """IVF index on one GPU.  Built by ``IVFIndex.build`` or ``IVFIndex.load``.
 
@@ -51,15 +59,20 @@ class IVFIndex:
     def __init__(self, shard: CorpusShard, centroids: torch.Tensor, offsets: torch.Tensor, ids: torch.Tensor,
                  id_base: int, score_function: str):
         _check_score_function(score_function)
-        self.shard, self.score_function, self.id_base = shard, score_function, int(id_base)
+        self.score_function, self.id_base = score_function, int(id_base)
         self.device = shard.device
         self.centroids = centroids.to(self.device, torch.float32).contiguous()
+        self.nlist, self.dim, self.dtype = self.centroids.shape[0], shard.dim, shard.dtype
+        self._cshard = CorpusShard.from_embeddings(self.centroids, device=self.device)
+        self._set_lists(shard, offsets, ids)
+
+    def _set_lists(self, shard: CorpusShard, offsets: torch.Tensor, ids: torch.Tensor) -> None:
+        """The list-ordered rows and their layout (``build``, ``load``, ``add``)."""
+        self.shard, self.n = shard, shard.n
         self.offsets = offsets.to(self.device, torch.int64).contiguous()
         self.ids = ids.to(self.device, torch.int32).contiguous()
-        self.nlist, self.dim, self.n, self.dtype = self.centroids.shape[0], shard.dim, shard.n, shard.dtype
         self.list_sizes = (self.offsets[1:] - self.offsets[:-1]).cpu()
         self.max_list_len = int(self.list_sizes.max()) if self.nlist else 0
-        self._cshard = CorpusShard.from_embeddings(self.centroids, device=self.device)
         # position of every global id (ids are a permutation of id_base .. id_base + n - 1)
         self._pos = torch.empty(self.n, dtype=torch.int64, device=self.device)
         self._pos[self.ids.long() - self.id_base] = torch.arange(self.n, device=self.device)
@@ -121,10 +134,7 @@ class IVFIndex:
                 new = torch.nn.functional.normalize(new, dim=1)
             cent = new.float().to(dev)
         del x
-        cshard = CorpusShard.from_embeddings(cent, device=dev)
-        bs = max(1, min(65536, _ASSIGN_BYTES // (4 * D)))
-        assign = torch.cat([_assign(cshard, _rows_f32(src, torch.arange(i, min(i + bs, n), device=dev)), score_function)
-                            for i in range(0, n, bs)])
+        assign = _assign_rows(CorpusShard.from_embeddings(cent, device=dev), src, score_function)
         perm = torch.sort(assign, stable=True).indices
         offsets = torch.zeros(nlist + 1, dtype=torch.int64, device=dev)
         torch.cumsum(torch.bincount(assign, minlength=nlist), 0, out=offsets[1:])
@@ -149,16 +159,27 @@ class IVFIndex:
             raise ValueError(f"nprobe={nprobe} must lie in [1, nlist={self.nlist}]")
         return self._cshard.search(queries.to(self.device), int(nprobe), self.score_function)[1].to(torch.int32)
 
-    def search(self, queries: torch.Tensor, k: int, nprobe: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    def search(self, queries: torch.Tensor, k: int, nprobe: int,
+               allow: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
         """Top-k of the undeleted documents in each query's ``nprobe`` probed lists, for fp32/bf16 queries [Q, D]:
         (scores fp32 [Q, k] descending, global ids int64 [Q, k]), tail (-inf, -1) when fewer than k are probed.  Scores,
-        order and ties are those of ``CorpusShard.search`` on the same stored rows."""
+        order and ties are those of ``CorpusShard.search`` on the same stored rows.
+
+        ``allow``: boolean device tensor [n] (all queries) or [Q, n] (one row per query), indexed by global id - id_base
+        as in ``CorpusShard.search``: only those documents may be returned.  The probes do not depend on the filter —
+        they are still the ``nprobe`` nearest centroids — so a selective filter can return fewer than k documents even
+        where the whole index holds more.  The result is exactly ``CorpusShard.search(allow=allow & probed)``."""
         if not 1 <= int(k) <= 4096:
             raise ValueError(f"k={k} must lie in [1, 4096]")
         probes = self.probe(queries, nprobe)
         qb, q_scale, c_scale = self.shard._queries(queries, self.score_function)
         nq = qb.shape[0]
-        mask, _ = self.shard._mask(None, nq)
+        if allow is None:
+            mask, pitch = self.shard._mask(None, nq)
+        else:
+            # document order -> list order with one gather, then packed with the deletions ANDed in
+            allow = _check_allow(allow, self.device, self.n, nq)
+            mask, pitch = self.shard._mask(allow.index_select(-1, self.ids - self.id_base), nq)
         dt = self.shard._dtype_id()
         lib = _lib.lib()
         need = lib.sgpt_ivf_search_workspace_bytes(dt, nq, self.nlist, int(nprobe), self.max_list_len, self.dim)
@@ -169,13 +190,68 @@ class IVFIndex:
         out_s = torch.empty((nq, k), dtype=torch.float32, device=self.device)
         out_i = torch.empty((nq, k), dtype=torch.int64, device=self.device)
         with torch.cuda.device(self.device):
-            rc = lib.sgpt_ivf_search(dt, qb.data_ptr(), self.shard.vectors.data_ptr(), _lib.ptr(q_scale), c_scale, nq,
-                                     self.n, self.dim, self.offsets.data_ptr(), self.nlist, self.max_list_len,
-                                     self.ids.data_ptr(), probes.data_ptr(), int(nprobe), int(k), _lib.ptr(mask),
-                                     out_s.data_ptr(), out_i.data_ptr(), self._ws.data_ptr(), self._ws.numel(),
-                                     _lib.current_stream())
+            if allow is None:
+                rc = lib.sgpt_ivf_search(dt, qb.data_ptr(), self.shard.vectors.data_ptr(), _lib.ptr(q_scale), c_scale,
+                                         nq, self.n, self.dim, self.offsets.data_ptr(), self.nlist, self.max_list_len,
+                                         self.ids.data_ptr(), probes.data_ptr(), int(nprobe), int(k), _lib.ptr(mask),
+                                         out_s.data_ptr(), out_i.data_ptr(), self._ws.data_ptr(), self._ws.numel(),
+                                         _lib.current_stream())
+            else:
+                rc = lib.sgpt_ivf_search_masked(dt, qb.data_ptr(), self.shard.vectors.data_ptr(), _lib.ptr(q_scale),
+                                                c_scale, nq, self.n, self.dim, self.offsets.data_ptr(), self.nlist,
+                                                self.max_list_len, self.ids.data_ptr(), probes.data_ptr(), int(nprobe),
+                                                int(k), _lib.ptr(mask), pitch, out_s.data_ptr(), out_i.data_ptr(),
+                                                self._ws.data_ptr(), self._ws.numel(), _lib.current_stream())
         _lib.check(rc, "sgpt_ivf_search")
         return out_s, out_i
+
+    def add(self, emb: torch.Tensor) -> None:
+        """Append fp32/bf16 embeddings [m, D] as documents id_base + n .. id_base + n + m - 1 (as ``CorpusShard.add``).
+
+        The rows are stored as ``CorpusShard.add`` stores them for the index's dtype, and each goes to the list of its
+        best centroid — the assignment of ``build``'s final pass, on the stored row.  Every list keeps its rows in their
+        order, followed by its new rows in input order; deletions stay with their documents and new rows start
+        undeleted.  The centroids are never retrained, so after heavy growth or drift of the data rebuild the index.
+
+        The inner shard is rebuilt out of place: peak device memory is the old index plus the new one plus the m rows
+        staged in the index's format (and one assignment batch, as in ``build``)."""
+        m = int(emb.shape[0])
+        if emb.dim() != 2 or emb.shape[1] != self.dim:
+            raise ValueError(f"add: embeddings must be [m, {self.dim}], got {tuple(emb.shape)}")
+        if self.id_base + self.n + m >= 2 ** 31:
+            raise ValueError(f"add: global ids must fit in int32 (id_base + n + m = {self.id_base + self.n + m} >= 2^31)")
+        if m == 0:
+            return
+        n, dev, old = self.n, self.device, self.shard
+        new = CorpusShard.from_embeddings(emb.to(dev), device=dev, dtype=self.dtype)
+        lists = _assign_rows(self._cshard, new, self.score_function)
+        added = torch.bincount(lists, minlength=self.nlist)
+        shift = torch.cumsum(added, 0) - added  # new rows inserted before list l
+        sizes = self.offsets[1:] - self.offsets[:-1]
+        offsets = self.offsets.clone()
+        offsets[1:] += torch.cumsum(added, 0)
+        # destinations: old position p of list l -> p + shift[l]; new rows after their list's old rows, in input order
+        old_list = torch.repeat_interleave(torch.arange(self.nlist, device=dev), sizes, output_size=n)
+        old_dest = torch.arange(n, device=dev) + shift[old_list]
+        order = torch.sort(lists, stable=True).indices
+        rank = torch.arange(m, device=dev) - shift[lists[order]]  # place inside the list's new rows
+        new_dest = torch.empty(m, dtype=torch.int64, device=dev)
+        new_dest[order] = offsets[lists[order]] + sizes[lists[order]] + rank
+        inner = CorpusShard(self.dim, n + m, device=dev, dtype=self.dtype)
+        fields = ("vectors", "scales", "cos_scales") if self.dtype == "int8" else ("vectors", "inv_norms")
+        for f in fields:
+            dst = getattr(inner, f)[:n + m]
+            dst.index_copy_(0, old_dest, getattr(old, f)[:n])
+            dst.index_copy_(0, new_dest, getattr(new, f)[:m])
+        inner.n = n + m
+        ids = torch.empty(n + m, dtype=torch.int32, device=dev)
+        ids[old_dest] = self.ids
+        ids[new_dest] = torch.arange(self.id_base + n, self.id_base + n + m, dtype=torch.int32, device=dev)
+        if old._deleted["any"]:
+            deleted = unpack_mask(_bit_slice(old._deleted["words"], old._deleted_at, n), n)
+            inner.remove(old_dest[deleted])
+        del new
+        self._set_lists(inner, offsets, ids)
 
     def remove(self, ids) -> None:
         """Delete documents by global id: no search returns them afterwards."""
