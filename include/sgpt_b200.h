@@ -445,6 +445,29 @@ int sgpt_ivf_search_masked(int dtype, const void* Q, const void* C, const float*
                            int64_t mask_pitch_words, float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes,
                            sgpt_stream_t stream);
 
+/* sgpt_ivf_range_search: threshold (range) search over the same lists.  Every input means what it means in
+ * sgpt_ivf_search_masked, with `threshold` in place of k.  Query q's result is every position of its probed lists whose
+ * score is >= threshold (a NaN score counts as -1), which the mask allows and whose doc_ids entry is >= 0, with the
+ * exact search's score bits: exactly the set sgpt_range_search_masked returns over those positions.
+ *   out_counts  int64 [nq] (device), always written.  The entries go to out_scores fp32 / out_ids int64 (global ids)
+ *               [cap] in query order, query q's at [off[q], off[q] + counts[q]) with off the exclusive sum of the counts,
+ *               if and only if off[q] + counts[q] <= cap; entries that do not fit are not written (those slots keep their
+ *               bits), and cap = 0 only counts.  The running offset carries across blocks of 256 queries on the device,
+ *               with no host synchronisation.
+ *   order       within a query, its probes in the order given, and within each probe ascending list position.  This is
+ *               NOT id order: sort by (query, id) for the order of sgpt_range_search.  No atomics decide any order, so a
+ *               second launch returns the same bits.
+ * The workspace holds sgpt_ivf_search's plus the compaction's per-pair and per-query offsets; the device inputs bound
+ * every access as in sgpt_ivf_search.  SGPT_ERR_INVALID, before any CUDA call, for sgpt_ivf_search_masked's rejections
+ * other than those about k, a NaN threshold, cap < 0, a null out_counts, null out_scores or out_ids with cap > 0, and a
+ * workspace smaller than sgpt_ivf_range_search_workspace_bytes (which returns -1 for arguments the search rejects). */
+int64_t sgpt_ivf_range_search_workspace_bytes(int dtype, int nq, int nlist, int nprobe, int64_t max_list_len, int D);
+int sgpt_ivf_range_search(int dtype, const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq,
+                          int64_t n, int D, const int64_t* list_offsets, int nlist, int64_t max_list_len,
+                          const int32_t* doc_ids, const int32_t* probes, int nprobe, float threshold,
+                          const uint32_t* mask, int64_t mask_pitch_words, int64_t* out_counts, int64_t cap,
+                          float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
+
 /* bf16 -> fp32 conversion of count elements (count % 4 == 0), e.g. of the residual stream. */
 int sgpt_bf16_to_f32(const void* x, float* y, int64_t count, sgpt_stream_t stream);
 

@@ -116,6 +116,39 @@ def _check_allow(allow, device, n: int, nq: int) -> torch.Tensor:
     return allow
 
 
+def _mask_rows(mask: Tuple[Optional[torch.Tensor], int], first: int) -> Tuple[Optional[torch.Tensor], int]:
+    """The (bitmap, pitch) of a search's queries first .. : per-query bitmaps lose their first rows, a shared one stays."""
+    return (mask[0][first:], mask[1]) if mask[1] > 0 else mask
+
+
+def _grown_range(nq: int, device, run, capacity: Optional[int] = None
+                 ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """A range search in CSR form whose output buffer starts at `capacity` entries (default max(4096, 64 nq)) and grows
+    once.  ``run(first, counts, cap, out_s, out_i)`` runs the queries first .. nq - 1 into buffers of cap entries, writing
+    counts int64 [nq - first] always and the entries of the queries that fit (a prefix).  Returns (offsets int64 [nq+1],
+    scores, ids) in the order `run` writes them."""
+    cap = max(4096, 64 * nq) if capacity is None else max(1, int(capacity))
+    counts = torch.empty(nq, dtype=torch.int64, device=device)
+    out_s = torch.empty(cap, dtype=torch.float32, device=device)
+    out_i = torch.empty(cap, dtype=torch.int64, device=device)
+    run(0, counts, cap, out_s, out_i)
+    offsets = torch.zeros(nq + 1, dtype=torch.int64, device=device)
+    torch.cumsum(counts, 0, out=offsets[1:])
+    total = int(offsets[-1])
+    if total > cap:
+        # the queries that fitted are a prefix: grow the buffer and run the others once more into its tail
+        first = int(torch.searchsorted(offsets[1:], cap, right=True))
+        done = int(offsets[first])
+        grown_s = torch.empty(total, dtype=torch.float32, device=device)
+        grown_i = torch.empty(total, dtype=torch.int64, device=device)
+        grown_s[:done].copy_(out_s[:done])
+        grown_i[:done].copy_(out_i[:done])
+        rest = torch.empty(nq - first, dtype=torch.int64, device=device)
+        run(first, rest, total - done, grown_s[done:], grown_i[done:])
+        out_s, out_i = grown_s, grown_i
+    return offsets, out_s[:total], out_i[:total]
+
+
 def _check_dtype(dtype: str, dim: int) -> None:
     if dtype not in SHARD_DTYPES:
         raise ValueError(f"shard dtype {dtype!r} must be one of {SHARD_DTYPES}")
@@ -408,29 +441,10 @@ class CorpusShard:
     def _range(self, qb: torch.Tensor, q_scale: Optional[torch.Tensor], c_scale: Optional[int], threshold: float,
                capacity: Optional[int] = None, mask: Tuple[Optional[torch.Tensor], int] = (None, 0)
                ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
-        nq = qb.shape[0]
-        cap = max(4096, 64 * nq) if capacity is None else max(1, int(capacity))
-        counts = torch.empty(nq, dtype=torch.int64, device=self.device)
-        out_s = torch.empty(cap, dtype=torch.float32, device=self.device)
-        out_i = torch.empty(cap, dtype=torch.int64, device=self.device)
-        self._range_call(qb, q_scale, c_scale, threshold, counts, cap, out_s, out_i, mask)
-        offsets = torch.zeros(nq + 1, dtype=torch.int64, device=self.device)
-        torch.cumsum(counts, 0, out=offsets[1:])
-        total = int(offsets[-1])
-        if total > cap:
-            # the queries that fitted are a prefix: grow the buffer and run the others once more into its tail
-            first = int(torch.searchsorted(offsets[1:], cap, right=True))
-            done = int(offsets[first])
-            grown_s = torch.empty(total, dtype=torch.float32, device=self.device)
-            grown_i = torch.empty(total, dtype=torch.int64, device=self.device)
-            grown_s[:done].copy_(out_s[:done])
-            grown_i[:done].copy_(out_i[:done])
-            rest = torch.empty(nq - first, dtype=torch.int64, device=self.device)
-            rest_mask = (mask[0][first:], mask[1]) if mask[1] > 0 else mask  # per-query bitmaps: rows of the rest
-            self._range_call(qb[first:], None if q_scale is None else q_scale[first:], c_scale, threshold, rest,
-                             total - done, grown_s[done:], grown_i[done:], rest_mask)
-            out_s, out_i = grown_s, grown_i
-        return offsets, out_s[:total], out_i[:total]
+        def run(first, counts, cap, out_s, out_i):
+            self._range_call(qb[first:], None if q_scale is None else q_scale[first:], c_scale, threshold, counts, cap,
+                             out_s, out_i, _mask_rows(mask, first))
+        return _grown_range(qb.shape[0], self.device, run, capacity)
 
     def range_search(self, queries: torch.Tensor, threshold: float, score_function: str = "cos_sim",
                      allow: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:

@@ -9,6 +9,10 @@ The search is exact relative to its lists: ``IVFIndex.search`` returns exactly w
 the undeleted documents of the probed lists — the same scores of the same stored rows, the same order and tie rule on
 global ids, the tail (-inf, -1) when fewer than k documents are probed.  ``nprobe == nlist`` is the exact search.
 Recall against the full exact search depends on the clustering only.
+
+``IVFIndex.range_search`` is the threshold counterpart (``sgpt_ivf_range_search``): exactly ``CorpusShard.range_search``
+over the undeleted documents of the probed lists.  ``paraphrase_mining_embeddings`` and ``community_detection``
+(mining.py) run over an index with the stored rows themselves as queries.
 """
 from __future__ import annotations
 
@@ -20,7 +24,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .index import CorpusShard, _bit_slice, _check_allow, _check_score_function, unpack_mask
+from .index import (CorpusShard, _bit_slice, _check_allow, _check_score_function, _grown_range, _mask_rows,
+                    unpack_mask)
 
 FORMAT = "sgpt_b200.IVFIndex/1"
 _ASSIGN_BYTES = 256 << 20  # score matrix of one assignment batch (dense search over the centroids)
@@ -173,37 +178,129 @@ class IVFIndex:
             raise ValueError(f"k={k} must lie in [1, 4096]")
         probes = self.probe(queries, nprobe)
         qb, q_scale, c_scale = self.shard._queries(queries, self.score_function)
-        nq = qb.shape[0]
-        if allow is None:
-            mask, pitch = self.shard._mask(None, nq)
-        else:
-            # document order -> list order with one gather, then packed with the deletions ANDed in
-            allow = _check_allow(allow, self.device, self.n, nq)
-            mask, pitch = self.shard._mask(allow.index_select(-1, self.ids - self.id_base), nq)
-        dt = self.shard._dtype_id()
-        lib = _lib.lib()
-        need = lib.sgpt_ivf_search_workspace_bytes(dt, nq, self.nlist, int(nprobe), self.max_list_len, self.dim)
+        return self._search_rows(qb, q_scale, c_scale, probes, int(k), self._list_mask(allow, qb.shape[0]))
+
+    def range_search(self, queries: torch.Tensor, threshold: float, nprobe: int,
+                     allow: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """Every undeleted document of each query's ``nprobe`` probed lists whose score is >= threshold, for fp32/bf16
+        queries [Q, D]: (offsets int64 [Q+1], scores fp32 [E], global ids int64 [E]) on the device, query q's documents at
+        offsets[q] .. offsets[q+1] in ascending id order.  Queries are converted and scored as in ``search``; a NaN score
+        counts as -1.  The output buffer starts and grows once as in ``CorpusShard.range_search``.
+
+        ``allow`` as in ``search`` (boolean [n] or [Q, n], indexed by global id - id_base); the probes ignore it.  The
+        result is exactly ``CorpusShard.range_search(allow=allow & probed)`` of the source documents, deleted ones left
+        out: the same offsets, scores and ids."""
+        if threshold != threshold:
+            raise ValueError("threshold is NaN")
+        probes = self.probe(queries, nprobe)
+        qb, q_scale, c_scale = self.shard._queries(queries, self.score_function)
+        return self._range_rows(qb, q_scale, c_scale, probes, threshold, self._list_mask(allow, qb.shape[0]))
+
+    # ---- the calls behind search / range_search, on query rows in the shard's format --------------------------------
+    def _workspace(self, need: int, what: str) -> torch.Tensor:
         if need < 0:
-            raise ValueError(f"sgpt_ivf_search rejects nq={nq} nprobe={nprobe}: {lib.sgpt_last_error().decode()}")
+            raise ValueError(f"{what} rejects these arguments: {_lib.lib().sgpt_last_error().decode()}")
         if self._ws is None or self._ws.numel() < need:
             self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+        return self._ws
+
+    def _list_mask(self, allow: Optional[torch.Tensor], nq: int) -> Tuple[Optional[torch.Tensor], int]:
+        """(bitmap, pitch) over list positions: `allow` (document order) permuted to list order with one gather, then
+        packed with the deletions ANDed in (``CorpusShard._mask``)."""
+        if allow is None:
+            return self.shard._mask(None, nq)
+        allow = _check_allow(allow, self.device, self.n, nq)
+        return self.shard._mask(allow.index_select(-1, self.ids - self.id_base), nq)
+
+    def _search_rows(self, qb, q_scale, c_scale, probes, k: int, mask) -> Tuple[torch.Tensor, torch.Tensor]:
+        """sgpt_ivf_search (shared or no bitmap) or sgpt_ivf_search_masked (per-query bitmaps) of prepared rows."""
+        nq, nprobe = qb.shape[0], probes.shape[1]
+        dt, lib = self.shard._dtype_id(), _lib.lib()
+        ws = self._workspace(lib.sgpt_ivf_search_workspace_bytes(dt, nq, self.nlist, nprobe, self.max_list_len,
+                                                                 self.dim), "sgpt_ivf_search")
         out_s = torch.empty((nq, k), dtype=torch.float32, device=self.device)
         out_i = torch.empty((nq, k), dtype=torch.int64, device=self.device)
         with torch.cuda.device(self.device):
-            if allow is None:
+            if mask[1] == 0:
                 rc = lib.sgpt_ivf_search(dt, qb.data_ptr(), self.shard.vectors.data_ptr(), _lib.ptr(q_scale), c_scale,
                                          nq, self.n, self.dim, self.offsets.data_ptr(), self.nlist, self.max_list_len,
-                                         self.ids.data_ptr(), probes.data_ptr(), int(nprobe), int(k), _lib.ptr(mask),
-                                         out_s.data_ptr(), out_i.data_ptr(), self._ws.data_ptr(), self._ws.numel(),
+                                         self.ids.data_ptr(), probes.data_ptr(), nprobe, k, _lib.ptr(mask[0]),
+                                         out_s.data_ptr(), out_i.data_ptr(), ws.data_ptr(), ws.numel(),
                                          _lib.current_stream())
             else:
                 rc = lib.sgpt_ivf_search_masked(dt, qb.data_ptr(), self.shard.vectors.data_ptr(), _lib.ptr(q_scale),
                                                 c_scale, nq, self.n, self.dim, self.offsets.data_ptr(), self.nlist,
-                                                self.max_list_len, self.ids.data_ptr(), probes.data_ptr(), int(nprobe),
-                                                int(k), _lib.ptr(mask), pitch, out_s.data_ptr(), out_i.data_ptr(),
-                                                self._ws.data_ptr(), self._ws.numel(), _lib.current_stream())
+                                                self.max_list_len, self.ids.data_ptr(), probes.data_ptr(), nprobe, k,
+                                                _lib.ptr(mask[0]), mask[1], out_s.data_ptr(), out_i.data_ptr(),
+                                                ws.data_ptr(), ws.numel(), _lib.current_stream())
         _lib.check(rc, "sgpt_ivf_search")
         return out_s, out_i
+
+    def _range_call(self, qb, q_scale, c_scale, probes, threshold: float, mask, counts: torch.Tensor, cap: int,
+                    out_s: Optional[torch.Tensor], out_i: Optional[torch.Tensor]) -> None:
+        """One sgpt_ivf_range_search of prepared rows: counts int64 [Q] always, the entries of the queries that fit into
+        `cap` into out_s / out_i in the entry point's order (probe order, then list position)."""
+        nq, nprobe = qb.shape[0], probes.shape[1]
+        dt, lib = self.shard._dtype_id(), _lib.lib()
+        ws = self._workspace(lib.sgpt_ivf_range_search_workspace_bytes(dt, nq, self.nlist, nprobe, self.max_list_len,
+                                                                       self.dim), "sgpt_ivf_range_search")
+        with torch.cuda.device(self.device):
+            rc = lib.sgpt_ivf_range_search(dt, qb.data_ptr(), self.shard.vectors.data_ptr(), _lib.ptr(q_scale), c_scale,
+                                           nq, self.n, self.dim, self.offsets.data_ptr(), self.nlist, self.max_list_len,
+                                           self.ids.data_ptr(), probes.data_ptr(), nprobe, float(threshold),
+                                           _lib.ptr(mask[0]), mask[1], counts.data_ptr(), cap, _lib.ptr(out_s),
+                                           _lib.ptr(out_i), ws.data_ptr(), ws.numel(), _lib.current_stream())
+        _lib.check(rc, "sgpt_ivf_range_search")
+
+    def _range_rows(self, qb, q_scale, c_scale, probes, threshold: float, mask, capacity: Optional[int] = None
+                    ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """``_range_call`` through the grow-once buffer of ``CorpusShard._range``, then every query's entries sorted by
+        global id with one device sort of the unique keys q * 2^31 + id."""
+        nq = qb.shape[0]
+
+        def run(first, counts, cap, out_s, out_i):
+            self._range_call(qb[first:], None if q_scale is None else q_scale[first:], c_scale, probes[first:],
+                             threshold, _mask_rows(mask, first), counts, cap, out_s, out_i)
+
+        offsets, s, ids = _grown_range(nq, self.device, run, capacity)
+        q = torch.repeat_interleave(torch.arange(nq, device=self.device), offsets[1:] - offsets[:-1],
+                                    output_size=s.numel())
+        o = torch.sort(q * (1 << 31) + ids).indices
+        return offsets, s[o], ids[o]
+
+    # ---- the index's own rows as queries (mining) -------------------------------------------------------------------
+    def _undeleted(self) -> Optional[torch.Tensor]:
+        """Positions of the undeleted rows, ascending (int64), or None when nothing is deleted."""
+        if self.shard.n_deleted == 0:
+            return None
+        deleted = unpack_mask(_bit_slice(self.shard._deleted["words"], self.shard._deleted_at, self.n), self.n)
+        return (~deleted).nonzero().flatten()
+
+    def _stored_blocks(self, rows: int):
+        """The undeleted positions in position (= list) order, in blocks of at most `rows`: slices when nothing is
+        deleted, else int64 position tensors."""
+        keep = self._undeleted()
+        total = self.n if keep is None else keep.numel()
+        for a in range(0, total, rows):
+            b = min(a + rows, total)
+            yield slice(a, b) if keep is None else keep[a:b]
+
+    def _stored_queries(self, pos, nprobe: int):
+        """Stored rows at positions `pos` (a slice or an int64 tensor) as queries, with no re-quantization: (rows,
+        q_scale, c_scale, probes).  bf16 rows take their inv_norms (cos_sim) or no scale (dot); int8 rows their cos_scales
+        (cos_sim) or scales (dot).  The probes are those of the stored row (dequantized for int8).  A slice is a view of
+        the shard's rows, passed to the kernels as it is."""
+        sh, cos = self.shard, self.score_function == "cos_sim"
+        if isinstance(pos, slice):
+            take, idx = (lambda t: t[pos]), torch.arange(pos.start, pos.stop, device=self.device)
+        else:
+            take, idx = (lambda t: t.index_select(0, pos)), pos
+        if sh.dtype == "int8":
+            scales = sh.cos_scales if cos else sh.scales
+            q_scale, c_scale = take(scales), scales.data_ptr()
+        else:
+            q_scale, c_scale = (take(sh.inv_norms), sh.inv_norms.data_ptr()) if cos else (None, None)
+        return take(sh.vectors), q_scale, c_scale, self.probe(_rows_f32(sh, idx), nprobe)
 
     def add(self, emb: torch.Tensor) -> None:
         """Append fp32/bf16 embeddings [m, D] as documents id_base + n .. id_base + n + m - 1 (as ``CorpusShard.add``).

@@ -6,18 +6,24 @@ search kernels, which never write a score matrix: paraphrase mining takes each c
 and selects and deduplicates the pairs there with sorts over (score, i, j); community detection counts every row's
 documents above the threshold first and fetches the members of the qualifying rows only.  Host work is proportional
 to the result.
+
+Both also take an ``IVFIndex`` with ``nprobe``: every undeleted stored row is a query over the undeleted documents of
+its probed lists (the IVF search and IVF range search), so the cost grows with n x nprobe x the list length instead of
+n^2, and ``nprobe == nlist`` gives the exact functions' result.
 """
 from __future__ import annotations
 
-from typing import List, Tuple, Union
+from typing import List, Optional, Tuple, Union
 
 import torch
 
 from .index import CorpusShard, resolve_score_function
+from .ivf import IVFIndex
 
 MAX_K = 4096  # the library's top-k limit (include/sgpt_b200.h)
 _CANDIDATES_PER_STEP = 1 << 24  # row top-k entries selected per step of paraphrase mining
 _MEMBERS_PER_BLOCK = 1 << 26    # community members fetched per range search call
+_COUNT_ROWS = 1 << 16           # stored rows per count-only IVF range pass of community detection
 
 
 def _as_shard(embeddings: Union[torch.Tensor, CorpusShard]) -> CorpusShard:
@@ -31,6 +37,15 @@ def _as_shard(embeddings: Union[torch.Tensor, CorpusShard]) -> CorpusShard:
     if emb.dim() == 1:
         emb = emb.unsqueeze(0)
     return CorpusShard.from_embeddings(emb if emb.is_cuda else emb.to("cuda:0"))
+
+
+def _check_nprobe(embeddings, nprobe) -> None:
+    """`nprobe` goes with an IVFIndex and only with one."""
+    if isinstance(embeddings, IVFIndex):
+        if nprobe is None:
+            raise ValueError("mining an IVFIndex needs nprobe (the lists each row scans)")
+    elif nprobe is not None:
+        raise ValueError("nprobe applies to an IVFIndex only")
 
 
 def _tuple_order(s: torch.Tensor, i: torch.Tensor, j: torch.Tensor, n: int, descending: bool) -> torch.Tensor:
@@ -97,9 +112,9 @@ def paraphrase_mining(model, sentences: List[str], show_progress_bar: bool = Fal
     return paraphrase_mining_embeddings(embeddings, *args, **kwargs)
 
 
-def paraphrase_mining_embeddings(embeddings: Union[torch.Tensor, CorpusShard], query_chunk_size: int = 5000,
+def paraphrase_mining_embeddings(embeddings: Union[torch.Tensor, CorpusShard, IVFIndex], query_chunk_size: int = 5000,
                                  corpus_chunk_size: int = 100000, max_pairs: int = 500000, top_k: int = 100,
-                                 score_function="cos_sim") -> List[list]:
+                                 score_function="cos_sim", nprobe: Optional[int] = None) -> List[list]:
     """ST/util.py:129-189: the most similar pairs (i, j) inside one corpus, as ``[[score, i, j], ...]``, best first.
 
     For every corpus chunk of ``corpus_chunk_size`` documents every row takes its top min(top_k + 1, chunk length)
@@ -107,12 +122,21 @@ def paraphrase_mining_embeddings(embeddings: Union[torch.Tensor, CorpusShard], q
     therefore changes which candidates exist and is honoured.  ``query_chunk_size`` only bounds the reference's score
     matrix and is ignored.  The candidates go through ``PairSelector`` (:151-188, see there for the tie rule at the
     ``max_pairs`` cut).  ``embeddings`` is a tensor (fp32 / bf16, any device; stored bf16-rounded) or a CorpusShard;
-    i and j are row positions.  ``score_function``: "cos_sim" / "dot" or the reference's callables."""
+    i and j are row positions.  ``score_function``: "cos_sim" / "dot" or the reference's callables.
+
+    ``embeddings`` may also be an ``IVFIndex``, with ``nprobe`` (required there, a ValueError with any other input):
+    then row i's candidates are its top-(top_k + 1) over the undeleted documents of its ``nprobe`` probed lists (the
+    probes of its stored row), i and j are global id - id_base (row positions of the embeddings the index was built
+    from), deleted documents are neither rows nor candidates, ``score_function`` must be the index's, and
+    ``corpus_chunk_size`` does nothing.  ``nprobe == nlist`` gives the pairs of the exact function with one chunk."""
     del query_chunk_size
     name = resolve_score_function(score_function)
+    _check_nprobe(embeddings, nprobe)
     k = int(top_k) + 1  # :148
     if k > MAX_K:
         raise ValueError(f"top_k + 1 = {k} exceeds the library's top-k limit of {MAX_K}")
+    if isinstance(embeddings, IVFIndex):
+        return _pairs_list(_ivf_pairs(embeddings, max_pairs, k, name, int(nprobe)))
     shard = _as_shard(embeddings)
     n = shard.n
     selector = PairSelector(n, max_pairs, shard.device)
@@ -127,12 +151,42 @@ def paraphrase_mining_embeddings(embeddings: Union[torch.Tensor, CorpusShard], q
                 s, j = chunk.search(rows[qs:qe], kc, name)
                 i = torch.arange(qs, qe, device=shard.device).unsqueeze(1).expand(-1, kc)
                 selector.add(s.reshape(-1), i.reshape(-1), j.reshape(-1))
+    return _pairs_list(selector)
+
+
+def _pairs_list(selector: PairSelector) -> List[list]:
     s, i, j = selector.result()
     return [[score, a, b] for score, a, b in zip(s.tolist(), i.tolist(), j.tolist())]
 
 
-def community_detection(embeddings: Union[torch.Tensor, CorpusShard], threshold: float = 0.75,
-                        min_community_size: int = 10, init_max_size: int = 1000) -> List[List[int]]:
+def _check_index_score_function(index: IVFIndex, name: str) -> None:
+    if name != index.score_function:
+        raise ValueError(f"score_function {name!r} differs from the IVFIndex's {index.score_function!r}")
+
+
+def _ivf_pairs(index: IVFIndex, max_pairs: int, k: int, name: str, nprobe: int) -> PairSelector:
+    """The candidates of paraphrase mining over an IVF index, in a PairSelector.
+
+    The rows are the undeleted stored rows, fed in position order, i.e. list order: neighbouring rows probe the same
+    lists, so the grouped scan's 128-row pair tiles fill up and every list tile is read once for many rows.  This is what
+    makes an IVF self-join cheap.  PairSelector does not depend on the order of its input."""
+    _check_index_score_function(index, name)
+    selector = PairSelector(index.n, max_pairs, index.device)
+    if k <= 0:
+        return selector
+    step = max(256, _CANDIDATES_PER_STEP // k // 256 * 256)
+    mask = index.shard._mask(None, 0)  # the deletions, shared by every row
+    for pos in index._stored_blocks(step):
+        qb, q_scale, c_scale, probes = index._stored_queries(pos, nprobe)
+        s, j = index._search_rows(qb, q_scale, c_scale, probes, k, mask)
+        i = (index.ids[pos].long() - index.id_base).unsqueeze(1).expand(-1, k)
+        selector.add(s.reshape(-1), i.reshape(-1), (j - index.id_base).reshape(-1))
+    return selector
+
+
+def community_detection(embeddings: Union[torch.Tensor, CorpusShard, IVFIndex], threshold: float = 0.75,
+                        min_community_size: int = 10, init_max_size: int = 1000,
+                        nprobe: Optional[int] = None) -> List[List[int]]:
     """ST/util.py:385-448 ("fast clustering"): communities of documents whose cosine score against a central row is
     >= threshold, largest first, without overlaps.  ``embeddings`` is a tensor (any device; stored bf16-rounded) or a
     CorpusShard; the ids are row positions.
@@ -143,18 +197,66 @@ def community_detection(embeddings: Union[torch.Tensor, CorpusShard], threshold:
     the ``topk`` branch), in ascending id order otherwise (the branch that scans the whole row).  The communities are
     sorted stably by size, largest first (:430), and a community that shares a member with an earlier one is dropped
     (:432-446).  The counts of all rows come from one count-only range search; members are fetched for the qualifying
-    rows only, in blocks of bounded size."""
+    rows only, in blocks of bounded size.
+
+    ``embeddings`` may also be a cos_sim ``IVFIndex`` (the reference always scores with cos_sim), with ``nprobe``
+    (required there, a ValueError with any other input): then row i's documents are those of its ``nprobe`` probed lists
+    (the probes of its stored row) with score >= threshold, counted by count-only IVF range searches over all stored rows
+    and fetched for the qualifying rows only.  The ids are global id - id_base (row positions of the embeddings the
+    index was built from), N is the index's n, and deleted documents are neither central rows nor members.
+    ``nprobe == nlist`` gives the communities of the exact function."""
+    _check_nprobe(embeddings, nprobe)
+    if isinstance(embeddings, IVFIndex):
+        return _ivf_communities(embeddings, threshold, min_community_size, init_max_size, int(nprobe))
     shard = _as_shard(embeddings)
     n = shard.n
     if min_community_size > n:
         raise ValueError(f"min_community_size={min_community_size} exceeds the number of embeddings ({n})")
-    init_max_size = min(init_max_size, n)
     rows, inv = shard.stored(), shard.inv_norms
     cscale = inv.data_ptr()
     counts = torch.empty(n, dtype=torch.int64, device=shard.device)
     shard._range_call(rows, inv, cscale, threshold, counts, 0, None, None)
     central = torch.nonzero(counts >= min_community_size).flatten()
-    sizes = counts[central].tolist()
+
+    def fetch(idx, total):
+        return shard._range(rows[idx].contiguous(), inv[idx].contiguous(), cscale, threshold, total)
+    return _communities(central, counts[central].tolist(), fetch, min(init_max_size, n), shard.device)
+
+
+def _ivf_communities(index: IVFIndex, threshold: float, min_community_size: int, init_max_size: int,
+                     nprobe: int) -> List[List[int]]:
+    """community_detection over an IVF index: counts from count-only IVF range searches over the undeleted stored rows
+    in position (= list) order, so that neighbouring rows probe the same lists; then the members of the central rows."""
+    _check_index_score_function(index, "cos_sim")
+    n, dev = index.n, index.device
+    if min_community_size > n:
+        raise ValueError(f"min_community_size={min_community_size} exceeds the number of embeddings ({n})")
+    mask = index.shard._mask(None, 0)  # the deletions
+    by_pos = torch.zeros(n, dtype=torch.int64, device=dev)  # deleted rows keep count 0
+    alive = torch.zeros(n, dtype=torch.bool, device=dev)
+    for pos in index._stored_blocks(_COUNT_ROWS):
+        qb, q_scale, c_scale, probes = index._stored_queries(pos, nprobe)
+        counts = torch.empty(qb.shape[0], dtype=torch.int64, device=dev)
+        index._range_call(qb, q_scale, c_scale, probes, threshold, mask, counts, 0, None, None)
+        by_pos[pos] = counts
+        alive[pos] = True
+    # id order, so that the central rows come in ascending id as in the exact function
+    local = index.ids.long() - index.id_base
+    counts = torch.empty_like(by_pos).index_copy_(0, local, by_pos)
+    alive = torch.empty_like(alive).index_copy_(0, local, alive)
+    central = torch.nonzero((counts >= min_community_size) & alive).flatten()
+
+    def fetch(idx, total):
+        qb, q_scale, c_scale, probes = index._stored_queries(index._pos[idx], nprobe)
+        offsets, s, ids = index._range_rows(qb, q_scale, c_scale, probes, threshold, mask, total)
+        return offsets, s, ids - index.id_base
+    return _communities(central, counts[central].tolist(), fetch, min(init_max_size, n), dev)
+
+
+def _communities(central: torch.Tensor, sizes: List[int], fetch, init_max_size: int, device) -> List[List[int]]:
+    """The communities of the central rows (ascending id) with member counts `sizes`: ``fetch(idx, total)`` returns the
+    range search of central[idx] in CSR form (each row's members in ascending id, total entries), in blocks of at most
+    _MEMBERS_PER_BLOCK members; then the reference's member order, size order and de-duplication (:411-446)."""
     communities: List[List[int]] = []
     a = 0
     while a < len(sizes):
@@ -162,10 +264,9 @@ def community_detection(embeddings: Union[torch.Tensor, CorpusShard], threshold:
         while b < len(sizes) and (b == a or total + sizes[b] <= _MEMBERS_PER_BLOCK):
             total += sizes[b]
             b += 1
-        idx = central[a:b]
-        offsets, s, ids = shard._range(rows[idx].contiguous(), inv[idx].contiguous(), cscale, threshold, total)
+        offsets, s, ids = fetch(central[a:b], total)
         cnt = offsets[1:] - offsets[:-1]
-        seg = torch.repeat_interleave(torch.arange(b - a, device=shard.device), cnt)
+        seg = torch.repeat_interleave(torch.arange(b - a, device=device), cnt)
         # topk-branch rows: score descending (stable: ties keep the ascending ids); the others keep the id order
         key = torch.where((cnt < init_max_size)[seg], -s + 0.0, torch.zeros_like(s))
         o = torch.argsort(key, stable=True)
