@@ -468,6 +468,75 @@ int sgpt_ivf_range_search(int dtype, const void* Q, const void* C, const float* 
                           const uint32_t* mask, int64_t mask_pitch_words, int64_t* out_counts, int64_t cap,
                           float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * IVF-PQ search: the IVF lists above with every document stored as m bytes of product-quantization codes instead of its
+ * row, scanned from per-query lookup tables, plus an exact re-rank of a short candidate list against a stored shard.
+ *
+ * Definitions.  D, m, dsub = D / m, nbits = 8 (256 codewords per sub-quantizer).  m % 16 == 0 (a document's code row
+ * starts 16-byte aligned, so a run of list positions is one aligned byte range), D % m == 0 and D % 8 == 0.
+ *   Stored document: x~ = normalize(x) for cos_sim, x for dot, x the stored row of the source (an int8 row dequantized
+ *     with its scale).  Residual r = x~ - c[list(x)] (c: the coarse centroids fp32 [nlist, D]).  Code:
+ *     code[j] = argmin_c ||r[j dsub .. (j+1) dsub) - B[j][c]||^2 (B: the codebooks fp32 [m, 256, dsub]), ties to the
+ *     lowest c.  (The library's encoder evaluates it in fp32: d = 0; for t ascending: e = r_t - B_t, d = d + e * e,
+ *     each operation rounded on its own.)
+ *   Query: q~ = F.normalize(q) for cos_sim, q for dot, in fp32.
+ *   Tables: lut[q][j][c] = sum_t q~[j dsub + t] B[j][c][t] and base[q][p] = sum_t q~[t] c[probe[q][p]][t], both fp32 FMA
+ *     chains from 0 in ascending t.
+ *   ADC score of the document at list position pos for the pair (q, p):
+ *     acc = 0; for j = 0 .. m-1: acc += lut[q][j][codes[pos][j]]   (plain fp32 adds, in this order, never reassociated)
+ *     score = fixnan(acc + base[q][p])   (NaN counts as -1).
+ *   The order holds however the kernel stages the tables: a document's partial sum carries across table chunks, so a
+ *   restatement of these two lines reproduces every device score bit for bit from the device's tables.
+ *
+ * sgpt_pq_tables: lut_out fp32 [nq, m, 256] and base_out fp32 [nq, nprobe] of Q fp32 [nq, D] (q~, already normalized
+ *   for cos_sim), codebooks fp32 [m, 256, dsub], centroids fp32 [nlist, D], probes int32 [nq, nprobe].  A probe outside
+ *   [0, nlist) is skipped: no centroid is read and its base is 0.  SGPT_ERR_INVALID, before any CUDA call, for nq < 0,
+ *   D not a positive multiple of 8, m not a positive multiple of 16 or above 4096, D % m != 0, nlist < 1, nprobe outside
+ *   [1, nlist] and null pointers.
+ *
+ * sgpt_ivfpq_search: per query, the top-k by ADC score over its probed positions that the mask allows and whose doc_ids
+ *   entry is >= 0: score descending, ties by ascending global id, tail (-inf, -1).  This is sgpt_ivf_search's contract
+ *   with the ADC score in place of the dot product.
+ *   lut, base   the tables of sgpt_pq_tables for these queries and probes (device; lut 16-byte aligned).
+ *   codes       uint8 [n, m] in list order (device, 16-byte aligned); list l is positions
+ *               [list_offsets[l], list_offsets[l+1]).  list_offsets, max_list_len, doc_ids, probes and mask (the shared
+ *               bitmap of allowed positions, pitch 0, or NULL) as in sgpt_ivf_search.
+ *   Any nq (blocks of 256 queries reuse ws); no host synchronisation.  Offsets are clamped and skipped probes never read
+ *   as in sgpt_ivf_search, so inconsistent device inputs give wrong results, never an out-of-bounds access.
+ *   SGPT_ERR_INVALID, before any CUDA call, for sgpt_ivf_search's rejections with the same wording (nq < 0, nlist < 1,
+ *   nprobe outside [1, nlist], k outside [1, 4096], n outside [0, 2^31), max_list_len outside [0, n], nprobe x
+ *   max_list_len beyond the selection's 2^32 entries, null inputs or outputs, a workspace smaller than
+ *   sgpt_ivfpq_search_workspace_bytes), and m not a positive multiple of 16 or above 4096, and an unaligned lut or codes.
+ *   The workspace query returns -1 for arguments the search rejects.
+ *
+ * sgpt_rerank: the exact score of each candidate against a stored shard, then its top-k.  dtype, Q, C, q_scale,
+ *   c_scale, D, n and id_base mean what they mean in sgpt_search_masked (Q and C 16-byte aligned).  cand_ids int64
+ *   [nq, kc] (device): global ids; a candidate < 0 or outside [id_base, id_base + n) is an empty slot, and the valid
+ *   candidates of one query must be distinct.  out_scores fp32 [nq, k], out_ids int64 [nq, k]: the top-k of the
+ *   candidates' scores with the exact search's tie rule (score descending, ids ascending), tail (-inf, -1).
+ *   int8:  acc = the exact s32 dot product, score = fixnan(float_rn(acc) * q_scale[q] * c_scale[row]) in the filter
+ *          epilogue's order: bit-identical to sgpt_search_masked's score of that document.
+ *   bf16:  every product is exact in fp32.  Lane l (0..31) sums the 8-element groups g = l, l + 32, l + 64, ... of the
+ *          row in ascending g, and each group's elements in ascending order (acc_l += Q[8g+i] C[8g+i], one rounding per
+ *          add); then for o = 16, 8, 4, 2, 1: acc_l = acc_l + acc_(l xor o) for every lane; score =
+ *          fixnan(acc_0 * q_scale[q] * c_scale[row]).  Reproducible in numpy bit for bit; within fp32 rounding of the
+ *          tensor-core sum of sgpt_search_masked.
+ *   SGPT_ERR_INVALID, before any CUDA call, for an unknown dtype, nq < 0, kc outside [1, 2^24], the D rules of the
+ *   dtype, n outside [0, 2^31), id_base < 0 or id_base + n > 2^31, k outside [1, 4096], null inputs or outputs, an
+ *   unaligned Q or C and a workspace smaller than sgpt_rerank_workspace_bytes (which returns -1 for bad nq / kc).
+ * ------------------------------------------------------------------------------------------------------------------ */
+int sgpt_pq_tables(const float* Q, const float* codebooks, const float* centroids, const int32_t* probes, int nq, int D,
+                   int m, int nlist, int nprobe, float* lut_out, float* base_out, sgpt_stream_t stream);
+int64_t sgpt_ivfpq_search_workspace_bytes(int nq, int nlist, int nprobe, int64_t max_list_len, int m);
+int sgpt_ivfpq_search(const float* lut, const float* base, const uint8_t* codes, int nq, int64_t n, int m,
+                      const int64_t* list_offsets, int nlist, int64_t max_list_len, const int32_t* doc_ids,
+                      const int32_t* probes, int nprobe, int k, const uint32_t* mask, float* out_scores,
+                      int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
+int64_t sgpt_rerank_workspace_bytes(int nq, int64_t kc);
+int sgpt_rerank(int dtype, const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq, int64_t n,
+                int D, int64_t id_base, const int64_t* cand_ids, int64_t kc, int k, float* out_scores,
+                int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
+
 /* bf16 -> fp32 conversion of count elements (count % 4 == 0), e.g. of the residual stream. */
 int sgpt_bf16_to_f32(const void* x, float* y, int64_t count, sgpt_stream_t stream);
 

@@ -14,7 +14,7 @@ from .config import ModelConfig, preset  # noqa: F401
 
 __all__ = ["ModelConfig", "preset", "Encoder", "CustomEmbedder", "SentenceEncoder", "SentenceBERTBOSEOS",
            "SentenceBERTAsym", "DenseRetrievalExactSearch", "CorpusShard", "merge_topk", "semantic_search",
-           "merge_topk_packed", "unpack_topk", "pack_mask", "IVFIndex", "sharded_search", "PeerGather", "ShardedDenseRetrievalExactSearch", "DenseHead", "AsymHeads", "load_st_directory", "GenericDataLoader", "EvaluateRetrieval",
+           "merge_topk_packed", "unpack_topk", "pack_mask", "IVFIndex", "IVFPQIndex", "sharded_search", "PeerGather", "ShardedDenseRetrievalExactSearch", "DenseHead", "AsymHeads", "load_st_directory", "GenericDataLoader", "EvaluateRetrieval",
            "InformationRetrievalEvaluator", "paraphrase_mining", "paraphrase_mining_embeddings", "community_detection"]
 
 
@@ -46,6 +46,9 @@ def __getattr__(name):  # lazy: torch / CUDA pieces are imported on first use
     if name == "IVFIndex":
         from .ivf import IVFIndex
         return IVFIndex
+    if name == "IVFPQIndex":
+        from .ivfpq import IVFPQIndex
+        return IVFPQIndex
     if name in ("paraphrase_mining", "paraphrase_mining_embeddings", "community_detection"):
         from . import mining
         return getattr(mining, name)

@@ -102,6 +102,11 @@ _SIGNATURES = {
     "sgpt_ivf_range_search_workspace_bytes": (i64, [i32, i32, i32, i32, i64, i32]),
     "sgpt_ivf_range_search": (i32, [i32, vp, vp, vp, vp, i32, i64, i32, vp, i32, i64, vp, vp, i32, f32, vp, i64, vp, i64,
                                     vp, vp, vp, i64, vp]),
+    "sgpt_pq_tables": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]),
+    "sgpt_ivfpq_search_workspace_bytes": (i64, [i32, i32, i32, i64, i32]),
+    "sgpt_ivfpq_search": (i32, [vp, vp, vp, i32, i64, i32, vp, i32, i64, vp, vp, i32, i32, vp, vp, vp, vp, i64, vp]),
+    "sgpt_rerank_workspace_bytes": (i64, [i32, i64]),
+    "sgpt_rerank": (i32, [i32, vp, vp, vp, vp, i32, i64, i32, i64, vp, i64, i32, vp, vp, vp, i64, vp]),
 }
 DTYPE_BF16, DTYPE_I8 = 0, 1
 

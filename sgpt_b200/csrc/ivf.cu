@@ -23,6 +23,7 @@
 #include "common.cuh"
 #include "gemm_api.h"
 #include "host_utils.h"
+#include "ivf.cuh"
 #include "topk.cuh"
 
 using namespace sgpt;
@@ -36,18 +37,8 @@ constexpr int kScanThreads = 1024;
 
 inline int64_t align256(int64_t x) { return (x + 255) & ~int64_t(255); }
 
-// positions [b, e) of list l: the offsets clamped to [0, n] and the length to max_len
-__device__ __forceinline__ void list_range(const int64_t* __restrict__ offsets, int l, int n, long long max_len, int& b,
-                                           int& e) {
-  long long lo = __ldg(reinterpret_cast<const long long*>(offsets) + l);
-  long long hi = __ldg(reinterpret_cast<const long long*>(offsets) + l + 1);
-  lo = lo < 0 ? 0 : (lo > n ? n : lo);
-  hi = hi < lo ? lo : (hi > n ? n : hi);
-  if (hi - lo > max_len) hi = lo + max_len;
-  b = static_cast<int>(lo);
-  e = static_cast<int>(hi);
-}
-
+// kHist = false (the IVF-PQ search): no per-list histogram
+template <bool kHist>
 __global__ void __launch_bounds__(kThreads) ivf_count_kernel(const int32_t* __restrict__ probes,
                                                              const int64_t* __restrict__ offsets, int nlist, int n,
                                                              long long max_len, int nb, int nprobe,
@@ -64,7 +55,7 @@ __global__ void __launch_bounds__(kThreads) ivf_count_kernel(const int32_t* __re
     len = e - b;
   }
   counts[static_cast<long long>(p) * nb + q] = len;  // the selection's counts[g * nq + q]
-  if (len > 0) atomicAdd(hist + l, 1);
+  if (kHist && len > 0) atomicAdd(hist + l, 1);
 }
 
 // exclusive scan of two values per thread over the CTA (kScanThreads); *tot = the CTA's sums
@@ -335,7 +326,7 @@ Layout make_layout(int nq, int nlist, int nprobe, int64_t max_list_len, int D, i
   Layout w{};
   w.nb = nq < kIvfBlock ? (nq > 0 ? nq : 1) : kIvfBlock;
   w.pairs = static_cast<int64_t>(w.nb) * nprobe;
-  w.Ls = max_list_len < 2 ? 2 : (max_list_len + 1) & ~int64_t(1);
+  w.Ls = ivf_list_stride(max_list_len);
   // sum over lists of ceil(P_l / 128) <= (lists with a pair) + pairs / 128, and every list has at most ceil(L / 256) tiles
   const int64_t lists_hit = nlist < w.pairs ? nlist : w.pairs;
   int64_t blocks = lists_hit + w.pairs / kPairRows;
@@ -383,7 +374,7 @@ int check_sizes(const char* fn, int dtype, int nq, int nlist, int nprobe, int64_
   SGPT_REQUIRE(max_list_len >= 0 && max_list_len < (1ll << 31), "%s: max_list_len=%lld outside [0, 2^31)", fn,
                (long long)max_list_len);
   // the selection ranks nprobe lists of max_list_len entries (each padded to 32) in one 2^32-entry space
-  const int64_t Ls = max_list_len < 2 ? 2 : (max_list_len + 1) & ~int64_t(1);
+  const int64_t Ls = ivf_list_stride(max_list_len);
   SGPT_REQUIRE(static_cast<int64_t>(nprobe) * ((Ls + 31) & ~int64_t(31)) < (1ll << 32),
                "%s: nprobe=%d lists of max_list_len=%lld entries exceed the 2^32-entry selection space", fn, nprobe,
                (long long)max_list_len);
@@ -447,12 +438,8 @@ int ivf_scan_block(const Layout& w, uint8_t* base, int s8, const void* Q, const 
   const int32_t* pr = probes + static_cast<long long>(q0) * nprobe;
   // hist and fill are adjacent
   SGPT_CHECK_CUDA(cudaMemsetAsync(hist, 0, static_cast<size_t>(w.pair_off - w.hist), stream));
-  {
-    LaunchScope _ls(kCatMisc, stream);
-    SGPT_CHECK_CUDA(launch_kernel(ivf_count_kernel, dim3(static_cast<unsigned>((pairs + kThreads - 1) / kThreads)),
-                                  dim3(kThreads), 0, stream, pr, list_offsets, nlist, N, max_len, nb, nprobe, counts,
-                                  hist));
-  }
+  const int rc = launch_ivf_counts(pr, list_offsets, nlist, N, max_len, nb, nprobe, counts, hist, stream);
+  if (rc != SGPT_OK) return rc;
   if (n > 0 && w.max_units > 0) {
     {
       LaunchScope _ls(kCatMisc, stream);
@@ -506,23 +493,47 @@ int ivf_search(const char* fn, int dtype, const void* Q, const void* C, const fl
     int rc = ivf_scan_block(w, base, s8, Q, C, q_scale, c_scale, n, D, list_offsets, nlist, max_list_len, doc_ids,
                             probes, nprobe, mask, mask_pitch, q0, nb, stream);
     if (rc != SGPT_OK) return rc;
-    TopkSrc src{};
-    src.packed = reinterpret_cast<uint2*>(base + w.cand);
-    src.packed_global = 1;
-    src.counts = reinterpret_cast<int*>(base + w.counts);
-    src.G = nprobe;
-    src.nq = nb;
-    src.L = w.Ls;
-    src.stride_g = w.Ls;
-    src.stride_q = static_cast<long long>(nprobe) * w.Ls;
-    rc = launch_topk_select(src, nb, k, out_scores + static_cast<long long>(q0) * k,
-                            out_ids + static_cast<long long>(q0) * k, stream);
+    rc = launch_ivf_select(reinterpret_cast<const uint2*>(base + w.cand), reinterpret_cast<const int*>(base + w.counts),
+                           nb, nprobe, w.Ls, k, out_scores + static_cast<long long>(q0) * k,
+                           out_ids + static_cast<long long>(q0) * k, stream);
     if (rc != SGPT_OK) return rc;
   }
   return SGPT_OK;
 }
 
 }  // namespace
+
+namespace sgpt {
+
+int launch_ivf_counts(const int32_t* probes, const int64_t* offsets, int nlist, int n, long long max_len, int nb,
+                      int nprobe, int* counts, int* hist, cudaStream_t stream) {
+  const long long pairs = static_cast<long long>(nb) * nprobe;
+  LaunchScope _ls(kCatMisc, stream);
+  const dim3 grid(static_cast<unsigned>((pairs + kThreads - 1) / kThreads));
+  if (hist != nullptr)
+    SGPT_CHECK_CUDA(launch_kernel(ivf_count_kernel<true>, grid, dim3(kThreads), 0, stream, probes, offsets, nlist, n,
+                                  max_len, nb, nprobe, counts, hist));
+  else
+    SGPT_CHECK_CUDA(launch_kernel(ivf_count_kernel<false>, grid, dim3(kThreads), 0, stream, probes, offsets, nlist, n,
+                                  max_len, nb, nprobe, counts, hist));
+  return SGPT_OK;
+}
+
+int launch_ivf_select(const uint2* cand, const int* counts, int nb, int nprobe, long long Ls, int k, float* out_scores,
+                      int64_t* out_ids, cudaStream_t stream) {
+  TopkSrc src{};
+  src.packed = cand;
+  src.packed_global = 1;
+  src.counts = counts;
+  src.G = nprobe;
+  src.nq = nb;
+  src.L = Ls;
+  src.stride_g = Ls;
+  src.stride_q = static_cast<long long>(nprobe) * Ls;
+  return launch_topk_select(src, nb, k, out_scores, out_ids, stream);
+}
+
+}  // namespace sgpt
 
 extern "C" int sgpt_ivf_search(int dtype, const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq,
                                int64_t n, int D, const int64_t* list_offsets, int nlist, int64_t max_list_len,

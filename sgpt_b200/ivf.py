@@ -54,6 +54,53 @@ def _assign_rows(cshard: CorpusShard, shard: CorpusShard, score_function: str) -
                       for i in range(0, n, bs)])
 
 
+def _kmeans(x: torch.Tensor, nlist: int, n_iter: int, g: torch.Generator, score_function: str) -> torch.Tensor:
+    """Coarse k-means of ``IVFIndex.build`` (and ``IVFPQIndex.train``) over the training rows x fp32 [T, D] (device,
+    already normalized for cos_sim): centroids fp32 [nlist, D] on x's device.  Starts from x[:nlist]; assignment is the
+    exact search (k = 1) against the centroids as a bf16 shard, the update is the mean of the assigned rows summed in fp64
+    on the host in row order (no atomics), an empty list is re-seeded with a row drawn from `g`, and for cos_sim the
+    centroids are normalized (spherical k-means)."""
+    T, D = x.shape
+    dev, cos = x.device, score_function == "cos_sim"
+    cent = x[:nlist].clone()
+    step = max(1, (64 << 20) // (8 * D))  # rows per host transfer of the update
+    for _ in range(int(n_iter)):
+        a = _assign(CorpusShard.from_embeddings(cent, device=dev), x, score_function).cpu()
+        sums = torch.zeros(nlist, D, dtype=torch.float64)
+        for i in range(0, T, step):  # index_add_ on the host adds the rows in order: reproducible bits
+            sums.index_add_(0, a[i:i + step], x[i:i + step].cpu().double())
+        counts = torch.bincount(a, minlength=nlist)
+        new = sums / counts.clamp(min=1)[:, None].double()
+        empty = (counts == 0).nonzero().flatten()
+        if len(empty):
+            new[empty] = x[torch.randint(T, (len(empty),), generator=g).to(dev)].double().cpu()
+        if cos:
+            new = torch.nn.functional.normalize(new, dim=1)
+        cent = new.float().to(dev)
+    return cent
+
+
+def _merge_lists(offsets: torch.Tensor, lists: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Destinations of an append to list-ordered storage (``IVFIndex.add``, ``IVFPQIndex.add``): the n old positions
+    (offsets int64 [nlist + 1], device) and m new rows whose lists are `lists` int64 [m].  Every list keeps its rows in
+    their order, followed by its new rows in input order.  Returns (new offsets, old_dest int64 [n], new_dest int64 [m])."""
+    nlist, dev = offsets.numel() - 1, offsets.device
+    n, m = int(offsets[-1]), lists.numel()
+    added = torch.bincount(lists, minlength=nlist)
+    shift = torch.cumsum(added, 0) - added  # new rows inserted before list l
+    sizes = offsets[1:] - offsets[:-1]
+    new_offsets = offsets.clone()
+    new_offsets[1:] += torch.cumsum(added, 0)
+    # destinations: old position p of list l -> p + shift[l]; new rows after their list's old rows, in input order
+    old_list = torch.repeat_interleave(torch.arange(nlist, device=dev), sizes, output_size=n)
+    old_dest = torch.arange(n, device=dev) + shift[old_list]
+    order = torch.sort(lists, stable=True).indices
+    rank = torch.arange(m, device=dev) - shift[lists[order]]  # place inside the list's new rows
+    new_dest = torch.empty(m, dtype=torch.int64, device=dev)
+    new_dest[order] = new_offsets[lists[order]] + sizes[lists[order]] + rank
+    return new_offsets, old_dest, new_dest
+
+
 class IVFIndex:
     """IVF index on one GPU.  Built by ``IVFIndex.build`` or ``IVFIndex.load``.
 
@@ -123,21 +170,7 @@ class IVFIndex:
         x = _rows_f32(src, sample)
         if cos:
             x = torch.nn.functional.normalize(x, dim=1)
-        cent = x[:nlist].clone()
-        step = max(1, (64 << 20) // (8 * D))  # rows per host transfer of the update
-        for _ in range(int(n_iter)):
-            a = _assign(CorpusShard.from_embeddings(cent, device=dev), x, score_function).cpu()
-            sums = torch.zeros(nlist, D, dtype=torch.float64)
-            for i in range(0, T, step):  # index_add_ on the host adds the rows in order: reproducible bits
-                sums.index_add_(0, a[i:i + step], x[i:i + step].cpu().double())
-            counts = torch.bincount(a, minlength=nlist)
-            new = sums / counts.clamp(min=1)[:, None].double()
-            empty = (counts == 0).nonzero().flatten()
-            if len(empty):
-                new[empty] = x[torch.randint(T, (len(empty),), generator=g).to(dev)].double().cpu()
-            if cos:
-                new = torch.nn.functional.normalize(new, dim=1)
-            cent = new.float().to(dev)
+        cent = _kmeans(x, nlist, n_iter, g, score_function)
         del x
         assign = _assign_rows(CorpusShard.from_embeddings(cent, device=dev), src, score_function)
         perm = torch.sort(assign, stable=True).indices
@@ -322,18 +355,7 @@ class IVFIndex:
         n, dev, old = self.n, self.device, self.shard
         new = CorpusShard.from_embeddings(emb.to(dev), device=dev, dtype=self.dtype)
         lists = _assign_rows(self._cshard, new, self.score_function)
-        added = torch.bincount(lists, minlength=self.nlist)
-        shift = torch.cumsum(added, 0) - added  # new rows inserted before list l
-        sizes = self.offsets[1:] - self.offsets[:-1]
-        offsets = self.offsets.clone()
-        offsets[1:] += torch.cumsum(added, 0)
-        # destinations: old position p of list l -> p + shift[l]; new rows after their list's old rows, in input order
-        old_list = torch.repeat_interleave(torch.arange(self.nlist, device=dev), sizes, output_size=n)
-        old_dest = torch.arange(n, device=dev) + shift[old_list]
-        order = torch.sort(lists, stable=True).indices
-        rank = torch.arange(m, device=dev) - shift[lists[order]]  # place inside the list's new rows
-        new_dest = torch.empty(m, dtype=torch.int64, device=dev)
-        new_dest[order] = offsets[lists[order]] + sizes[lists[order]] + rank
+        offsets, old_dest, new_dest = _merge_lists(self.offsets, lists)
         inner = CorpusShard(self.dim, n + m, device=dev, dtype=self.dtype)
         fields = ("vectors", "scales", "cos_scales") if self.dtype == "int8" else ("vectors", "inv_norms")
         for f in fields:
