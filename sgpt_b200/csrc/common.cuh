@@ -196,6 +196,9 @@ __device__ __forceinline__ void sts_v4(uint32_t addr, uint32_t a, uint32_t b, ui
 __device__ __forceinline__ void sts_v2(uint32_t addr, uint32_t a, uint32_t b) {
   asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(a), "r"(b) : "memory");
 }
+__device__ __forceinline__ void sts_b32(uint32_t addr, uint32_t a) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(a) : "memory");
+}
 __device__ __forceinline__ float4 lds_v4(uint32_t addr) {
   float4 v;
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
@@ -347,6 +350,21 @@ __device__ __forceinline__ void wgmma_s8_m64n256(int32_t (&d)[128], uint64_t des
 // named barrier over `count` threads (a multiple of 32) of the CTA
 __device__ __forceinline__ void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+// arrive at a named barrier without waiting (the other `count` - 32 k threads wait in named_bar_sync)
+__device__ __forceinline__ void named_bar_arrive(int id, int count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
+// Per-warpgroup register budget (all 128 threads of the warpgroup execute it): warp-specialised kernels move registers
+// from the warpgroup that issues TMA loads to the ones that hold the wgmma accumulators.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
 }
 
 // ---------------------------------------------------------------------------------------------------------------

@@ -15,7 +15,7 @@ template <int BN, class Epi, int CL = 1, bool kS8 = false>
 static int launch_gemm(const void* a, int64_t lda, const void* b, int64_t ldb, int M, int N, int K,
                        const typename Epi::Params& ep, cudaStream_t stream, int cat = kCatGemm,
                        TileMap tmap = TileMap()) {
-  using Cfg = GemmCfg<BN, EpiStaging<Epi>::value>;
+  using Cfg = GemmCfg<BN, Epi::kStagingBytes>;
   // one 128-byte row segment per box row: 64 bf16 or 128 int8
   auto make_map = kS8 ? make_tma_2d_u8 : make_tma_2d_bf16;
   const uint32_t box_k = kS8 ? 2 * kGemmBK : kGemmBK;
@@ -43,10 +43,9 @@ static int launch_gemm(const void* a, int64_t lda, const void* b, int64_t ldb, i
   return SGPT_OK;
 }
 
-// nn.Linear dispatch: 128 x 128 tiles (the 128 x 128 fp32 accumulator the epilogue reads back from shared memory leaves room
-// for four operand stages; 256-wide tiles would leave one).  Tile rasterisation (gemm.cuh TileMap::band): banded M-fastest
-// order once the weight matrix no longer fits in the H100's 50 MB L2 next to the activations.  SGPT_GEMM_BAND=<g> forces a
-// band height (0 = N fastest) for A/B measurements; read per call.
+// nn.Linear dispatch: gemm_linear_kernel, 128 x 128 tiles.  Tile rasterisation (gemm.cuh TileMap::band): banded
+// M-fastest order once the weight matrix no longer fits in the H100's 50 MB L2 next to the activations.
+// SGPT_GEMM_BAND=<g> forces a band height (0 = N fastest) for A/B measurements; read per call.
 static int pick_band(int M, int N, int K) {
   if (const char* e = getenv("SGPT_GEMM_BAND")) return atoi(e);
   const long long w_bytes = 2ll * N * K;
@@ -54,13 +53,31 @@ static int pick_band(int M, int N, int K) {
   return (w_bytes >= (32ll << 20) && m_tiles >= 16) ? 8 : 0;
 }
 
-template <class Epi>
+template <class Op>
 static int launch_linear(const void* x, int64_t ldx, const void* w, int64_t ldw, int M, int N, int K,
-                         const typename Epi::Params& p, cudaStream_t stream, int ksplit = 1) {
+                         const typename Op::Params& p, cudaStream_t stream, int ksplit = 1) {
   TileMap tm;
   tm.ksplit = ksplit;
   tm.band = pick_band(M, N, K);
-  return launch_gemm<128, Epi, 1>(x, ldx, w, ldw, M, N, K, p, stream, kCatGemm, tm);
+  CUtensorMap ta, tb;
+  int rc = make_tma_2d_bf16(&ta, x, static_cast<uint64_t>(M), static_cast<uint64_t>(K), static_cast<uint64_t>(ldx),
+                            kGemmBM, kGemmBK);
+  if (rc != SGPT_OK) return rc;
+  rc = make_tma_2d_bf16(&tb, w, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldw), kLinBN,
+                        kGemmBK);
+  if (rc != SGPT_OK) return rc;
+  auto kern = gemm_linear_kernel<Op>;
+  static PerDeviceOnce attr_once;
+  if (attr_once.first()) {
+    SGPT_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, LinearCfg::kSmemBytes));
+  }
+  const long long units = static_cast<long long>((M + kGemmBM - 1) / kGemmBM) * ((N + kLinBN - 1) / kLinBN) * ksplit;
+  if (units == 0) return SGPT_OK;
+  const long long ctas = units < sm_count() ? units : sm_count();
+  LaunchScope _ls(kCatGemm, stream);
+  SGPT_CHECK_CUDA(launch_kernel(kern, dim3(static_cast<unsigned>(ctas)), dim3(kLinThreads), LinearCfg::kSmemBytes, stream,
+                                ta, tb, M, N, K, p, tm));
+  return SGPT_OK;
 }
 
 // Split-K for the reduce-add (residual) epilogues: OFF unless SGPT_GEMM_SPLITK=2/3/4 asks for it (experiments, tests).
@@ -153,7 +170,7 @@ int launch_sample_maxima(const void* Q, const void* C, const float* q_scale, con
 template <class Epi>
 static int launch_ivf_units(const CUtensorMap& ta, const CUtensorMap& tb, int rows, int n, int D,
                             const typename Epi::Params& p, bool s8, cudaStream_t stream) {
-  using Cfg = GemmCfg<kSimBN, EpiStaging<Epi>::value>;
+  using Cfg = GemmCfg<kSimBN, Epi::kStagingBytes>;
   auto kern = s8 ? gemm_bf16_tn_kernel<kSimBN, Epi, 1, true, true> : gemm_bf16_tn_kernel<kSimBN, Epi, 1, false, true>;
   static PerDeviceOnce attr_once;
   if (attr_once.first()) {
@@ -238,11 +255,11 @@ extern "C" int sgpt_linear(const void* x, int64_t ldx, const void* w, int64_t ld
                                 static_cast<uint64_t>(ldo), 32, 64);
       if (rc != SGPT_OK) return rc;
       if (epilogue == SGPT_EPI_BF16) {
-        EpiBiasActBF16<false>::Params p{om, bias, out, static_cast<int>(ldo)};
-        return launch_linear<EpiBiasActBF16<false>>(x, ldx, w, ldw, M, N, K, p, stream);
+        OpTmaBiasActBF16<false>::Params p{om, bias};
+        return launch_linear<OpTmaBiasActBF16<false>>(x, ldx, w, ldw, M, N, K, p, stream);
       }
-      EpiBiasActBF16<true>::Params p{om, bias, out, static_cast<int>(ldo)};
-      return launch_linear<EpiBiasActBF16<true>>(x, ldx, w, ldw, M, N, K, p, stream);
+      OpTmaBiasActBF16<true>::Params p{om, bias};
+      return launch_linear<OpTmaBiasActBF16<true>>(x, ldx, w, ldw, M, N, K, p, stream);
     }
     case SGPT_EPI_RESID_BF16: {
       SGPT_REQUIRE(resid != nullptr && resid == out,
@@ -252,30 +269,15 @@ extern "C" int sgpt_linear(const void* x, int64_t ldx, const void* w, int64_t ld
       int rc = make_tma_2d_bf16(&om, out, static_cast<uint64_t>(M), static_cast<uint64_t>(N),
                                 static_cast<uint64_t>(ldo), 32, 64);
       if (rc != SGPT_OK) return rc;
-      EpiResidualBF16::Params p{om, bias, out, static_cast<int>(ldo)};
-      return launch_linear<EpiResidualBF16>(x, ldx, w, ldw, M, N, K, p, stream, pick_ksplit(K));
+      OpTmaResidAddBF16::Params p{om, bias};
+      return launch_linear<OpTmaResidAddBF16>(x, ldx, w, ldw, M, N, K, p, stream, pick_ksplit(K));
     }
-    case 102:
-    case 103:
-    case 104:
-    case 105: {  // profiling aids: bf16 epilogue without the TMA store (102) / without the smem-reuse wait (103)
-      CUtensorMap om;
-      int rc = make_tma_2d_bf16(&om, out, static_cast<uint64_t>(M), static_cast<uint64_t>(N),
-                                static_cast<uint64_t>(ldo), 32, 64);
-      if (rc != SGPT_OK) return rc;
-      OpTmaBiasActBF16<false>::Params p{om, bias, out, static_cast<int>(ldo)};
-      if (epilogue == 102) return launch_linear<EpiTma<OpTmaBiasActBF16<false>, 1>>(x, ldx, w, ldw, M, N, K, p, stream);
-      if (epilogue == 105) return launch_linear<EpiTma<OpTmaBiasActBF16<false>, 4>>(x, ldx, w, ldw, M, N, K, p, stream);
-      if (epilogue == 104) return launch_linear<EpiTma<OpTmaBiasActBF16<false>, 3>>(x, ldx, w, ldw, M, N, K, p, stream);
-      return launch_linear<EpiTma<OpTmaBiasActBF16<false>, 2>>(x, ldx, w, ldw, M, N, K, p, stream);
-    }
-    case 100: {  // profiling aid: mainloop only
-      EpiDebugNull<false>::Params p{0};
-      return launch_linear<EpiDebugNull<false>>(x, ldx, w, ldw, M, N, K, p, stream);
-    }
-    case 101: {  // profiling aid: mainloop + accumulator loads
-      EpiDebugNull<true>::Params p{0};
-      return launch_linear<EpiDebugNull<true>>(x, ldx, w, ldw, M, N, K, p, stream);
+    case 100:
+    case 101: {  // profiling aids: the mainloop and the fp32 accumulator hand-over alone (100) / + its read-back (101)
+      TileMap tm;
+      tm.band = pick_band(M, N, K);
+      if (epilogue == 100) return launch_gemm<128, EpiDebugNull<false>>(x, ldx, w, ldw, M, N, K, {0}, stream, kCatGemm, tm);
+      return launch_gemm<128, EpiDebugNull<true>>(x, ldx, w, ldw, M, N, K, {0}, stream, kCatGemm, tm);
     }
     default:
       set_error("sgpt_linear: unknown epilogue %d", epilogue);
@@ -300,9 +302,8 @@ extern "C" int sgpt_linear_qkv_rotary(const void* x, int64_t ldx, const void* w_
   int rc = make_tma_2d_bf16(&om, qkv, static_cast<uint64_t>(M), static_cast<uint64_t>(N), static_cast<uint64_t>(N), 32,
                             64);
   if (rc != SGPT_OK) return rc;
-  EpiRotaryBF16::Params p{om, pos, reinterpret_cast<const float2*>(cos_sin), M, d_model, head_dim, rotary_dim, max_pos,
-                          qkv, N};
-  return launch_linear<EpiRotaryBF16>(x, ldx, w_qkv, d_model, M, N, d_model, p, stream);
+  OpTmaRotaryBF16::Params p{om, pos, reinterpret_cast<const float2*>(cos_sin), M, d_model, head_dim, rotary_dim, max_pos};
+  return launch_linear<OpTmaRotaryBF16>(x, ldx, w_qkv, d_model, M, N, d_model, p, stream);
 }
 
 extern "C" int sgpt_scores(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* scores,

@@ -4,25 +4,21 @@
 //   A : activations / queries, row-major [M,K]  -> K-major wgmma operand A
 //   B : nn.Linear weight [out,in] / corpus shard [n,D], row-major [N,K] -> K-major wgmma operand B
 //
-// Roles (9 warps = 288 threads, 1 CTA per SM):
+// Two kernels share the operand pipeline (a TMA producer filling a kStages-deep smem ring of {A 128x64, B BNx64} tiles,
+// SWIZZLE_128B, handed over with mbarriers only; the producer runs ahead across tiles):
+//
+// gemm_bf16_tn_kernel (similarity, filter and IVF scans; 9 warps = 288 threads, 1 CTA per SM):
 //   warps 0..7   two consumer warpgroups: warpgroup g runs wgmma m64nBNk16 for rows [64 g, 64 g + 64) of the 128 x BN
 //                tile with the fp32 accumulator in its registers, then the epilogue
-//   warp  8      TMA producer (one lane; kStages-deep smem ring of {A 128x64, B BNx64} bf16 tiles, SWIZZLE_128B)
+//   warp  8      TMA producer
+//   The consumers park the accumulator in shared memory (fp32, 128 rows x BN, each 128-byte row segment XOR-swizzled by
+//   (row & 7) so that both the fragment stores and the row reads are free of bank conflicts), and the epilogue warps read
+//   it back with thread = row, 32 consecutive columns per read (acc_ld_32): the score epilogues compare, scale and append
+//   per query row.  E = 4 or 8 epilogue warps: warp w owns the 32-row slab (w % 4) and, with 8 warps, the column half
+//   (w / 4).  EpiStaged<Op> (similarity scores) adds an smem transpose so that lane = column pair and each warp
+//   instruction touches one contiguous row segment.
 //
-// The producer runs ahead across tiles, so the next tile's operands stream in while the current tile's epilogue runs;
-// smem stages are handed over with mbarriers only.
-//
-// Epilogue data paths.  The consumers park the accumulator in shared memory (fp32, 128 rows x BN, each 128-byte row
-// segment XOR-swizzled by (row & 7) so that both the fragment stores and the row reads are free of bank conflicts), and
-// the epilogue warps read it back with thread = row, 32 consecutive columns per read (acc_ld_32).  E = 4 or 8 epilogue
-// warps: warp w owns the 32-row slab (w % 4) and, with 8 warps, the column half (w / 4).  Two families:
-//   EpiTma<Op>    (nn.Linear outputs)  thread = row: bias/activation in registers, the 128-byte row segment is written
-//                 to a per-warp smem box in the SWIZZLE_128B layout and one elected lane hands the [32 x 128 B] box to
-//                 the TMA engine — a plain tensor store (bf16 outputs) or a reduce-add into the residual stream
-//                 (`resid += acc + bias`, performed by the L2; no residual load in the SM at all).  M/N tails are clipped
-//                 by the tensor map.
-//   EpiStaged<Op> (similarity scores)  smem transpose so that lane = column pair and each warp instruction touches one
-//                 contiguous row segment.
+// gemm_linear_kernel (nn.Linear outputs, bf16; 3 warpgroups = 384 threads, 1 CTA per SM): ping-pong consumers, see there.
 #pragma once
 #include <type_traits>
 
@@ -35,17 +31,15 @@ constexpr int kGemmBM = 128;
 constexpr int kGemmBK = 64;
 constexpr int kGemmMmaWarps = 8;                        // two consumer warpgroups of 64 rows
 constexpr int kGemmThreads = 32 * (kGemmMmaWarps + 1);  // + the TMA producer warp
-constexpr int kStageBytesPerWarp = 4096;                // per epilogue warp (EpiTma): one TMA box of 32 x 128 B
 
-template <int BN, int kStagingOverride = 0>
+template <int BN, int kStaging>
 struct GemmCfg {
   static constexpr int kABytes = kGemmBM * kGemmBK * 2;
   static constexpr int kBBytes = BN * kGemmBK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;  // 32 KB (BN 128) / 48 KB (BN 256)
   static constexpr int kBarrierBytes = 512;
   static constexpr int kAccBytes = kGemmBM * BN * 4;     // the fp32 accumulator handed to the epilogue
-  // epilogue staging: one 4 KB box per epilogue warp; an epilogue that needs another size states its own total
-  static constexpr int kStagingBytes = kStagingOverride > 0 ? kStagingOverride : kGemmMmaWarps * kStageBytesPerWarp;
+  static constexpr int kStagingBytes = kStaging;         // the epilogue's own shared memory (Epi::kStagingBytes)
   static constexpr int kStagesFit = (232448 - 1024 - kAccBytes - kStagingBytes - kBarrierBytes) / kStageBytes;
   static constexpr int kStages = kStagesFit < 4 ? kStagesFit : 4;
   static_assert(kStages >= 2, "not enough shared memory for a double-buffered mainloop");
@@ -53,18 +47,6 @@ struct GemmCfg {
   static constexpr int kSmemBytes = 1024 + kStages * kStageBytes + kAccBytes + kStagingBytes + kBarrierBytes;
   static_assert(kSmemBytes <= 232448, "exceeds the 227 KB per-CTA shared memory limit");
 };
-
-// Epilogue states with a `ks` member are told which K slice of a split-K launch the current work unit covers
-template <class State, class = void>
-struct StateHasKs { static constexpr bool value = false; };
-template <class State>
-struct StateHasKs<State, decltype((void)State::ks)> { static constexpr bool value = true; };
-
-// Epilogues may state a total staging size (kStagingBytes member); 0 / absent = the default rule of GemmCfg.
-template <class Epi, class = void>
-struct EpiStaging { static constexpr int value = 0; };
-template <class Epi>
-struct EpiStaging<Epi, decltype((void)Epi::kStagingBytes)> { static constexpr int value = Epi::kStagingBytes; };
 
 // [0] SM cycles, [1] nanoseconds spent inside GEMM kernels (sgpt_profile_gemm_clock); one thread per launch adds to it
 __device__ unsigned long long g_gemm_clock[2];
@@ -175,7 +157,7 @@ template <int BN, class Epi, int CL = 1, bool kS8 = false, bool kUnits = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, int M,
                     int N, int K, const __grid_constant__ typename Epi::Params ep, TileMap tmap) {
-  using Cfg = GemmCfg<BN, EpiStaging<Epi>::value>;
+  using Cfg = GemmCfg<BN, Epi::kStagingBytes>;
   using Acc = typename std::conditional<kS8, int32_t, float>::type;
   constexpr int kBK = kS8 ? 2 * kGemmBK : kGemmBK;  // K elements per k-block (128 bytes per row either way)
   constexpr int kMmaK = kS8 ? 32 : 16;              // K elements per wgmma
@@ -269,7 +251,6 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
     for (int unit = cid; unit < num_tiles; unit += ncl) {
       const int tile = unit / ksplit;
       const int ks = unit - tile * ksplit;
-      if constexpr (StateHasKs<typename Epi::State>::value) st.ks = static_cast<uint32_t>(ks);
       int m0, n0, Me = M, Ne = N;  // this warp's 32-row slab / column half, and the bounds its epilogue sees
       if constexpr (kUnits) {
         const int4 u = __ldg(ep.units + unit);
@@ -357,94 +338,218 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// TMA epilogue driver: accumulator -> registers (thread = row) -> Op (bias / activation) -> swizzled smem box -> TMA
+// Linear-layer GEMM: out[M,N] (bf16) = Op(A[M,K] B[N,K]^T), written by TMA as a tensor store or a reduce-add.
+//
+// Roles (3 warpgroups = 384 threads, 1 CTA per SM):
+//   warpgroup 0      TMA producer (one lane), lowered to 40 registers per thread (setmaxnreg.dec)
+//   warpgroups 1, 2  consumers, raised to 232 registers per thread (setmaxnreg.inc).  Consumer c takes work units
+//                    c, c + 2, c + 4, ... of the CTA's sequence and computes each whole 128 x 128 tile (two m64n128k16
+//                    per K step, 128 fp32 accumulators per thread), then runs its epilogue.
+// Ping-pong: once a consumer has issued its last k-block it arrives at the other consumer's turn barrier, so one
+// consumer's mainloop runs while the other runs its epilogue (kBarTurn + c, 256 threads: every arrive is matched by the
+// one wait of the next unit).  The producer walks the same unit sequence (TileMap banding, split-K); each ring stage is
+// read by the one consumer that owns the unit, so it is released by 4 arrivals, one per warp of that warpgroup.
+// Epilogue: Op::pair maps each fp32 accumulator pair to two bf16 in registers; the words go to the consumer's own 32 KB
+// output tile (8 SWIZZLE_128B boxes of 32 rows x 64 columns, the box of the output tensor map) and one thread hands the
+// boxes to the TMA engine.  The tile is rewritten only once the previous tile's stores have read it (wait_group.read),
+// which by then lies a whole mainloop back.  The score epilogues keep gemm_bf16_tn_kernel: they need a thread to own a
+// query row (per-row thresholds and candidate lists), i.e. the fp32 hand-over through shared memory.
 // ---------------------------------------------------------------------------------------------------------------
-struct EpiTmaState {
-  uint32_t it;  // boxes issued so far by this warp (selects the double buffer)
-  uint32_t ks;  // K slice of the current work unit (split-K launches; 0 otherwise): only slice 0 adds the bias
+constexpr int kLinThreads = 384;
+constexpr int kLinBN = 128;
+struct LinearCfg {
+  static constexpr int kABytes = kGemmBM * kGemmBK * 2;
+  static constexpr int kStageBytes = kABytes + kLinBN * kGemmBK * 2;  // 32 KB
+  static constexpr int kStages = 4;
+  static constexpr int kOutBytes = kGemmBM * kLinBN * 2;              // one consumer's bf16 output tile
+  static constexpr int kBarrierBytes = 512;
+  // smem: [<=1024 align slack][stages * (A|B)][2 output tiles][barriers]
+  static constexpr int kSmemBytes = 1024 + kStages * kStageBytes + 2 * kOutBytes + kBarrierBytes;
+  static_assert(kSmemBytes <= 232448, "exceeds the 227 KB per-CTA shared memory limit");
 };
+// named barriers of gemm_linear_kernel (0 is __syncthreads): all consumers; turn of consumer c; epilogue of consumer c
+constexpr int kBarConsumers = 1, kBarTurn = 2, kBarEpi = 4;
 
-// Ops whose result is ADDED to the output (TMA reduce-add) can run split-K: they declare kSplitK and take a flag that
-// tells whether this K slice contributes the bias.
-template <class Op, class = void>
-struct OpSplitK { static constexpr bool value = false; };
 template <class Op>
-struct OpSplitK<Op, decltype((void)Op::kSplitK)> { static constexpr bool value = true; };
+__global__ void __launch_bounds__(kLinThreads, 1)
+gemm_linear_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, int M, int N,
+                   int K, const __grid_constant__ typename Op::Params ep, TileMap tmap) {
+  using Cfg = LinearCfg;
+  constexpr int kStages = Cfg::kStages;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem_tiles = smem;
+  uint8_t* out_smem = smem + kStages * Cfg::kStageBytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(out_smem + 2 * Cfg::kOutBytes);
+  uint64_t* empty_bar = full_bar + kStages;
+  uint64_t* probe = empty_bar + kStages;  // clock probe: start cycle and time (kept out of the consumers' registers)
 
-template <class Op, int kDebug = 0>  // kDebug: 1 = skip the TMA store (timing experiment), 2 = skip the smem-reuse wait
-struct EpiTma {
-  using Params = typename Op::Params;
-  using State = EpiTmaState;
-  static constexpr int kEpiWarps = 8;  // 2 warps per 32-row slab; each owns ONE 4 KB smem box
-  static constexpr int kCols = 64;     // bf16 columns per 128-byte row segment
-  static __device__ __forceinline__ void init(State& st, const Params&) { st.it = 0; st.ks = 0; }
-  template <int BN, int kSlabBytes>
-  static __device__ __forceinline__ void pre_tile(State&, const Params&, int, int, int, float*, int, int) {}
-  static __device__ __forceinline__ void finish(State&, const Params&, int lane_row) {
-    if ((lane_row & 31) == 0) bulk_wait_group<0>();  // all stores of this warp have fully completed
+  const int m_tiles = (M + kGemmBM - 1) / kGemmBM;
+  const int n_tiles = (N + kLinBN - 1) / kLinBN;
+  const int ksplit = tmap.ksplit;
+  const int num_units = m_tiles * n_tiles * ksplit;
+  const int num_kb = (K + kGemmBK - 1) / kGemmBK;
+  const int kb_per = (num_kb + ksplit - 1) / ksplit;  // k-blocks per slice (the host keeps every slice non-empty)
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tma_a);
+    tma_prefetch_desc(&tma_b);
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 4);  // one arrive per warp of the consumer that owns the stage's unit
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_sync();  // everything above overlapped the previous kernel's tail; global memory is touched only below
+
+  if (threadIdx.x < 128) {
+    // ===================== TMA producer =====================
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
+        const int tile = unit / ksplit, ks = unit - tile * ksplit;
+        int mg, nt;
+        tmap.coords(tile, m_tiles, n_tiles, mg, nt);
+        const int kb_end = min(num_kb, (ks + 1) * kb_per);
+        for (int kb = ks * kb_per; kb < kb_end; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem_tiles + stage * Cfg::kStageBytes;
+          mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+          tma_load_2d(sa, &tma_a, &full_bar[stage], kb * kGemmBK, mg * kGemmBM);
+          tma_load_2d(sa + Cfg::kABytes, &tma_b, &full_bar[stage], kb * kGemmBK, nt * kLinBN);
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+    return;
   }
 
-  template <int BN, int kSlabBytes>
-  static __device__ __forceinline__ void tile(State& st, const Params& p, int m0, int n0, int lane, uint32_t trow,
-                                              float* slab, int M, int N) {
-    if (m0 >= M) return;  // whole 32-row slab out of range (warp-uniform)
-    const uint32_t sbase = smem_u32(slab);
+  // ===================== consumers: whole tiles, alternating =====================
+  setmaxnreg_inc<232>();
+  const int c = (threadIdx.x >> 7) - 1;
+  const int t = threadIdx.x & 127;
+  const int lane = t & 31;
+  const int r0 = 16 * (t >> 5) + (lane >> 2);  // this thread's fragment rows: r0 + {0, 8, 64, 72}
+  const int c0 = 2 * (lane & 3);               // this thread's fragment column pairs: c0 + 8 j, j = 0..15
+  const uint32_t out_tile = smem_u32(out_smem + c * Cfg::kOutBytes);
+  const bool clock_probe = (blockIdx.x == 0 && threadIdx.x == 128);
+  if (clock_probe) {
+    probe[0] = static_cast<uint64_t>(clock64());
+    probe[1] = global_timer_ns();
+  }
+  int stage = 0;
+  uint32_t phase = 0;
+  int i = 0;  // position of the unit in this CTA's sequence
+  for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x, ++i) {
+    const int tile = unit / ksplit, ks = unit - tile * ksplit;
+    const int kb_begin = ks * kb_per, kb_end = min(num_kb, kb_begin + kb_per);
+    if ((i & 1) != c) {  // the other consumer's unit: step over its k-blocks in the ring
+      stage += kb_end - kb_begin;
+      phase ^= static_cast<uint32_t>(stage / kStages) & 1u;
+      stage %= kStages;
+      continue;
+    }
+    float acc0[64], acc1[64];  // rows [0, 64) and [64, 128) of the tile
+#pragma unroll
+    for (int j = 0; j < 64; ++j) acc0[j] = acc1[j] = 0.f;
+    if (i > 0) named_bar_sync(kBarTurn + c, 256);  // the other consumer has issued its last k-block
+    int prev_stage = -1;
+    for (int kb = kb_begin; kb < kb_end; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem_tiles + stage * Cfg::kStageBytes);
+      const uint64_t da0 = make_wgmma_desc_sw128(sa), da1 = make_wgmma_desc_sw128(sa + 64 * 128);
+      const uint64_t db = make_wgmma_desc_sw128(sa + Cfg::kABytes);
+      wgmma_fence_acc(acc0);
+      wgmma_fence_acc(acc1);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kGemmBK / 16; ++k) {
+        const int scale_d = (kb > kb_begin || k > 0) ? 1 : 0;
+        wgmma_bf16_m64n128(acc0, da0 + 2 * k, db + 2 * k, scale_d);
+        wgmma_bf16_m64n128(acc1, da1 + 2 * k, db + 2 * k, scale_d);
+      }
+      wgmma_commit();
+      wgmma_fence_acc(acc0);
+      wgmma_fence_acc(acc1);
+      // one k-block stays in flight: the stage of the PREVIOUS k-block has been read once its group completed
+      wgmma_wait<1>();
+      if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+      prev_stage = stage;
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
+    }
+    if (unit + static_cast<int>(gridDim.x) < num_units) named_bar_arrive(kBarTurn + (c ^ 1), 256);
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc0);
+    wgmma_fence_acc(acc1);
+    if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+
+    int mg, nt;
+    tmap.coords(tile, m_tiles, n_tiles, mg, nt);
+    const int m0 = mg * kGemmBM, n0 = nt * kLinBN;
+    // epilogue: all results are computed before any is stored, so the loads inside Op::rows / Op::col / Op::pair are
+    // ordinary loads the compiler batches up front (the volatile smem stores would otherwise fence them apart)
+    typename Op::Rows rw;
+    Op::rows(ep, rw, m0 + r0, M);
+    uint32_t o[4][16];  // [fragment row][column pair]
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const typename Op::Col cl = Op::col(ep, n0 + c0 + 8 * j, N, ks == 0);
+      o[0][j] = Op::pair(ep, rw, cl, 0, acc0[4 * j], acc0[4 * j + 1]);
+      o[1][j] = Op::pair(ep, rw, cl, 1, acc0[4 * j + 2], acc0[4 * j + 3]);
+      o[2][j] = Op::pair(ep, rw, cl, 2, acc1[4 * j], acc1[4 * j + 1]);
+      o[3][j] = Op::pair(ep, rw, cl, 3, acc1[4 * j + 2], acc1[4 * j + 3]);
+    }
+    if (t == 0) bulk_wait_group_read<0>();  // this consumer's previous stores have read the output tile
+    named_bar_sync(kBarEpi + c, 128);
+    // box b = (row / 32) * 2 + column / 64; 16-byte chunk q of box row rr sits at q ^ (rr & 7), and rr & 7 = lane / 4
+#pragma unroll
+    for (int ri = 0; ri < 4; ++ri) {
+      const int row = r0 + 8 * (ri & 1) + 64 * (ri >> 1);
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const uint32_t box = static_cast<uint32_t>((row >> 5) * 2 + (j >> 3));
+        sts_b32(out_tile + box * 4096u + static_cast<uint32_t>(row & 31) * 128u +
+                    ((static_cast<uint32_t>(j & 7) ^ static_cast<uint32_t>(lane >> 2)) << 4) + 4u * (lane & 3),
+                o[ri][j]);
+      }
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(kBarEpi + c, 128);
+    if (t == 0) {
 #pragma unroll 1
-    for (int c = 0; c < BN; c += kCols) {
-      const int n = n0 + c;
-      if (n >= N) break;  // warp-uniform
-      // kBoxes smem boxes per warp, used round-robin: a box may be rewritten once the TMA store issued kBoxes
-      // iterations ago has finished READING it (the stores themselves complete asynchronously)
-      constexpr int kBoxes = kSlabBytes / 4096;
-      static_assert(kBoxes == 1 || kBoxes == 2, "one or two 4 KB boxes per epilogue warp");
-      const uint32_t box = sbase + (kBoxes == 2 ? (st.it & 1u) * 4096u : 0u);
-      if (st.it >= kBoxes && kDebug == 0) {
-        if (lane == 0) bulk_wait_group_read<kBoxes - 1>();
-        __syncwarp();
+      for (int b = 0; b < 8; ++b) {  // boxes wholly past M or N are skipped; the tensor map clips the others
+        const int bm = m0 + 32 * (b >> 1), bn = n0 + 64 * (b & 1);
+        if (bm < M && bn < N)
+          Op::issue(ep, reinterpret_cast<const void*>(__cvta_shared_to_generic(out_tile + b * 4096u)), bn, bm);
       }
-      uint32_t v[kCols];
-      acc_ld_32(trow + 4 * c, *reinterpret_cast<uint32_t(*)[32]>(&v[0]));
-      acc_ld_32(trow + 4 * (c + 32), *reinterpret_cast<uint32_t(*)[32]>(&v[32]));
-      // 8 chunks of 16 bytes; chunk j of row r lives at position j ^ (r & 7) of the row (SWIZZLE_128B)
-      // All 8 chunks are computed before any of them is stored: the bias / rotary-table loads inside Op::chunk are then
-      // independent ordinary loads the compiler batches up front (one exposed latency per box instead of one per chunk;
-      // the volatile smem stores would otherwise fence them apart).
-      const uint32_t row_addr = box + lane * 128u;
-      uint32_t o[8][4];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        if constexpr (OpSplitK<Op>::value)
-          Op::chunk(p, &v[8 * j], n + 8 * j, N, m0 + lane, o[j], st.ks == 0);
-        else
-          Op::chunk(p, &v[8 * j], n + 8 * j, N, m0 + lane, o[j]);
-      }
-      if (kDebug == 4) {  // experiment: straight 16-byte global stores from the thread = row layout (no smem, no TMA)
-        if (m0 + lane < M) {
-          uint4* g = reinterpret_cast<uint4*>(static_cast<uint8_t*>(p.out_ptr) +
-                                              (static_cast<size_t>(m0 + lane) * p.ldc + n) * 2);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) g[j] = make_uint4(o[j][0], o[j][1], o[j][2], o[j][3]);
-        }
-        ++st.it;
-        continue;
-      }
-#pragma unroll
-      for (int j = 0; j < 8; ++j) sts_v4(row_addr + ((j ^ (lane & 7)) << 4), o[j][0], o[j][1], o[j][2], o[j][3]);
-      if (kDebug != 3) fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0 && kDebug != 1 && kDebug != 3) {
-        Op::issue(p, reinterpret_cast<const void*>(__cvta_shared_to_generic(box)), n, m0);
-        bulk_commit_group();
-      }
-      ++st.it;
+      bulk_commit_group();
     }
   }
-};
-
-// bias index helper: columns beyond N are clipped by the tensor map, their bias is read from the last valid entry
-__device__ __forceinline__ float bias_at(const float* bias, int col, int N) {
-  return bias ? __ldg(bias + (col < N ? col : N - 1)) : 0.f;
+  if (t == 0) bulk_wait_group<0>();  // all stores of this consumer have fully completed
+  named_bar_sync(kBarConsumers, 256);
+  if (clock_probe) {
+    atomicAdd(&g_gemm_clock[0], static_cast<unsigned long long>(clock64()) - probe[0]);
+    atomicAdd(&g_gemm_clock[1], static_cast<unsigned long long>(global_timer_ns()) - probe[1]);
+  }
 }
+
+// ---------------------------------------------------------------------------------------------------------------
+// Linear-layer epilogue ops, applied in the accumulator fragment, whose rows are r, r + 8, r + 64, r + 72 (ri = 0..3) and
+// whose column pairs start at col0 + 8 j (j = 0..15) of the tile: Op::rows fetches what the rows need (r0: global row of
+// ri = 0), Op::col what the pair starting at global column `col` needs, and Op::pair maps the fp32 accumulators of the
+// pair in row ri to two packed bf16.
+// ---------------------------------------------------------------------------------------------------------------
+// bias of columns (col, col + 1), 0 without a bias; columns beyond N are clipped by the tensor map, their bias is read
+// from the last valid entry
+__device__ __forceinline__ float2 bias_pair(const float* bias, int col, int N) {
+  if (bias == nullptr) return make_float2(0.f, 0.f);
+  if (col + 2 <= N) return __ldg(reinterpret_cast<const float2*>(bias + col));
+  return make_float2(__ldg(bias + (col < N ? col : N - 1)), __ldg(bias + (col + 1 < N ? col + 1 : N - 1)));
+}
+struct NoRows {};
 
 // out_bf16[m, n] = act(acc + bias[n])          act = identity | gelu_new
 template <bool kGelu>
@@ -452,29 +557,19 @@ struct OpTmaBiasActBF16 {
   struct Params {
     CUtensorMap out_map;  // bf16 [M, N], box 32 rows x 64 cols, SWIZZLE_128B
     const float* bias;    // may be null
-    void* out_ptr;        // same tensor as out_map (direct-store variant)
-    int ldc;
   };
-  // 8 consecutive columns starting at `col` -> 16 bytes
-  static __device__ __forceinline__ void chunk(const Params& p, const uint32_t* acc, int col, int N,
-                                               int /*row*/, uint32_t (&o)[4]) {
-    float x[8];
-    if (p.bias && col + 8 <= N) {
-      const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + col));
-      const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + col) + 1);
-      const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-      for (int i = 0; i < 8; ++i) x[i] = __uint_as_float(acc[i]) + bb[i];
-    } else {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) x[i] = __uint_as_float(acc[i]) + bias_at(p.bias, col + i, N);
-    }
+  using Rows = NoRows;
+  using Col = float2;  // bias
+  static __device__ __forceinline__ void rows(const Params&, Rows&, int, int) {}
+  static __device__ __forceinline__ Col col(const Params& p, int c, int N, bool) { return bias_pair(p.bias, c, N); }
+  static __device__ __forceinline__ uint32_t pair(const Params&, const Rows&, Col b, int, float x0, float x1) {
+    x0 = x0 + b.x;
+    x1 = x1 + b.y;
     if (kGelu) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) x[i] = gelu_new(x[i]);
+      x0 = gelu_new(x0);
+      x1 = gelu_new(x1);
     }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) o[i] = pack_bf16(x[2 * i], x[2 * i + 1]);
+    return pack_bf16(x0, x1);
   }
   static __device__ __forceinline__ void issue(const Params& p, const void* box, int n, int m0) {
     tma_store_2d(&p.out_map, box, n, m0);
@@ -483,38 +578,38 @@ struct OpTmaBiasActBF16 {
 
 // GPT-J fused q/k/v projection: out_bf16[m, n] = rotary(acc) for the first `rotary_dim` dims of every q and k head
 // (HF:gptj/modeling_gptj.py:55-67, 196-207: interleaved pairs (x[2i], x[2i+1]) -> (x[2i] c - x[2i+1] s, x[2i+1] c + x[2i] s)
-// with angle pos[m] * 10000^(-2i/rotary_dim)); v columns and the non-rotary dims pass through.  No bias (:98-101).
+// with angle pos[m] * 10000^(-2i/rotary_dim)); v columns and the non-rotary dims pass through.  No bias (:98-101).  The
+// rotated pairs are exactly the accumulator fragment's column pairs.
 struct OpTmaRotaryBF16 {
   struct Params {
     CUtensorMap out_map;     // bf16 [M, 3d]
     const int32_t* pos;      // [M] position of each token row
     const float2* table;     // [max_pos, rotary_dim/2] (cos, sin)
     int M, d_model, head_dim, rotary_dim, max_pos;
-    void* out_ptr;
-    int ldc;
   };
-  static __device__ __forceinline__ void chunk(const Params& p, const uint32_t* acc, int col, int N, int row,
-                                               uint32_t (&o)[4]) {
-    float x[8];
+  struct Rows { const float2* t[4]; };  // the table row of each fragment row's position
+  using Col = int;                       // rotated pair: its index in the head's table row; -1: passes through
+  static __device__ __forceinline__ void rows(const Params& p, Rows& rw, int r0, int) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) x[i] = __uint_as_float(acc[i]);
-    const int in_head = col % p.head_dim;  // 8-column chunks never straddle heads (head_dim % 8 == 0)
-    if (col < 2 * p.d_model && in_head < p.rotary_dim) {
+    for (int ri = 0; ri < 4; ++ri) {
+      const int row = r0 + 8 * (ri & 1) + 64 * (ri >> 1);
       int ps = __ldg(p.pos + (row < p.M ? row : p.M - 1));
       ps = min(max(ps, 0), p.max_pos - 1);
-      const float4* t4 = reinterpret_cast<const float4*>(p.table + static_cast<size_t>(ps) * (p.rotary_dim >> 1) +
-                                                         (in_head >> 1));
-      const float4 a = __ldg(t4), b = __ldg(t4 + 1);  // (c0,s0,c1,s1), (c2,s2,c3,s3)
-      const float cs[4] = {a.x, a.z, b.x, b.z}, sn[4] = {a.y, a.w, b.y, b.w};
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float e = x[2 * i], od = x[2 * i + 1];
-        x[2 * i] = e * cs[i] - od * sn[i];
-        x[2 * i + 1] = od * cs[i] + e * sn[i];
-      }
+      rw.t[ri] = p.table + static_cast<size_t>(ps) * (p.rotary_dim >> 1);
     }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) o[i] = pack_bf16(x[2 * i], x[2 * i + 1]);
+  }
+  static __device__ __forceinline__ Col col(const Params& p, int c, int, bool) {
+    const int in_head = c % p.head_dim;
+    return (c < 2 * p.d_model && in_head < p.rotary_dim) ? (in_head >> 1) : -1;
+  }
+  static __device__ __forceinline__ uint32_t pair(const Params&, const Rows& rw, Col k, int ri, float x0, float x1) {
+    if (k >= 0) {
+      const float2 cs = __ldg(rw.t[ri] + k);
+      const float e = x0, od = x1;
+      x0 = e * cs.x - od * cs.y;
+      x1 = od * cs.x + e * cs.y;
+    }
+    return pack_bf16(x0, x1);
   }
   static __device__ __forceinline__ void issue(const Params& p, const void* box, int n, int m0) {
     tma_store_2d(&p.out_map, box, n, m0);
@@ -522,31 +617,20 @@ struct OpTmaRotaryBF16 {
 };
 
 // resid_bf16[m, n] += acc + bias[n]     (the residual stream updated in place by a bf16 TMA reduce-add performed by
-// the L2: no residual load in the SM)
+// the L2: no residual load in the SM).  Split-K: every K slice adds its partial sum, only slice 0 adds the bias.
 struct OpTmaResidAddBF16 {
   struct Params {
     CUtensorMap out_map;  // bf16 [M, N], box 32 rows x 64 cols, SWIZZLE_128B
     const float* bias;    // may be null
-    void* out_ptr;
-    int ldc;
   };
-  static constexpr bool kSplitK = true;
-  static __device__ __forceinline__ void chunk(const Params& p, const uint32_t* acc, int col, int N,
-                                               int /*row*/, uint32_t (&o)[4], bool add_bias) {
-    const float* bias = add_bias ? p.bias : nullptr;
-    float x[8];
-    if (bias && col + 8 <= N) {
-      const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias + col));
-      const float4 b1 = __ldg(reinterpret_cast<const float4*>(bias + col) + 1);
-      const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-      for (int i = 0; i < 8; ++i) x[i] = __uint_as_float(acc[i]) + bb[i];
-    } else {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) x[i] = __uint_as_float(acc[i]) + bias_at(bias, col + i, N);
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) o[i] = pack_bf16(x[2 * i], x[2 * i + 1]);
+  using Rows = NoRows;
+  using Col = float2;  // bias (0 in the K slices after the first)
+  static __device__ __forceinline__ void rows(const Params&, Rows&, int, int) {}
+  static __device__ __forceinline__ Col col(const Params& p, int c, int N, bool first_slice) {
+    return bias_pair(first_slice ? p.bias : nullptr, c, N);
+  }
+  static __device__ __forceinline__ uint32_t pair(const Params&, const Rows&, Col b, int, float x0, float x1) {
+    return pack_bf16(x0 + b.x, x1 + b.y);
   }
   static __device__ __forceinline__ void issue(const Params& p, const void* box, int n, int m0) {
     tma_reduce_add_2d(&p.out_map, box, n, m0);
@@ -565,6 +649,7 @@ struct EpiStaged {
   using Params = typename Op::Params;
   using State = EpiNoState;
   static constexpr int kEpiWarps = 4;
+  static constexpr int kStagingBytes = kEpiWarps * 32 * 256;  // one [32 x 32] float2 slab per epilogue warp
   static __device__ __forceinline__ void init(State&, const Params&) {}
   template <int BN, int kSlabBytes>
   static __device__ __forceinline__ void pre_tile(State&, const Params&, int, int, int, float*, int, int) {}
@@ -1025,17 +1110,14 @@ using EpiIvfRows = EpiIvfRowsT<false>;
 using EpiIvfRowsMasked = EpiIvfRowsT<true>;
 
 
-template <bool kGelu>
-using EpiBiasActBF16 = EpiTma<OpTmaBiasActBF16<kGelu>>;
-using EpiResidualBF16 = EpiTma<OpTmaResidAddBF16>;
-using EpiRotaryBF16 = EpiTma<OpTmaRotaryBF16>;
-
-// Bring-up / profiling aids (sgpt_linear epilogue codes 100, 101): no epilogue work at all, or accumulator loads only.
+// Profiling aids (sgpt_linear epilogue codes 100, 101): the mainloop and the accumulator hand-over with no epilogue work
+// at all, or with the accumulator loads only.
 template <bool kLoad>
 struct EpiDebugNull {
   struct Params { int dummy; };
   using State = EpiNoState;
   static constexpr int kEpiWarps = 4;
+  static constexpr int kStagingBytes = EpiStaged<OpScoresF32T<false>>::kStagingBytes;  // (none used)
   static __device__ __forceinline__ void init(State&, const Params&) {}
   template <int BN, int kSlabBytes>
   static __device__ __forceinline__ void pre_tile(State&, const Params&, int, int, int, float*, int, int) {}
