@@ -45,7 +45,8 @@ const char* sgpt_last_error(void);
  * into it with a bf16 TMA reduce.  Sums and statistics are fp32. */
 
 /* F1. resid[t,:] = bf16(wte[ids[t],:] (+ wpe[pos[t],:] if wpe != NULL))       HF:gpt_neo/modeling_gpt_neo.py:462-463
- *     ids,pos int32[T]; wte bf16[vocab,d]; wpe bf16[max_pos,d] or NULL (GPT-J / BLOOM); resid bf16[T,d]. */
+ *     ids,pos int32[T]; wte bf16[vocab,d]; wpe bf16[max_pos,d] or NULL (GPT-J / BLOOM); resid bf16[T,d].
+ *     An id outside [0, vocab) or a position outside [0, max_pos) is clamped to the nearest row of its table. */
 int sgpt_embed_tokens(const int32_t* ids, const int32_t* pos, const void* wte, const void* wpe, void* resid, int T,
                       int d, int vocab, int max_pos, sgpt_stream_t stream);
 
@@ -108,7 +109,8 @@ int sgpt_attention(const void* qkv, void* out, const int32_t* cu_seqlens, int B,
  *     the index instead of reading out of bounds.
  *     out = (accumulate ? out : 0) + out_scale * pool(x): the building block of the all-hidden-state modes below; mode
  *     is one of MEAN / WEIGHTEDMEAN / LASTTOKEN; normalize (if set) acts on the accumulated rows, so pass it with the
- *     last state.
+ *     last state.  The result is bit-reproducible: a sequence's row depends neither on the launch nor on the sequence's
+ *     position in the batch.
  * ------------------------------------------------------------------------------------------------------------------ */
 #define SGPT_POOL_MEAN 0
 #define SGPT_POOL_WEIGHTEDMEAN 1
@@ -219,7 +221,9 @@ int sgpt_lm_logprobs(sgpt_model_t m, const void* lm_head_w, const float* lm_head
                      int rows_per_chunk, sgpt_stream_t stream);
 
 /* Building blocks of the above.  sgpt_token_logprobs: logits fp32[M,lds] (vocab valid columns) -> log-softmax value of
- * the target column per row (+ optional argmax).  sgpt_segment_sum: out[r] = sum(x[offsets[r]..offsets[r+1])) in index
+ * the target column per row (+ optional argmax: the lowest index of the largest value that is not NaN, so a row of -inf
+ * gives 0; NaN is never chosen, where torch.argmax would return the first NaN, and a row of NaN only gives 0).
+ * sgpt_segment_sum: out[r] = sum(x[offsets[r]..offsets[r+1])) in index
  * order — the per-request `float(logits.sum())` of sgptce.py:250; offsets int32[R+1]. */
 int sgpt_token_logprobs(const float* logits, int64_t lds, int M, int vocab, const float* bias, const int32_t* targets,
                         float* logprob, int32_t* greedy, sgpt_stream_t stream);

@@ -359,8 +359,8 @@ __global__ void __launch_bounds__(128) pool_kernel(const void* __restrict__ x, c
                                                    const float* __restrict__ pw, int n_pw,
                                                    const int32_t* __restrict__ cu, const float2* __restrict__ stats,
                                                    const float4* __restrict__ g, const float4* __restrict__ bta,
-                                                   float4* __restrict__ out, float* __restrict__ sumsq, int d4,
-                                                   int mode, int clamp_den, int accumulate, float out_scale,
+                                                   float4* __restrict__ out, int d4, int mode, int clamp_den,
+                                                   int accumulate, float out_scale,
                                                    int x_bf16) {
   pdl_sync();  // programmatic dependent launch: see common.cuh
   __shared__ float4 part[4][32];
@@ -421,11 +421,6 @@ __global__ void __launch_bounds__(128) pool_kernel(const void* __restrict__ x, c
       o.x += prev.x; o.y += prev.y; o.z += prev.z; o.w += prev.w;
     }
     if (col_ok) out[static_cast<size_t>(b) * d4 + col] = o;
-    if (sumsq != nullptr) {
-      float ss = col_ok ? (o.x * o.x + o.y * o.y) + (o.z * o.z + o.w * o.w) : 0.f;
-      ss = warp_sum(ss);
-      if (threadIdx.x == 0) atomicAdd(sumsq + b, ss);
-    }
   }
 }
 
@@ -544,18 +539,28 @@ __global__ void __launch_bounds__(256) pool_lnf_fused_kernel(const void* __restr
   if (col < d4) out[static_cast<size_t>(b) * d4 + col] = o;
 }
 
-// P2: x[b,:] /= max(sqrt(sumsq[b]), 1e-12)      (F.normalize(p=2, dim=1))
-__global__ void __launch_bounds__(256) l2_scale_rows_kernel(float4* __restrict__ x, const float* __restrict__ sumsq,
-                                                            int B, int d4) {
+// P2: x[b,:] /= max(||x[b,:]||_2, 1e-12)      (F.normalize(p=2, dim=1)).  One CTA per row sums the squares in a fixed
+// order, so a row's result depends neither on the launch nor on the other rows of the batch.
+__global__ void __launch_bounds__(256) l2_scale_rows_kernel(float4* __restrict__ x, int d4) {
   pdl_sync();  // programmatic dependent launch: see common.cuh
-  const long long total = static_cast<long long>(B) * d4;
-  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int b = static_cast<int>(i / d4);
-    const float inv = 1.0f / fmaxf(sqrtf(__ldg(sumsq + b)), 1e-12f);
-    float4 v = x[i];
+  __shared__ float s_ss[8];
+  float4* r = x + static_cast<size_t>(blockIdx.x) * d4;
+  float ss = 0.f;
+  for (int c = threadIdx.x; c < d4; c += 256) {
+    const float4 v = r[c];
+    ss += (v.x * v.x + v.y * v.y) + (v.z * v.z + v.w * v.w);
+  }
+  ss = warp_sum(ss);
+  if ((threadIdx.x & 31) == 0) s_ss[threadIdx.x >> 5] = ss;
+  __syncthreads();
+  float tot = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) tot += s_ss[i];
+  const float inv = 1.0f / fmaxf(sqrtf(tot), 1e-12f);
+  for (int c = threadIdx.x; c < d4; c += 256) {
+    float4 v = r[c];
     v.x *= inv; v.y *= inv; v.z *= inv; v.w *= inv;
-    x[i] = v;
+    r[c] = v;
   }
 }
 
@@ -744,19 +749,17 @@ extern "C" int sgpt_layernorm_gather(const void* x, const int32_t* row_idx, cons
 // `stats`: (mean, rstd) per row, or null (no ln_f)
 static int pool_launch(const void* x, int x_bf16, const int32_t* pos, const int32_t* cu_seqlens, const float* gamma,
                        const float* beta, const float* pos_weights, int n_pos_weights, float* out, const float2* stats,
-                       float* sumsq, int B, int d, int mode, int clamp_denominator, int normalize, int accumulate,
-                       float out_scale, cudaStream_t stream) {
+                       int B, int d, int mode, int clamp_denominator, int normalize, int accumulate, float out_scale,
+                       cudaStream_t stream) {
   const int d4 = d / 4;
-  if (normalize) SGPT_CHECK_CUDA(cudaMemsetAsync(sumsq, 0, sizeof(float) * B, stream));
   dim3 grid(B, (d4 + 31) / 32);
   SGPT_CHECK_CUDA(launch_kernel(pool_kernel, grid, dim3(128), 0, stream, x, pos,
                                 pos_weights, n_pos_weights, cu_seqlens, stats, reinterpret_cast<const float4*>(gamma),
-                                reinterpret_cast<const float4*>(beta), reinterpret_cast<float4*>(out),
-                                normalize ? sumsq : nullptr, d4, mode, clamp_denominator, accumulate, out_scale,
-                                x_bf16));
+                                reinterpret_cast<const float4*>(beta), reinterpret_cast<float4*>(out), d4, mode,
+                                clamp_denominator, accumulate, out_scale, x_bf16));
   if (normalize) {
-    SGPT_CHECK_CUDA(launch_kernel(l2_scale_rows_kernel, dim3(grid_for(static_cast<long long>(B) * d4, 256)), dim3(256),
-                                  0, stream, reinterpret_cast<float4*>(out), sumsq, B, d4));
+    SGPT_CHECK_CUDA(launch_kernel(l2_scale_rows_kernel, dim3(B), dim3(256), 0, stream, reinterpret_cast<float4*>(out),
+                                  d4));
   }
   return SGPT_OK;
 }
@@ -800,9 +803,8 @@ extern "C" int sgpt_pool(const void* x, int x_bf16, const int32_t* pos, const in
     SGPT_CHECK_CUDA(cudaGetLastError());
     stats = reinterpret_cast<const float2*>(row_stats_ws);
   }
-  return pool_launch(x, x_bf16, pos, cu_seqlens, gamma, beta, pos_weights, n_pos_weights, out, stats,
-                     normalize ? row_stats_ws + 2 * static_cast<size_t>(T) : nullptr, B, d, mode, clamp_denominator,
-                     normalize, accumulate, out_scale, stream);
+  return pool_launch(x, x_bf16, pos, cu_seqlens, gamma, beta, pos_weights, n_pos_weights, out, stats, B, d, mode,
+                     clamp_denominator, normalize, accumulate, out_scale, stream);
 }
 
 extern "C" int sgpt_normalize_rows(float* x, int B, int d, sgpt_stream_t stream_) {

@@ -6,6 +6,7 @@
 // The [rows, vocab] fp32 logits live only in the caller's workspace, a chunk of rows at a time; the full
 // [batch, seq, vocab] tensor of the reference (:221) is never formed.
 #include <float.h>
+#include <math.h>
 
 #include "../../include/sgpt_b200.h"
 #include "common.cuh"
@@ -25,11 +26,13 @@ __global__ void __launch_bounds__(256) token_logprob_kernel(const float* __restr
   const int row = blockIdx.x;
   const float* z = logits + static_cast<size_t>(row) * lds;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  float m = -FLT_MAX;
+  float m = -INFINITY;
   int mi = 0x7fffffff;
   for (int v = threadIdx.x; v < vocab; v += 256) {
     const float x = z[v] + (bias != nullptr ? __ldg(bias + v) : 0.f);
-    if (x > m) { m = x; mi = v; }  // strided ascending visit: the first maximum a thread meets has its lowest index
+    // strided ascending visit: the first maximum a thread meets has its lowest index; a row of -inf takes its first
+    // entry, and NaN is never taken (no comparison with it is true)
+    if (x > m || (x == m && v < mi)) { m = x; mi = v; }
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
@@ -45,7 +48,7 @@ __global__ void __launch_bounds__(256) token_logprob_kernel(const float* __restr
     for (int w = 1; w < 8; ++w)
       if (s_val[w] > bm || (s_val[w] == bm && s_idx[w] < bi)) { bm = s_val[w]; bi = s_idx[w]; }
     s_bcast = bm;
-    if (greedy != nullptr) greedy[row] = bi;
+    if (greedy != nullptr) greedy[row] = bi == 0x7fffffff ? 0 : bi;  // a row of NaN only: 0, as torch.argmax
   }
   __syncthreads();
   const float mx = s_bcast;
