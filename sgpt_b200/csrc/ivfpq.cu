@@ -25,40 +25,58 @@ namespace {
 
 constexpr int kPqBlock = 256;     // queries per block of sgpt_ivfpq_search (blocks reuse the workspace)
 constexpr int kTile = 256;        // documents per staged code tile = threads of the scan CTA
-constexpr int kWholeMaxM = 128;   // m up to this: the query's whole table (m KB) stays in shared memory for the unit
+constexpr int kWholeMaxM = 128;   // 8-bit m up to this: the query's whole table (m KB) stays in shared memory for the unit
 constexpr int kChunkM = 64;       // larger m: table and codes staged kChunkM subspaces per step, two buffers of each
 constexpr int kThreads = 256;
 constexpr int kBarBytes = 128;    // the three mbarriers, padded
 constexpr int kMaxM = 4096;
 constexpr int kMaxCandidates = 1 << 24;
+// 4-bit codes: a table is m x 64 bytes, so the code buffers dominate shared memory.  The limits keep the staged code rows
+// at the 8-bit sizes (whole rows of at most 128 bytes, chunks of 64 bytes): m <= 256 takes 88 KB (2 CTAs per SM), the
+// chunked path 56 KB (4 CTAs), m = 96 30 KB.
+constexpr int kWholeMaxM4 = 256;
+constexpr int kChunkM4 = 128;
+constexpr int kMinBlocks4 = 4;    // __launch_bounds__ of the 4-bit scan: at most 64 registers per thread
+
+template <int kBits> __host__ __device__ constexpr int whole_max_m() { return kBits == 8 ? kWholeMaxM : kWholeMaxM4; }
+template <int kBits> __host__ __device__ constexpr int chunk_m() { return kBits == 8 ? kChunkM : kChunkM4; }
+// bytes of `subspaces` codes of one document
+template <int kBits> __host__ __device__ constexpr int code_bytes(int subspaces) {
+  return kBits == 8 ? subspaces : subspaces >> 1;
+}
 
 inline int64_t align256(int64_t x) { return (x + 255) & ~int64_t(255); }
 
 // Shared-memory pitch of a staged code row of `bytes` (a multiple of 16): an odd number of 16-byte units, so that the
-// 16-byte code reads of 8 consecutive threads (one shared-memory wavefront) hit 8 distinct bank groups.
+// 16-byte code reads of 8 consecutive threads (one shared-memory wavefront) hit 8 distinct bank groups.  4-bit rows are
+// m / 2 bytes, and m % 32 == 0 keeps them (and every 128-subspace chunk) a whole number of 16-byte units.
 __host__ __device__ constexpr int code_pitch(int bytes) { return ((bytes / 16) & 1) ? bytes : bytes + 16; }
 
-template <bool kWhole>
+template <bool kWhole, int kBits = 8>
 size_t scan_smem_bytes(int m) {
-  const int mc = kWhole ? m : kChunkM;
-  const size_t table = kWhole ? static_cast<size_t>(m) * 1024 : 2 * static_cast<size_t>(kChunkM) * 1024;
-  return kBarBytes + 2 * static_cast<size_t>(kTile) * code_pitch(mc) + table;
+  constexpr size_t kTabBytes = static_cast<size_t>(4) << kBits;  // one subspace's table
+  const int mc = kWhole ? m : chunk_m<kBits>();
+  const size_t table = kWhole ? static_cast<size_t>(m) * kTabBytes : 2 * static_cast<size_t>(mc) * kTabBytes;
+  return kBarBytes + 2 * static_cast<size_t>(kTile) * code_pitch(code_bytes<kBits>(mc)) + table;
 }
 
 // ---- tables ---------------------------------------------------------------------------------------------------------
-// lut[q][j][c] = sum_t Q[q][j dsub + t] B[j][c][t], one thread per (q, j, c): an fp32 FMA chain from 0 in ascending t
+// lut[q][j][c] = sum_t Q[q][j dsub + t] B[j][c][t], one thread per (q, j, c), c < 2^kBits: an fp32 FMA chain from 0 in
+// ascending t
+template <int kBits>
 __global__ void __launch_bounds__(kThreads) pq_lut_kernel(const float* __restrict__ Q, const float* __restrict__ cb,
                                                           int nq, int D, int m, float* __restrict__ lut) {
+  constexpr int kK = 1 << kBits;
   pdl_sync();
   const long long i = static_cast<long long>(blockIdx.x) * kThreads + threadIdx.x;
-  if (i >= static_cast<long long>(nq) * m * 256) return;
-  const int c = static_cast<int>(i & 255);
-  const long long qj = i >> 8;
+  if (i >= static_cast<long long>(nq) * m * kK) return;
+  const int c = static_cast<int>(i & (kK - 1));
+  const long long qj = i >> kBits;
   const int j = static_cast<int>(qj % m);
   const long long q = qj / m;
   const int dsub = D / m;
   const float* x = Q + q * D + static_cast<long long>(j) * dsub;
-  const float* b = cb + (static_cast<long long>(j) * 256 + c) * dsub;
+  const float* b = cb + (static_cast<long long>(j) * kK + c) * dsub;
   float acc = 0.f;
   for (int t = 0; t < dsub; ++t) acc = fmaf(__ldg(x + t), __ldg(b + t), acc);
   lut[i] = acc;
@@ -86,9 +104,9 @@ __global__ void __launch_bounds__(kThreads) pq_base_kernel(const float* __restri
 
 // ---- scan -----------------------------------------------------------------------------------------------------------
 struct ScanArgs {
-  const float* lut;         // [nb][m][256] of the block's queries
+  const float* lut;         // [nb][m][2^nbits] of the block's queries
   const float* base;        // [nb][nprobe]
-  const uint8_t* codes;     // [n][m] in list order
+  const uint8_t* codes;     // [n][m nbits / 8] in list order
   int n, m;
   const int64_t* offsets;   // [nlist + 1]
   int nlist;
@@ -109,8 +127,13 @@ struct Step {
   int p, b, e, t, c;
 };
 
-template <bool kWhole>
-__global__ void __launch_bounds__(kThreads, 1) ivfpq_scan_kernel(const ScanArgs a) {
+// kBits = 8: a code is a byte, tables of 256 entries.  kBits = 4: code j is the low (even j) or high (odd j) nibble of
+// byte j / 2, tables of 16 entries; a warp looks up the same subspace at the same time, and its 16 consecutive words sit
+// in 16 distinct banks, so every lookup is one conflict-free wavefront.
+template <bool kWhole, int kBits = 8>
+__global__ void __launch_bounds__(kThreads, kBits == 8 ? 1 : kMinBlocks4) ivfpq_scan_kernel(const ScanArgs a) {
+  constexpr int kK = 1 << kBits;         // table entries per subspace
+  constexpr int kCm = chunk_m<kBits>();  // subspaces per chunk (chunked path)
   extern __shared__ __align__(128) uint8_t smem[];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int units_per_q = (a.nprobe + a.slice - 1) / a.slice;
@@ -120,9 +143,10 @@ __global__ void __launch_bounds__(kThreads, 1) ivfpq_scan_kernel(const ScanArgs 
   const int p_hi = min(a.nprobe, p_lo + a.slice);
   const int t_lo = grp * a.group_tiles, t_hi = t_lo + a.group_tiles;  // this unit's tiles of each list
   const int m = a.m;
-  const int mc = kWhole ? m : kChunkM;  // subspaces per step (the last chunk may hold fewer)
-  const int nc = kWhole ? 1 : (m + kChunkM - 1) / kChunkM;
-  const int pitch = code_pitch(mc);
+  const int row_bytes = code_bytes<kBits>(m);  // of a document's codes in global memory
+  const int mc = kWhole ? m : kCm;  // subspaces per step (the last chunk may hold fewer)
+  const int nc = kWhole ? 1 : (m + kCm - 1) / kCm;
+  const int pitch = code_pitch(code_bytes<kBits>(mc));
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem);  // [0], [1]: the two step buffers; [2]: the whole table
   uint8_t* codes_s = smem + kBarBytes;
   float* lut_s = reinterpret_cast<float*>(codes_s + 2 * kTile * pitch);
@@ -134,7 +158,7 @@ __global__ void __launch_bounds__(kThreads, 1) ivfpq_scan_kernel(const ScanArgs 
   }
   __syncthreads();
   pdl_sync();
-  const float* lut_q = a.lut + static_cast<long long>(ql) * m * 256;
+  const float* lut_q = a.lut + static_cast<long long>(ql) * m * kK;
   const int32_t* probes_q = a.probes + static_cast<long long>(ql) * a.nprobe;
 
   auto seek = [&](Step& s) {  // first probed list at or after probe s.p that has a tile in [t_lo, t_hi)
@@ -163,25 +187,27 @@ __global__ void __launch_bounds__(kThreads, 1) ivfpq_scan_kernel(const ScanArgs 
     if (warp != 0) return;
     const int pos0 = s.b + kTile * s.t;
     const int cnt = min(kTile, s.e - pos0);
-    const int c0 = s.c * kChunkM;
-    const int bytes = kWhole ? m : min(kChunkM, m - c0);
-    if (lane == 0) mbar_expect_tx(bar + buf, static_cast<uint32_t>(cnt * bytes + (kWhole ? 0 : bytes * 1024)));
+    const int c0 = s.c * kCm;
+    const int sub = kWhole ? m : min(kCm, m - c0);  // subspaces of the step
+    const int bytes = code_bytes<kBits>(sub);
+    if (lane == 0) mbar_expect_tx(bar + buf, static_cast<uint32_t>(cnt * bytes + (kWhole ? 0 : sub * kK * 4)));
     __syncwarp();
     if (!kWhole && lane == 0)
-      bulk_load_1d(lut_s + buf * kChunkM * 256, lut_q + static_cast<long long>(c0) * 256,
-                   static_cast<uint32_t>(bytes * 1024), bar + buf);
-    const uint8_t* src = a.codes + static_cast<long long>(pos0) * m + c0;
+      bulk_load_1d(lut_s + buf * kCm * kK, lut_q + static_cast<long long>(c0) * kK, static_cast<uint32_t>(sub * kK * 4),
+                   bar + buf);
+    const uint8_t* src = a.codes + static_cast<long long>(pos0) * row_bytes + code_bytes<kBits>(c0);
     uint8_t* dst = codes_s + buf * kTile * pitch;
     for (int r = lane; r < cnt; r += 32)
-      bulk_load_1d(dst + r * pitch, src + static_cast<long long>(r) * m, static_cast<uint32_t>(bytes), bar + buf);
+      bulk_load_1d(dst + r * pitch, src + static_cast<long long>(r) * row_bytes, static_cast<uint32_t>(bytes),
+                   bar + buf);
   };
 
   Step cur{p_lo, 0, 0, 0, 0};
   seek(cur);
   if (cur.p >= p_hi) return;  // nothing probed (no copy in flight)
   if (kWhole && tid == 0) {
-    mbar_expect_tx(bar + 2, static_cast<uint32_t>(m * 1024));
-    bulk_load_1d(lut_s, lut_q, static_cast<uint32_t>(m * 1024), bar + 2);
+    mbar_expect_tx(bar + 2, static_cast<uint32_t>(m * kK * 4));
+    bulk_load_1d(lut_s, lut_q, static_cast<uint32_t>(m * kK * 4), bar + 2);
   }
   issue(cur, 0);
   uint32_t phase = 0;  // bit b: parity of buffer b's next completion
@@ -196,20 +222,32 @@ __global__ void __launch_bounds__(kThreads, 1) ivfpq_scan_kernel(const ScanArgs 
     phase ^= 1u << buf;
     const int pos0 = cur.b + kTile * cur.t;
     const int cnt = min(kTile, cur.e - pos0);
-    const int c0 = cur.c * kChunkM;
-    const int bytes = kWhole ? m : min(kChunkM, m - c0);
+    const int c0 = cur.c * kCm;
+    const int bytes = code_bytes<kBits>(kWhole ? m : min(kCm, m - c0));
     if (cur.c == 0) acc = 0.f;
     if (tid < cnt) {
       const uint8_t* row = codes_s + buf * kTile * pitch + tid * pitch;
-      const float* tab = kWhole ? lut_s : lut_s + buf * kChunkM * 256;
+      const float* tab = kWhole ? lut_s : lut_s + buf * kCm * kK;
       // acc += lut[j][code[j]] for j ascending: plain fp32 adds in this order (no reassociation without fast-math)
 #pragma unroll 1
       for (int u = 0; u < bytes; u += 16) {
         const uint4 v = *reinterpret_cast<const uint4*>(row + u);
-        const float* tj = tab + u * 256;
+        const float* tj = tab + u * (8 / kBits) * kK;  // the table of the unit's first subspace
         const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+        if constexpr (kBits == 8) {
 #pragma unroll
-        for (int i = 0; i < 16; ++i) acc += tj[i * 256 + ((w[i >> 2] >> (8 * (i & 3))) & 255u)];
+          for (int i = 0; i < 16; ++i) acc += tj[i * 256 + ((w[i >> 2] >> (8 * (i & 3))) & 255u)];
+        } else {
+          // code i of the unit is bits 4 (i & 7) .. 4 (i & 7) + 3 of word i / 8; its byte offset 4 code in the table
+          // of subspace i is taken straight from the word, so a lookup is a shift, a mask, an add and the load
+          const char* tb = reinterpret_cast<const char*>(tj);
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            const uint32_t x = w[i >> 3];
+            const uint32_t off = ((i & 7) == 0 ? x << 2 : x >> (4 * (i & 7) - 2)) & 0x3cu;
+            acc += *reinterpret_cast<const float*>(tb + i * 64 + off);
+          }
+        }
       }
     }
     if (cur.c == nc - 1) {  // block-uniform: the tile's scores are complete
@@ -343,17 +381,21 @@ int check_rerank_sizes(const char* fn, int nq, int64_t kc) {
   return SGPT_OK;
 }
 
-}  // namespace
+// the code width rules of the _nbits entry points (after the m rule)
+int check_nbits(const char* fn, int m, int nbits) {
+  SGPT_REQUIRE(nbits == 4 || nbits == 8, "%s: nbits=%d must be 4 or 8", fn, nbits);
+  SGPT_REQUIRE(nbits == 8 || m % 32 == 0, "%s: m=%d must be a multiple of 32 for 4-bit codes", fn, m);
+  return SGPT_OK;
+}
 
-extern "C" int sgpt_pq_tables(const float* Q, const float* codebooks, const float* centroids, const int32_t* probes,
-                              int nq, int D, int m, int nlist, int nprobe, float* lut_out, float* base_out,
-                              sgpt_stream_t stream_) {
-  const char* fn = "sgpt_pq_tables";
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+int pq_tables(const char* fn, const float* Q, const float* codebooks, const float* centroids, const int32_t* probes,
+              int nq, int D, int m, int nbits, int nlist, int nprobe, float* lut_out, float* base_out,
+              cudaStream_t stream) {
   SGPT_REQUIRE(nq >= 0, "%s: bad query count nq=%d", fn, nq);
   SGPT_REQUIRE(D > 0 && D % 8 == 0, "%s: D=%d must be a positive multiple of 8", fn, D);
   SGPT_REQUIRE(m >= 16 && m % 16 == 0 && m <= kMaxM, "%s: m=%d must be a positive multiple of 16, at most %d", fn, m,
                kMaxM);
+  if (check_nbits(fn, m, nbits) != SGPT_OK) return SGPT_ERR_INVALID;
   SGPT_REQUIRE(D % m == 0, "%s: D=%d is not a multiple of m=%d", fn, D, m);
   SGPT_REQUIRE(nlist >= 1, "%s: nlist=%d must be positive", fn, nlist);
   SGPT_REQUIRE(nprobe >= 1 && nprobe <= nlist, "%s: nprobe=%d outside [1, nlist=%d]", fn, nprobe, nlist);
@@ -361,27 +403,51 @@ extern "C" int sgpt_pq_tables(const float* Q, const float* codebooks, const floa
                "%s: null input (Q, codebooks, centroids and probes are required)", fn);
   SGPT_REQUIRE(lut_out != nullptr && base_out != nullptr, "%s: null output", fn);
   if (nq == 0) return SGPT_OK;
-  const long long entries = static_cast<long long>(nq) * m * 256, pairs = static_cast<long long>(nq) * nprobe;
+  const long long entries = (static_cast<long long>(nq) * m) << nbits, pairs = static_cast<long long>(nq) * nprobe;
+  const dim3 grid(static_cast<unsigned>((entries + kThreads - 1) / kThreads));
   LaunchScope _ls(kCatMisc, stream);
-  SGPT_CHECK_CUDA(launch_kernel(pq_lut_kernel, dim3(static_cast<unsigned>((entries + kThreads - 1) / kThreads)),
-                                dim3(kThreads), 0, stream, Q, codebooks, nq, D, m, lut_out));
+  if (nbits == 8)
+    SGPT_CHECK_CUDA(launch_kernel(pq_lut_kernel<8>, grid, dim3(kThreads), 0, stream, Q, codebooks, nq, D, m, lut_out));
+  else
+    SGPT_CHECK_CUDA(launch_kernel(pq_lut_kernel<4>, grid, dim3(kThreads), 0, stream, Q, codebooks, nq, D, m, lut_out));
   SGPT_CHECK_CUDA(launch_kernel(pq_base_kernel, dim3(static_cast<unsigned>((pairs + kThreads - 1) / kThreads)),
                                 dim3(kThreads), 0, stream, Q, centroids, probes, nq, D, nlist, nprobe, base_out));
   return SGPT_OK;
 }
 
-extern "C" int64_t sgpt_ivfpq_search_workspace_bytes(int nq, int nlist, int nprobe, int64_t max_list_len, int m) {
-  if (check_pq_sizes("sgpt_ivfpq_search_workspace_bytes", nq, nlist, nprobe, max_list_len, m) != SGPT_OK) return -1;
-  return make_pq_layout(nq, nlist, nprobe, max_list_len).total;
+// The scan instantiation of a code width: whole table or chunks, its shared memory, and the scan CTAs an SM holds
+struct ScanLaunch {
+  void (*kernel)(const ScanArgs);
+  size_t smem;
+  int per_sm;
+};
+
+template <int kBits>
+cudaError_t scan_launch(int m, ScanLaunch& l) {
+  const bool whole = m <= whole_max_m<kBits>();
+  l.kernel = whole ? ivfpq_scan_kernel<true, kBits> : ivfpq_scan_kernel<false, kBits>;
+  l.smem = whole ? scan_smem_bytes<true, kBits>(m) : scan_smem_bytes<false, kBits>(m);
+  l.per_sm = 1;
+  static PerDeviceOnce attr_once;
+  if (attr_once.first()) {
+    cudaError_t e = cudaFuncSetAttribute(ivfpq_scan_kernel<true, kBits>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         static_cast<int>(scan_smem_bytes<true, kBits>(whole_max_m<kBits>())));
+    if (e != cudaSuccess) return e;
+    e = cudaFuncSetAttribute(ivfpq_scan_kernel<false, kBits>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             static_cast<int>(scan_smem_bytes<false, kBits>(whole_max_m<kBits>() + 32)));
+    if (e != cudaSuccess) return e;
+  }
+  // 8-bit: one CTA per SM (its table takes up to 128 KB).  4-bit: as many as the registers and shared memory allow
+  if (kBits == 4) return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&l.per_sm, l.kernel, kThreads, l.smem);
+  return cudaSuccess;
 }
 
-extern "C" int sgpt_ivfpq_search(const float* lut, const float* base, const uint8_t* codes, int nq, int64_t n, int m,
-                                 const int64_t* list_offsets, int nlist, int64_t max_list_len, const int32_t* doc_ids,
-                                 const int32_t* probes, int nprobe, int k, const uint32_t* mask, float* out_scores,
-                                 int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream_) {
-  const char* fn = "sgpt_ivfpq_search";
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+int ivfpq_search(const char* fn, const float* lut, const float* base, const uint8_t* codes, int nq, int64_t n, int m,
+                 int nbits, const int64_t* list_offsets, int nlist, int64_t max_list_len, const int32_t* doc_ids,
+                 const int32_t* probes, int nprobe, int k, const uint32_t* mask, float* out_scores, int64_t* out_ids,
+                 void* ws, int64_t ws_bytes, cudaStream_t stream) {
   if (check_pq_sizes(fn, nq, nlist, nprobe, max_list_len, m) != SGPT_OK) return SGPT_ERR_INVALID;
+  if (check_nbits(fn, m, nbits) != SGPT_OK) return SGPT_ERR_INVALID;
   SGPT_REQUIRE(n >= 0 && n < (1ll << 31), "%s: corpus size n=%lld outside [0, 2^31)", fn, (long long)n);
   SGPT_REQUIRE(max_list_len <= n, "%s: max_list_len=%lld exceeds n=%lld", fn, (long long)max_list_len, (long long)n);
   SGPT_REQUIRE(lut != nullptr && base != nullptr && codes != nullptr && list_offsets != nullptr && doc_ids != nullptr &&
@@ -394,28 +460,22 @@ extern "C" int sgpt_ivfpq_search(const float* lut, const float* base, const uint
   SGPT_REQUIRE(ws != nullptr && ws_bytes >= w.total, "%s: workspace too small (%lld < %lld bytes)", fn,
                (long long)ws_bytes, (long long)w.total);
   if (nq == 0) return SGPT_OK;
-  const bool whole = m <= kWholeMaxM;
-  const size_t smem = whole ? scan_smem_bytes<true>(m) : scan_smem_bytes<false>(m);
-  static PerDeviceOnce attr_once;
-  if (attr_once.first()) {
-    SGPT_CHECK_CUDA(cudaFuncSetAttribute(ivfpq_scan_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         static_cast<int>(scan_smem_bytes<true>(kWholeMaxM))));
-    SGPT_CHECK_CUDA(cudaFuncSetAttribute(ivfpq_scan_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         static_cast<int>(scan_smem_bytes<false>(kWholeMaxM + 16))));
-  }
+  ScanLaunch sl{};
+  SGPT_CHECK_CUDA(nbits == 8 ? scan_launch<8>(m, sl) : scan_launch<4>(m, sl));
   uint8_t* wsb = static_cast<uint8_t*>(ws);
   uint2* cand = reinterpret_cast<uint2*>(wsb + w.cand);
   int* counts = reinterpret_cast<int*>(wsb + w.counts);
-  const int target_units = 2 * sm_count();
+  const int target_units = 2 * (sl.per_sm > 1 ? sl.per_sm : 1) * sm_count();
   for (int q0 = 0; q0 < nq; q0 += kPqBlock) {
     const int nb = nq - q0 < kPqBlock ? nq - q0 : kPqBlock;
     const int32_t* pr = probes + static_cast<long long>(q0) * nprobe;
     int rc = launch_ivf_counts(pr, list_offsets, nlist, static_cast<int>(n), max_list_len, nb, nprobe, counts, nullptr,
                                stream);
     if (rc != SGPT_OK) return rc;
-    // Work units: enough to fill the GPU twice over, with as few table stagings as that allows.  Many pairs: several
-    // probes per unit.  Fewer pairs than that target: one probe per unit, and each list's tiles split into groups
-    // (sized by the longest list, as the lengths are device data), so a long list does not run on a single SM.
+    // Work units: enough to fill every scan CTA slot of the GPU twice over, with as few table stagings as that allows.
+    // Many pairs: several probes per unit.  Fewer pairs than that target: one probe per unit, and each list's tiles
+    // split into groups (sized by the longest list, as the lengths are device data), so a long list does not run on a
+    // single SM.
     const long long pairs = static_cast<long long>(nb) * nprobe;
     long long slice = (pairs + target_units - 1) / target_units;
     slice = slice < 1 ? 1 : (slice > nprobe ? nprobe : slice);
@@ -428,24 +488,58 @@ extern "C" int sgpt_ivfpq_search(const float* lut, const float* base, const uint
     const long long group_tiles = (tiles_max + groups - 1) / groups;
     groups = (tiles_max + group_tiles - 1) / group_tiles;
     const long long units = static_cast<long long>(nb) * ((nprobe + slice - 1) / slice) * groups;
-    ScanArgs a{lut + static_cast<long long>(q0) * m * 256, base + static_cast<long long>(q0) * nprobe, codes,
+    ScanArgs a{lut + ((static_cast<long long>(q0) * m) << nbits), base + static_cast<long long>(q0) * nprobe, codes,
                static_cast<int>(n), m, list_offsets, nlist, static_cast<long long>(max_list_len), doc_ids, pr, nprobe,
                mask, cand, static_cast<long long>(w.Ls), static_cast<int>(slice), static_cast<int>(groups),
                static_cast<int>(group_tiles)};
     {
       LaunchScope _ls(kCatScores, stream);
-      if (whole)
-        SGPT_CHECK_CUDA(launch_kernel(ivfpq_scan_kernel<true>, dim3(static_cast<unsigned>(units)), dim3(kThreads), smem,
-                                      stream, a));
-      else
-        SGPT_CHECK_CUDA(launch_kernel(ivfpq_scan_kernel<false>, dim3(static_cast<unsigned>(units)), dim3(kThreads), smem,
-                                      stream, a));
+      SGPT_CHECK_CUDA(launch_kernel(sl.kernel, dim3(static_cast<unsigned>(units)), dim3(kThreads), sl.smem, stream, a));
     }
     rc = launch_ivf_select(cand, counts, nb, nprobe, w.Ls, k, out_scores + static_cast<long long>(q0) * k,
                            out_ids + static_cast<long long>(q0) * k, stream);
     if (rc != SGPT_OK) return rc;
   }
   return SGPT_OK;
+}
+
+}  // namespace
+
+extern "C" int sgpt_pq_tables_nbits(const float* Q, const float* codebooks, const float* centroids,
+                                    const int32_t* probes, int nq, int D, int m, int nbits, int nlist, int nprobe,
+                                    float* lut_out, float* base_out, sgpt_stream_t stream) {
+  return pq_tables("sgpt_pq_tables_nbits", Q, codebooks, centroids, probes, nq, D, m, nbits, nlist, nprobe, lut_out,
+                   base_out, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int sgpt_pq_tables(const float* Q, const float* codebooks, const float* centroids, const int32_t* probes,
+                              int nq, int D, int m, int nlist, int nprobe, float* lut_out, float* base_out,
+                              sgpt_stream_t stream) {
+  return pq_tables("sgpt_pq_tables", Q, codebooks, centroids, probes, nq, D, m, 8, nlist, nprobe, lut_out, base_out,
+                   static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int64_t sgpt_ivfpq_search_workspace_bytes(int nq, int nlist, int nprobe, int64_t max_list_len, int m) {
+  if (check_pq_sizes("sgpt_ivfpq_search_workspace_bytes", nq, nlist, nprobe, max_list_len, m) != SGPT_OK) return -1;
+  return make_pq_layout(nq, nlist, nprobe, max_list_len).total;
+}
+
+extern "C" int sgpt_ivfpq_search_nbits(const float* lut, const float* base, const uint8_t* codes, int nq, int64_t n,
+                                       int m, int nbits, const int64_t* list_offsets, int nlist, int64_t max_list_len,
+                                       const int32_t* doc_ids, const int32_t* probes, int nprobe, int k,
+                                       const uint32_t* mask, float* out_scores, int64_t* out_ids, void* ws,
+                                       int64_t ws_bytes, sgpt_stream_t stream) {
+  return ivfpq_search("sgpt_ivfpq_search_nbits", lut, base, codes, nq, n, m, nbits, list_offsets, nlist, max_list_len,
+                      doc_ids, probes, nprobe, k, mask, out_scores, out_ids, ws, ws_bytes,
+                      static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int sgpt_ivfpq_search(const float* lut, const float* base, const uint8_t* codes, int nq, int64_t n, int m,
+                                 const int64_t* list_offsets, int nlist, int64_t max_list_len, const int32_t* doc_ids,
+                                 const int32_t* probes, int nprobe, int k, const uint32_t* mask, float* out_scores,
+                                 int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream) {
+  return ivfpq_search("sgpt_ivfpq_search", lut, base, codes, nq, n, m, 8, list_offsets, nlist, max_list_len, doc_ids,
+                      probes, nprobe, k, mask, out_scores, out_ids, ws, ws_bytes, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int64_t sgpt_rerank_workspace_bytes(int nq, int64_t kc) {

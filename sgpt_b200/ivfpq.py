@@ -1,14 +1,17 @@
-"""IVF-PQ index: the IVF lists of ``IVFIndex`` with every document stored as m bytes of product-quantization codes.
+"""IVF-PQ index: the IVF lists of ``IVFIndex`` with every document stored as m product-quantization codes of 8 or 4 bits.
 
-A document costs m bytes of codes plus its int32 id and its int32 position in the id -> position map (m + 8 bytes and a
-deletion bit) instead of its full row: 104 bytes for a 768-dim document at m = 96 against 1536 in bf16.  A query probes
+A document costs m nbits / 8 bytes of codes plus its int32 id and its int32 position in the id -> position map
+(m nbits / 8 + 8 bytes and a deletion bit) instead of its full row: 104 bytes for a 768-dim document at m = 96 with 8-bit
+codes (56 with 4-bit codes) against 1536 in bf16.  With 4-bit codes (``nbits=4``, 16 codewords per subspace) a
+subspace's lookup table is 16 fp32 words, which a warp reads without bank conflicts, and the same bytes hold twice as
+many subspaces.  A query probes
 its ``nprobe`` nearest lists (``IVFIndex.probe``'s rule), and the scan scores every document of those lists from the
 query's lookup tables (include/sgpt_b200.h, IVF-PQ search): m shared-memory lookups per document instead of a D-long dot
 product.  The scores are approximations (asymmetric distance computation, ADC); ``search(..., refine=shard)`` re-ranks
 the PQ pass's best ``k_refine`` documents with their exact scores from a ``CorpusShard`` holding the same documents.
 
 Not supported: ``allow=`` filters, range search, paraphrase mining / community detection over an IVF-PQ index, code
-sizes other than 8 bits, OPQ rotations, fp16 tables and indexes spread over several GPUs.
+sizes other than 4 and 8 bits, OPQ rotations, fp16 tables and indexes spread over several GPUs.
 """
 from __future__ import annotations
 
@@ -24,30 +27,43 @@ from .index import CorpusShard, _bit_slice, _check_score_function, pack_mask, un
 from .ivf import _assign, _kmeans, _merge_lists, _rows_f32
 
 FORMAT = "sgpt_b200.IVFPQIndex/1"
-NBITS = 8
+NBITS = 8                 # the default code width
+_NBITS = (4, 8)           # the supported code widths
 _BATCH_BYTES = 256 << 20  # fp32 rows per encoding batch
-_QUERY_BLOCK = 1024       # queries per table / scan call (the tables take m KB per query)
+_QUERY_BLOCK = 1024       # queries per table / scan call with 8-bit codes (the tables take m KB per query)
 
 
-def _check_pq_shape(D: int, m: int) -> None:
+def _check_pq_shape(D: int, m: int, nbits: int = NBITS) -> None:
+    if nbits not in _NBITS:
+        raise ValueError(f"nbits={nbits} is not supported (only 4- and 8-bit codes are)")
     if D % 8 != 0:
         raise ValueError(f"embedding dimension {D} must be a multiple of 8")
     if m < 16 or m % 16 != 0 or D % m != 0:
         raise ValueError(f"m={m} must be a positive multiple of 16 that divides D={D}")
+    if nbits == 4 and m % 32 != 0:
+        raise ValueError(f"m={m} must be a multiple of 32 for nbits=4")
+
+
+def _pack_codes(codes: torch.Tensor, nbits: int) -> torch.Tensor:
+    """Code rows [T, m] (values < 2^nbits) as stored: uint8 [T, m nbits / 8].  4-bit: byte i = code[2i] | code[2i+1]
+    << 4 (include/sgpt_b200.h)."""
+    if nbits == 8:
+        return codes.to(torch.uint8)
+    return (codes[:, 0::2] | (codes[:, 1::2] << 4)).to(torch.uint8)
 
 
 def _nearest_codewords(r: torch.Tensor, codebooks: torch.Tensor) -> torch.Tensor:
-    """code[i][j] = argmin_c sum_t (r[i, j dsub + t] - B[j][c][t])^2, ties to the lowest c: d = 0, then for t ascending
-    e = r - B, d = d + e * e, every operation one fp32 rounding (no fused multiply-add, no GEMM), so a row's codes do not
-    depend on the rows encoded with it and numpy restates them exactly.  Row blocks of ~64 MB of distances.  int64
-    [T, m]."""
-    m, _, dsub = codebooks.shape
+    """code[i][j] = argmin_c sum_t (r[i, j dsub + t] - B[j][c][t])^2 over the K codewords of codebooks [m, K, dsub],
+    ties to the lowest c: d = 0, then for t ascending e = r - B, d = d + e * e, every operation one fp32 rounding (no
+    fused multiply-add, no GEMM), so a row's codes do not depend on the rows encoded with it and numpy restates them
+    exactly.  Row blocks of ~64 MB of distances.  int64 [T, m]."""
+    m, K, dsub = codebooks.shape
     T = r.shape[0]
-    rows = max(1, (64 << 20) // (4 * 256 * m))
+    rows = max(1, (64 << 20) // (4 * K * m))
     out = torch.empty((T, m), dtype=torch.int64, device=r.device)
     for i in range(0, T, rows):
         x = r[i:i + rows].view(-1, m, dsub)
-        d = torch.zeros((x.shape[0], m, 256), dtype=torch.float32, device=r.device)
+        d = torch.zeros((x.shape[0], m, K), dtype=torch.float32, device=r.device)
         for t in range(dsub):
             diff = x[:, :, t, None] - codebooks[None, :, :, t]
             d += diff * diff
@@ -55,27 +71,28 @@ def _nearest_codewords(r: torch.Tensor, codebooks: torch.Tensor) -> torch.Tensor
     return out
 
 
-def _train_codebooks(r: torch.Tensor, m: int, n_iter: int, g: torch.Generator) -> torch.Tensor:
-    """One 256-centroid k-means per subspace over the training residuals r fp32 [T, D] (device): codebooks fp32
-    [m, 256, dsub].  Starts from r[:256]; the update is the mean of the assigned sub-vectors summed in fp64 on the host in
-    row order, and an empty cell is re-seeded with a sub-vector of a row drawn from `g`."""
+def _train_codebooks(r: torch.Tensor, m: int, n_iter: int, g: torch.Generator, nbits: int = NBITS) -> torch.Tensor:
+    """One K-centroid k-means (K = 2^nbits) per subspace over the training residuals r fp32 [T, D] (device): codebooks
+    fp32 [m, K, dsub].  Starts from r[:K]; the update is the mean of the assigned sub-vectors summed in fp64 on the host
+    in row order, and an empty cell is re-seeded with a sub-vector of a row drawn from `g`."""
     T, D = r.shape
+    K = 1 << nbits
     dsub, dev = D // m, r.device
-    cb = r[:256].view(256, m, dsub).transpose(0, 1).contiguous()
+    cb = r[:K].view(K, m, dsub).transpose(0, 1).contiguous()
     step = max(1, (64 << 20) // (8 * D))  # rows per host transfer of the update
-    cell = torch.arange(m)[None, :] * 256
+    cell = torch.arange(m)[None, :] * K
     for _ in range(int(n_iter)):
         a = _nearest_codewords(r, cb).cpu()
-        sums = torch.zeros(m * 256, dsub, dtype=torch.float64)
+        sums = torch.zeros(m * K, dsub, dtype=torch.float64)
         for i in range(0, T, step):  # index_add_ on the host adds the rows in order: reproducible bits
             sums.index_add_(0, (a[i:i + step] + cell).flatten(), r[i:i + step].cpu().double().view(-1, dsub))
-        counts = torch.bincount((a + cell).flatten(), minlength=m * 256)
-        new = (sums / counts.clamp(min=1)[:, None].double()).view(m, 256, dsub)
+        counts = torch.bincount((a + cell).flatten(), minlength=m * K)
+        new = (sums / counts.clamp(min=1)[:, None].double()).view(m, K, dsub)
         empty = (counts == 0).nonzero().flatten()
         if len(empty):
             rows = r[torch.randint(T, (len(empty),), generator=g).to(dev)].cpu().double().view(-1, m, dsub)
-            j = empty // 256
-            new[j, empty % 256] = rows[torch.arange(len(empty)), j]
+            j = empty // K
+            new[j, empty % K] = rows[torch.arange(len(empty)), j]
         cb = new.float().to(dev)
     return cb
 
@@ -83,9 +100,11 @@ def _train_codebooks(r: torch.Tensor, m: int, n_iter: int, g: torch.Generator) -
 class IVFPQIndex:
     """IVF-PQ index on one GPU.  Made by ``train`` (empty) + ``add``, ``build`` or ``load``.
 
-    ``centroids`` fp32 [nlist, D] (searched as a bf16 shard to choose the probes), ``codebooks`` fp32 [m, 256, D / m],
-    ``codes`` uint8 [n, m] in list order (list l is positions ``offsets[l] .. offsets[l+1]``), ``ids`` int32 [n] the global
-    id of each position, and the deleted positions as a bitmap."""
+    ``centroids`` fp32 [nlist, D] (searched as a bf16 shard to choose the probes), ``codebooks`` fp32 [m, K, D / m]
+    with K = 2^nbits codewords per subspace (``nbits`` 8 or 4, read from the codebooks' shape), ``codes`` uint8
+    [n, m nbits / 8] in list order (list l is positions ``offsets[l] .. offsets[l+1]``; 4-bit codes two per byte, the
+    even subspace in the low nibble), ``ids`` int32 [n] the global id of each position, and the deleted positions as a
+    bitmap."""
 
     def __init__(self, centroids: torch.Tensor, codebooks: torch.Tensor, codes: torch.Tensor, offsets: torch.Tensor,
                  ids: torch.Tensor, deleted: Optional[torch.Tensor], id_base: int, score_function: str, device):
@@ -95,8 +114,11 @@ class IVFPQIndex:
         self.centroids = centroids.to(self.device, torch.float32).contiguous()
         self.codebooks = codebooks.to(self.device, torch.float32).contiguous()
         self.nlist, self.dim = self.centroids.shape
-        self.m = self.codebooks.shape[0]
-        _check_pq_shape(self.dim, self.m)
+        self.m, K = self.codebooks.shape[0], self.codebooks.shape[1]
+        if K not in (1 << b for b in _NBITS):
+            raise ValueError(f"codebooks hold {K} codewords per subspace (16 or 256 are supported)")
+        self.nbits = K.bit_length() - 1
+        _check_pq_shape(self.dim, self.m, self.nbits)
         self._cshard = CorpusShard.from_embeddings(self.centroids, device=self.device)
         self._ws: Optional[torch.Tensor] = None
         self._set_lists(codes, offsets, ids, deleted)
@@ -119,13 +141,14 @@ class IVFPQIndex:
     # ---- construction -------------------------------------------------------------------------------------------
     @classmethod
     def train(cls, sample: torch.Tensor, nlist: int, m: int, score_function: str = "cos_sim", n_iter: int = 10,
-              seed: int = 0, device=None, id_base: int = 0) -> "IVFPQIndex":
+              seed: int = 0, device=None, id_base: int = 0, nbits: int = NBITS) -> "IVFPQIndex":
         """An empty index (n = 0, documents will be numbered from ``id_base``) trained on the fp32/bf16 rows ``sample``
-        [T, D]: T >= 256 and T >= nlist.
+        [T, D]: T >= 2^nbits and T >= nlist.
 
         The rows (normalized for cos_sim) are shuffled with ``seed``; the coarse centroids are ``IVFIndex.build``'s
-        k-means over them, and the codebooks one 256-centroid k-means per subspace over the residuals to each row's
-        centroid (``_train_codebooks``), ``n_iter`` iterations each.  The same inputs and seed give bit-identical centroids
+        k-means over them, and the codebooks one 2^nbits-centroid k-means per subspace over the residuals to each row's
+        centroid (``_train_codebooks``), ``n_iter`` iterations each.  ``nbits``: 8 (256 codewords, m bytes of codes per
+        document) or 4 (16 codewords, m / 2 bytes; m % 32 == 0).  The same inputs and seed give bit-identical centroids
         and codebooks on the same device."""
         _check_score_function(score_function)
         x = torch.as_tensor(sample)
@@ -133,10 +156,11 @@ class IVFPQIndex:
         if x.dim() != 2:
             raise ValueError(f"sample must be [T, D], got {tuple(x.shape)}")
         T, D = x.shape
-        nlist, m = int(nlist), int(m)
-        _check_pq_shape(D, m)
-        if nlist < 1 or T < max(256, nlist):
-            raise ValueError(f"a sample of {T} rows is too small: it needs at least 256 and nlist={nlist} rows")
+        nlist, m, nbits = int(nlist), int(m), int(nbits)
+        _check_pq_shape(D, m, nbits)
+        K = 1 << nbits
+        if nlist < 1 or T < max(K, nlist):
+            raise ValueError(f"a sample of {T} rows is too small: it needs at least {K} and nlist={nlist} rows")
         if id_base < 0:
             raise ValueError("id_base must be >= 0")
         g = torch.Generator().manual_seed(int(seed))
@@ -146,16 +170,17 @@ class IVFPQIndex:
         cent = _kmeans(x, nlist, n_iter, g, score_function)
         lists = _assign(CorpusShard.from_embeddings(cent, device=dev), x, score_function)
         x -= cent[lists]
-        codebooks = _train_codebooks(x, m, n_iter, g)
+        codebooks = _train_codebooks(x, m, n_iter, g, nbits)
         del x
         empty = torch.zeros(nlist + 1, dtype=torch.int64)
-        return cls(cent, codebooks, torch.empty((0, m), dtype=torch.uint8), empty, torch.empty(0, dtype=torch.int32),
-                   None, id_base, score_function, dev)
+        return cls(cent, codebooks, torch.empty((0, m * nbits // 8), dtype=torch.uint8), empty,
+                   torch.empty(0, dtype=torch.int32), None, id_base, score_function, dev)
 
     @classmethod
     def build(cls, source: Union[CorpusShard, torch.Tensor], nlist: int, m: int, score_function: str = "cos_sim",
-              n_iter: int = 10, train_size: Optional[int] = None, seed: int = 0, device=None) -> "IVFPQIndex":
-        """``train`` on ``train_size`` rows of ``source`` (default min(n, max(64 nlist, 256))), drawn as
+              n_iter: int = 10, train_size: Optional[int] = None, seed: int = 0, device=None,
+              nbits: int = NBITS) -> "IVFPQIndex":
+        """``train`` (with ``nbits``) on ``train_size`` rows of ``source`` (default min(n, max(64 nlist, 256))), drawn as
         ``torch.randperm(n, generator=torch.Generator().manual_seed(seed))[:train_size]``, then ``add`` of all its rows in
         batches.  ``source``: a ``CorpusShard`` (its stored rows; an int8 shard's dequantized with their scales, its
         id_base and deletions carry over) or fp32/bf16 embeddings [n, D] (ids from 0)."""
@@ -166,7 +191,7 @@ class IVFPQIndex:
         n, dev = src.n, src.device
         T = min(n, int(train_size) if train_size is not None else max(64 * int(nlist), 256))
         sample = torch.randperm(n, generator=torch.Generator().manual_seed(int(seed)))[:T].to(dev)
-        index = cls.train(_rows_f32(src, sample), nlist, m, score_function, n_iter, seed, dev, src.id_base)
+        index = cls.train(_rows_f32(src, sample), nlist, m, score_function, n_iter, seed, dev, src.id_base, nbits)
         bs = max(1, _BATCH_BYTES // (4 * src.dim))
         for i in range(0, n, bs):
             index.add(_rows_f32(src, torch.arange(i, min(i + bs, n), device=dev)))
@@ -195,17 +220,18 @@ class IVFPQIndex:
         dev, n = self.device, self.n
         bs = max(1, _BATCH_BYTES // (4 * self.dim))
         lists = torch.empty(b, dtype=torch.int64, device=dev)
-        codes = torch.empty((b, self.m), dtype=torch.uint8, device=dev)
+        row_bytes = self.m * self.nbits // 8
+        codes = torch.empty((b, row_bytes), dtype=torch.uint8, device=dev)
         for i in range(0, b, bs):
             x = emb[i:i + bs].to(dev).float()  # (may be a view of emb: nothing below writes into it)
             lists[i:i + bs] = _assign(self._cshard, x, self.score_function)
             if self.score_function == "cos_sim":
                 x = torch.nn.functional.normalize(x, dim=1)
             r = x - self.centroids[lists[i:i + bs]]
-            codes[i:i + bs] = _nearest_codewords(r, self.codebooks).to(torch.uint8)
+            codes[i:i + bs] = _pack_codes(_nearest_codewords(r, self.codebooks), self.nbits)
             del x, r
         offsets, old_dest, new_dest = _merge_lists(self.offsets, lists)
-        all_codes = torch.empty((n + b, self.m), dtype=torch.uint8, device=dev)
+        all_codes = torch.empty((n + b, row_bytes), dtype=torch.uint8, device=dev)
         all_codes.index_copy_(0, old_dest, self.codes)
         all_codes.index_copy_(0, new_dest, codes)
         ids = torch.empty(n + b, dtype=torch.int32, device=dev)
@@ -227,25 +253,25 @@ class IVFPQIndex:
         return self._cshard.search(queries.to(self.device), int(nprobe), self.score_function)[1].to(torch.int32)
 
     def tables(self, queries: torch.Tensor, probes: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
-        """``sgpt_pq_tables`` of fp32/bf16 queries [Q, D] (normalized here for cos_sim) and their probes: (lut fp32
-        [Q, m, 256], base fp32 [Q, nprobe])."""
+        """``sgpt_pq_tables_nbits`` of fp32/bf16 queries [Q, D] (normalized here for cos_sim) and their probes: (lut fp32
+        [Q, m, 2^nbits], base fp32 [Q, nprobe])."""
         q = queries.to(self.device).float()
         if self.score_function == "cos_sim":
             q = torch.nn.functional.normalize(q, dim=1)
         q = q.contiguous()
         nq, nprobe = q.shape[0], probes.shape[1]
-        lut = torch.empty((nq, self.m, 256), dtype=torch.float32, device=self.device)
+        lut = torch.empty((nq, self.m, 1 << self.nbits), dtype=torch.float32, device=self.device)
         base = torch.empty((nq, nprobe), dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
-            rc = _lib.lib().sgpt_pq_tables(q.data_ptr(), self.codebooks.data_ptr(), self.centroids.data_ptr(),
-                                           probes.data_ptr(), nq, self.dim, self.m, self.nlist, nprobe, lut.data_ptr(),
-                                           base.data_ptr(), _lib.current_stream())
-        _lib.check(rc, "sgpt_pq_tables")
+            rc = _lib.lib().sgpt_pq_tables_nbits(q.data_ptr(), self.codebooks.data_ptr(), self.centroids.data_ptr(),
+                                                 probes.data_ptr(), nq, self.dim, self.m, self.nbits, self.nlist, nprobe,
+                                                 lut.data_ptr(), base.data_ptr(), _lib.current_stream())
+        _lib.check(rc, "sgpt_pq_tables_nbits")
         return lut, base
 
     def scan(self, lut: torch.Tensor, base: torch.Tensor, probes: torch.Tensor, k: int
              ) -> Tuple[torch.Tensor, torch.Tensor]:
-        """``sgpt_ivfpq_search`` of prepared tables: the top-k by ADC score of the undeleted probed documents."""
+        """``sgpt_ivfpq_search_nbits`` of prepared tables: the top-k by ADC score of the undeleted probed documents."""
         nq, nprobe = probes.shape
         out_s = torch.full((nq, k), -float("inf"), dtype=torch.float32, device=self.device)
         out_i = torch.full((nq, k), -1, dtype=torch.int64, device=self.device)
@@ -259,11 +285,12 @@ class IVFPQIndex:
             self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
         mask = None if self._deleted is None else torch.bitwise_not(self._deleted).contiguous()
         with torch.cuda.device(self.device):
-            rc = lib.sgpt_ivfpq_search(lut.data_ptr(), base.data_ptr(), self.codes.data_ptr(), nq, self.n, self.m,
-                                       self.offsets.data_ptr(), self.nlist, self.max_list_len, self.ids.data_ptr(),
-                                       probes.data_ptr(), nprobe, k, _lib.ptr(mask), out_s.data_ptr(), out_i.data_ptr(),
-                                       self._ws.data_ptr(), self._ws.numel(), _lib.current_stream())
-        _lib.check(rc, "sgpt_ivfpq_search")
+            rc = lib.sgpt_ivfpq_search_nbits(lut.data_ptr(), base.data_ptr(), self.codes.data_ptr(), nq, self.n,
+                                             self.m, self.nbits, self.offsets.data_ptr(), self.nlist, self.max_list_len,
+                                             self.ids.data_ptr(), probes.data_ptr(), nprobe, k, _lib.ptr(mask),
+                                             out_s.data_ptr(), out_i.data_ptr(), self._ws.data_ptr(), self._ws.numel(),
+                                             _lib.current_stream())
+        _lib.check(rc, "sgpt_ivfpq_search_nbits")
         return out_s, out_i
 
     def search(self, queries: torch.Tensor, k: int, nprobe: int, refine: Optional[CorpusShard] = None,
@@ -288,8 +315,9 @@ class IVFPQIndex:
                                  f"the index's documents (id_base={self.id_base}, n={self.n}, dim={self.dim})")
         queries = queries.to(self.device)
         outs = []
-        for a in range(0, max(queries.shape[0], 1), _QUERY_BLOCK):
-            q = queries[a:a + _QUERY_BLOCK]
+        block = _QUERY_BLOCK * (256 >> self.nbits)  # the same table bytes per call: 16x the queries with 4-bit codes
+        for a in range(0, max(queries.shape[0], 1), block):
+            q = queries[a:a + block]
             probes = self.probe(q, nprobe)
             s, i = self.scan(*self.tables(q, probes), probes, kk)
             outs.append((s, i) if refine is None else rerank(refine, q, i, k, self.score_function))
@@ -315,8 +343,9 @@ class IVFPQIndex:
 
     @property
     def nbytes(self) -> int:
-        """Device bytes of the index: per document m bytes of codes, an int32 id and an int32 position (m + 8) plus the
-        deletion bitmap, and the centroids (fp32 and their bf16 shard), codebooks and offsets."""
+        """Device bytes of the index: per document m nbits / 8 bytes of codes, an int32 id and an int32 position
+        (m nbits / 8 + 8) plus the deletion bitmap, and the centroids (fp32 and their bf16 shard), codebooks and
+        offsets."""
         per_doc = self.codes.numel() + 4 * self.ids.numel() + 4 * self._pos.numel()
         deleted = 0 if self._deleted is None else 4 * self._deleted.numel()
         cs = self._cshard
@@ -326,8 +355,8 @@ class IVFPQIndex:
 
     # ---- persistence --------------------------------------------------------------------------------------------
     def save(self, path: str) -> None:
-        """One directory: centroids.npy (fp32 [nlist, D]), codebooks.npy (fp32 [m, 256, D / m]), codes.npy (uint8
-        [n, m]), offsets.npy (int64 [nlist + 1]), ids.npy (int32 [n]), deleted.npy (uint32 [ceil(n / 32)], bit j set =
+        """One directory: centroids.npy (fp32 [nlist, D]), codebooks.npy (fp32 [m, 2^nbits, D / m]), codes.npy (uint8
+        [n, m nbits / 8]), offsets.npy (int64 [nlist + 1]), ids.npy (int32 [n]), deleted.npy (uint32 [ceil(n / 32)], bit j set =
         position j deleted) and meta.json."""
         os.makedirs(path, exist_ok=True)
         np.save(os.path.join(path, "centroids.npy"), self.centroids.cpu().numpy())
@@ -340,7 +369,7 @@ class IVFPQIndex:
             words = self._deleted[:len(words)].cpu().numpy().view(np.uint32)
         np.save(os.path.join(path, "deleted.npy"), words)
         with open(os.path.join(path, "meta.json"), "w") as f:
-            json.dump({"format": FORMAT, "dim": self.dim, "m": self.m, "nbits": NBITS, "n": self.n, "nlist": self.nlist,
+            json.dump({"format": FORMAT, "dim": self.dim, "m": self.m, "nbits": self.nbits, "n": self.n, "nlist": self.nlist,
                        "id_base": self.id_base, "score_function": self.score_function}, f)
 
     @classmethod
@@ -351,16 +380,17 @@ class IVFPQIndex:
             meta = json.load(f)
         if meta.get("format") != FORMAT:
             raise ValueError(f"{path}: not an IVFPQIndex directory ({meta})")
-        if int(meta.get("nbits", -1)) != NBITS:
-            raise ValueError(f"{path}: nbits={meta.get('nbits')} (only {NBITS}-bit codes are supported)")
+        nbits = meta.get("nbits", -1)
+        if not isinstance(nbits, int) or nbits not in _NBITS:
+            raise ValueError(f"{path}: nbits={nbits} (only 4- and 8-bit codes are supported)")
         n, dim, m = int(meta["n"]), int(meta["dim"]), int(meta["m"])
         nlist, id_base = int(meta["nlist"]), int(meta["id_base"])
         _check_score_function(meta["score_function"])
-        _check_pq_shape(dim, m)
+        _check_pq_shape(dim, m, nbits)
         arrays = {name: np.load(os.path.join(path, name + ".npy"))
                   for name in ("centroids", "codebooks", "codes", "offsets", "ids", "deleted")}
-        want = {"centroids": ((nlist, dim), np.float32), "codebooks": ((m, 256, dim // m), np.float32),
-                "codes": ((n, m), np.uint8), "offsets": ((nlist + 1,), np.int64), "ids": ((n,), np.int32),
+        want = {"centroids": ((nlist, dim), np.float32), "codebooks": ((m, 1 << nbits, dim // m), np.float32),
+                "codes": ((n, m * nbits // 8), np.uint8), "offsets": ((nlist + 1,), np.int64), "ids": ((n,), np.int32),
                 "deleted": (((n + 31) // 32,), np.uint32)}
         if nlist < 1:
             raise ValueError(f"{path}: nlist={nlist} must be positive")
