@@ -242,7 +242,9 @@ int sgpt_model_read_residual(sgpt_model_t m, float* dst, int64_t capacity_elems,
  * S1–S3. Exact dense retrieval over one corpus shard.
  * ------------------------------------------------------------------------------------------------------------------ */
 
-/* inv_norm[i] = 1 / max(||x_i||_2, 1e-12) for bf16 rows (F.normalize semantics, ST/util.py:41-42).  x bf16[n,D]. */
+/* inv_norm[i] = 1 / max(||x_i||_2, 1e-12) for bf16 rows (F.normalize semantics, ST/util.py:41-42).  x bf16[n,D].
+ *     fp32: per-lane sums of squares, a warp tree, then IEEE sqrt and divide.  A row holding a NaN gets 1 / 1e-12 like a
+ *     zero row (the max takes the non-NaN operand); its dot products are NaN regardless, so its scores are -1. */
 int sgpt_row_inv_norms(const void* x, float* inv_norm, int64_t n, int D, sgpt_stream_t stream);
 
 /* fp32 -> bf16 row conversion (round-to-nearest-even) used to store embeddings in a shard. */

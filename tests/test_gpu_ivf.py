@@ -50,6 +50,7 @@ def _probes(nq, nlist, nprobe, g, skipped=True):
 def _ivf(dtype, Q, C, q_scale, c_scale, offsets, ids, probes, k, mask=None):
     L, lib = _lib()
     nq, nprobe = probes.shape
+    D = Q.shape[1]
     nlist = offsets.numel() - 1
     max_len = int((offsets[1:] - offsets[:-1]).max())
     dt = L.DTYPE_I8 if dtype == "int8" else L.DTYPE_BF16
@@ -106,7 +107,7 @@ def _ints(shape, lo, hi, g):
     return torch.randint(lo, hi + 1, shape, generator=g).float()
 
 
-def _data(nq, g, sizes=SIZES):
+def _data(nq, g, sizes=SIZES, D=D):
     offsets, ids = _layout(sizes, int(torch.randint(1 << 30, (1,), generator=g)))
     n = int(offsets[-1])
     return _ints((nq, D), -2, 2, g), _ints((n, D), -2, 2, g), offsets, ids

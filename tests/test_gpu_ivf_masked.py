@@ -11,7 +11,7 @@ import math
 import pytest
 import torch
 
-from tests.test_gpu_ivf import D, SIZES, _data, _equal, _ints, _ivf, _planted, _probed_allow, _probes, _reference
+from tests.test_gpu_ivf import SIZES, _data, _equal, _ints, _ivf, _planted, _probed_allow, _probes, _reference
 
 pytestmark = pytest.mark.gpu
 
@@ -25,6 +25,7 @@ def _lib():
 def _ivf_masked(dtype, Q, C, offsets, ids, probes, k, mask, pitch, q_scale=None, c_scale=None):
     L, lib = _lib()
     nq, nprobe = probes.shape
+    D = Q.shape[1]
     nlist = offsets.numel() - 1
     max_len = int((offsets[1:] - offsets[:-1]).max())
     dt = L.DTYPE_I8 if dtype == "int8" else L.DTYPE_BF16

@@ -33,6 +33,7 @@ def _ivf_range(dtype, Q, C, q_scale, c_scale, offsets, ids, probes, threshold, c
     """(counts, scores, ids) of sgpt_ivf_range_search on sentinel-filled buffers; a second launch must give the same."""
     L, lib = _lib()
     nq, nprobe = probes.shape
+    D = Q.shape[1]
     nlist = offsets.numel() - 1
     max_len = int((offsets[1:] - offsets[:-1]).max())
     dt = L.DTYPE_I8 if dtype == "int8" else L.DTYPE_BF16

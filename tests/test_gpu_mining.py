@@ -44,7 +44,7 @@ def _pow2(m, g):
 
 def device_range(Q, C, threshold, cap, id_base=0, q_scale=None, c_scale=None):
     L, lib = _lib()
-    nq, n = Q.shape[0], C.shape[0]
+    nq, n, D = Q.shape[0], C.shape[0], Q.shape[1]
     Qd, Cd = Q.to(torch.bfloat16).cuda(), C.to(torch.bfloat16).cuda()
     qs = None if q_scale is None else q_scale.cuda()
     cs = None if c_scale is None else c_scale.cuda()

@@ -57,7 +57,7 @@ def _plan(nq, n, k):
 
 def _search(Q, C, k, id_base=0, q_scale=None, c_scale=None, packed=False):
     L, lib = _lib()
-    nq, n = Q.shape[0], C.shape[0]
+    nq, n, D = Q.shape[0], C.shape[0], Q.shape[1]
     ws = torch.empty(lib.sgpt_search_workspace_bytes(nq, n, k), dtype=torch.uint8, device="cuda")
     qs, cs = L.ptr(q_scale), L.ptr(c_scale)
     if packed:
@@ -101,19 +101,30 @@ def _ints(shape, lo, hi, g):
     return torch.randint(lo, hi + 1, shape, generator=g).float()
 
 
-def corpus(kind, nq, n, k, g):
+def planted_weights(D):
+    """(a, b): queries carry a in coordinate 0 and the planted documents are (b, 0, ..., 0), so a planted document scores
+    a * b >= D, strictly above the D - 1 that any other document of the k_sampled / k_unsampled corpora can reach.  Both
+    are exact in bf16 and int8 up to D = 8128: (8, 8) at D <= 64, else a power of two a <= 64 with b = ceil(D / a)."""
+    if D <= 64:
+        return 8, 8
+    a = min(64, 1 << math.ceil(math.log2(D) / 2))
+    return a, -(-D // a)
+
+
+def corpus(kind, nq, n, k, g, D=D):
     """(Q, C) fp32 with small-integer entries (NaN rows for 'nan_rows')."""
     if kind == "random":  # scores in a few hundred values: ties everywhere
         return _ints((nq, D), -2, 2, g), _ints((n, D), -2, 2, g)
     if kind == "identical":  # every document equal: the ids must be id_base .. id_base + k - 1
         return _ints((nq, D), -8, 8, g), _ints((1, D), -8, 8, g).expand(n, D).contiguous()
     if kind in ("k_sampled", "k_unsampled"):
-        # every query: coordinate 0 = 8, the others in {-1, 0, 1}.  Documents: coordinate 0 <= 0, others in {-1, 0, 1}
-        # -> scores <= 63; k special documents (8, 0, ..., 0) score exactly 64, each in its own 4-document block, inside
-        # the sampled tiles (then the admission threshold tau equals the k-th best score: `x >= tau` decides at equality)
-        # or outside them
+        # every query: coordinate 0 = a, the others in {-1, 0, 1}.  Documents: coordinate 0 <= 0, others in {-1, 0, 1}
+        # -> scores <= D - 1; k special documents (b, 0, ..., 0) score exactly a * b >= D (planted_weights), each in its
+        # own 4-document block, inside the sampled tiles (then the admission threshold tau equals the k-th best score:
+        # `x >= tau` decides at equality) or outside them
+        a, b = planted_weights(D)
         Q = _ints((nq, D), -1, 1, g)
-        Q[:, 0] = 8
+        Q[:, 0] = a
         C = _ints((n, D), -1, 1, g)
         C[:, 0] = _ints((n,), -8, 0, g)
         s = _stride(n)
@@ -122,7 +133,7 @@ def corpus(kind, nq, n, k, g):
         assert len(blocks) >= k
         pick = torch.tensor(blocks)[torch.randperm(len(blocks), generator=g)[:k]]
         C[pick] = 0.0
-        C[pick, 0] = 8.0
+        C[pick, 0] = float(b)
         return Q, C
     if kind == "negative":  # every score <= -1: zero-filled columns past n would score 0 and win if not masked
         return _ints((nq, D), 1, 3, g), _ints((n, D), -3, -1, g)

@@ -44,7 +44,7 @@ def _operands(Qf, Cf, dtype):
 def _search(Q, C, k, dtype, words=None, pitch=0, id_base=0, packed=False, masked=True):
     """The masked entry point (masked=False: the unmasked one of the same dtype)."""
     L, lib = _lib()
-    nq, n = Q.shape[0], C.shape[0]
+    nq, n, D = Q.shape[0], C.shape[0], Q.shape[1]
     dt = L.DTYPE_I8 if dtype == "int8" else L.DTYPE_BF16
     ws = torch.empty(lib.sgpt_search_workspace_bytes(nq, n, k), dtype=torch.uint8, device="cuda")
     st = L.current_stream()
@@ -218,7 +218,7 @@ def test_shared_mask_equals_the_same_mask_per_query(plan):
 
 def _range(Q, C, thr, words, pitch, cap, dtype="bf16", id_base=0):
     L, lib = _lib()
-    nq, n = Q.shape[0], C.shape[0]
+    nq, n, D = Q.shape[0], C.shape[0], Q.shape[1]
     dt = L.DTYPE_I8 if dtype == "int8" else L.DTYPE_BF16
     ws = torch.empty(lib.sgpt_range_search_workspace_bytes(nq, n), dtype=torch.uint8, device="cuda")
     counts = torch.full((nq,), -7, dtype=torch.int64, device="cuda")
