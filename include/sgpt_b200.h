@@ -391,6 +391,7 @@ int sgpt_search_gather_i8(sgpt_gather_t g, const void* Q, const void* C, const f
  * ------------------------------------------------------------------------------------------------------------------ */
 #define SGPT_DTYPE_BF16 0
 #define SGPT_DTYPE_I8 1
+#define SGPT_DTYPE_B1 3 /* binary corpus shards (packed sign bits), see below */
 int sgpt_search_masked(int dtype, const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq,
                        int64_t n, int D, int k, int64_t id_base, const uint32_t* mask, int64_t mask_pitch_words,
                        float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
@@ -407,6 +408,45 @@ int sgpt_search_gather_masked(int dtype, sgpt_gather_t g, const void* Q, const v
                               const float* c_scale, int nq, int64_t n, int D, int k, int64_t id_base,
                               const uint32_t* mask, int64_t mask_pitch_words, const int64_t* exclude_ids,
                               float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * Binary corpus shards: every document stored as D sign bits, D / 8 bytes (8x less than int8), searched exactly by a
+ * single-bit wgmma filter GEMM (wgmma .b1.b1.and.popc).  The format of sentence-transformers' quantize_embeddings(...,
+ * precision="ubinary").
+ *   Bits: a row x (fp32, or bf16 widened) becomes b_j = (x_j > t_j), t the fp32 thresholds [D] (NULL: all 0, which is
+ *     ubinary exactly).  The compare is strict (x_j == t_j gives 0) and a NaN gives 0.  Packed in np.packbits order:
+ *     dimension j is bit 7 - (j & 7) of byte j / 8; a row is D / 8 bytes.  popc = the row's number of set bits (int32).
+ *     D % 128 == 0 (rows a multiple of 16 bytes) and D <= 65536.
+ *   Score of query bits q against document bits d: a = popc(q AND d), h = popc(q) + popc(d) - 2 a (the Hamming
+ *     distance), s = D - 2 h = 4 a - 2 popc(d) - 2 popc(q) + D: the dot product of the two +-1 vectors, an integer with
+ *     |s| <= D, exact in fp32.  The device evaluates it as ((float)(4 a + D) - 2 popc(q)) - 2 popc(d), every step exact.
+ *     Every entry point below returns s; cos_sim of the +-1 vectors is s / D (one correctly rounded fp32 division,
+ *     monotone in s), which the caller applies to the scores it receives (sgpt_b200.index.CorpusShard does), and a
+ *     cos_sim threshold t is the threshold s0 = the smallest integer with fl(s0 / D) >= t on s.
+ *   Top-k: the tie rule of every search (score descending, ids ascending); with D + 1 possible scores, ties are common.
+ * sgpt_quantize_rows_b1: x fp32 [n, D] (x_bf16 = 0) or bf16 [n, D] (x_bf16 = 1), 16-byte aligned; thresholds fp32 [D] or
+ *   NULL; bits_out uint8 [n, D / 8] (16-byte aligned) and popc_out int32 [n].  SGPT_ERR_INVALID, before any CUDA call,
+ *   for n < 0, D not a positive multiple of 128 or above 65536, and (n > 0) null or unaligned pointers.
+ * SGPT_DTYPE_B1 in sgpt_search_masked, sgpt_search_packed_masked, sgpt_search_gather_masked and
+ *   sgpt_range_search_masked: Q uint8 [nq, D / 8] and C uint8 [n, D / 8] are bit rows; q_scale and c_scale point at the
+ *   int32 popcounts of the query and document rows (int32 [nq] and int32 [n], passed through the float pointers; NULL is
+ *   rejected when nq > 0).  Q, C and c_scale 16-byte aligned.  Masks, workspaces, output order and every other argument
+ *   as for the other dtypes; the range search's threshold applies to s (a Hamming radius r is the threshold D - 2 r).
+ *   SGPT_ERR_INVALID, before any CUDA call, for D % 128 != 0, D > 65536, null popcounts and unaligned rows, besides the
+ *   other rejections.  The IVF and IVF-PQ entry points reject SGPT_DTYPE_B1.
+ * SGPT_DTYPE_B1 in sgpt_rerank (rescoring bit candidates with the float query): Q fp32 [nq, D] (for cos_sim the caller
+ *   passes F.normalize(q)), C the bit rows [n, D / 8]; c_scale is not read.  The score is the asymmetric
+ *   r = sum_j q_j s_j, s_j = +1 where bit j is set and -1 elsewhere, evaluated in this order: lane l (0..31) takes the
+ *   16-byte bit units l, l + 32, l + 64, ... (128 dimensions each) in ascending order and the 128 dimensions of a unit in
+ *   ascending order, acc_l += (bit ? q_j : -q_j) with one rounding per add; then for o = 16, 8, 4, 2, 1:
+ *   acc_l = acc_l + acc_(l xor o); score = fixnan(acc_0 * q_scale[q]) with q_scale = fp32(1 / sqrt(D)) for cos_sim and
+ *   NULL (= 1) for dot.  Reproducible in numpy bit for bit.  D % 128 == 0 and D <= 65536.
+ *   (sgpt_b200.index.CorpusShard.search(..., rescore=) passes Q = q - t, the query centered on the shard's thresholds
+ *   t, normalized for cos_sim: with zero thresholds that is sentence-transformers' rescoring of q itself; with non-zero
+ *   thresholds it keeps a common offset of the embeddings, which the bits do not encode, out of the score.)
+ * ------------------------------------------------------------------------------------------------------------------ */
+int sgpt_quantize_rows_b1(const void* x, int x_bf16, const float* thresholds, void* bits_out, int32_t* popc_out,
+                          int64_t n, int D, sgpt_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * IVF (inverted-file) search: a corpus split into nlist lists (k-means cells), of which each query scans only the

@@ -110,8 +110,9 @@ _SIGNATURES = {
                                       i64, vp]),
     "sgpt_rerank_workspace_bytes": (i64, [i32, i64]),
     "sgpt_rerank": (i32, [i32, vp, vp, vp, vp, i32, i64, i32, i64, vp, i64, i32, vp, vp, vp, i64, vp]),
+    "sgpt_quantize_rows_b1": (i32, [vp, i32, vp, vp, vp, i64, i32, vp]),
 }
-DTYPE_BF16, DTYPE_I8 = 0, 1
+DTYPE_BF16, DTYPE_I8, DTYPE_B1 = 0, 1, 3
 
 ABI_VERSION = 4  # include/sgpt_b200.h SGPT_ABI_VERSION these signatures / struct layouts were written for
 IPC_HANDLE_BYTES = 64

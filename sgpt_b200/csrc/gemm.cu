@@ -11,12 +11,14 @@
 
 namespace sgpt {
 
-template <int BN, class Epi, int CL = 1, bool kS8 = false>
+// a, b, lda, ldb and K in TMA elements: bf16, int8, or bytes of packed bits (kB1)
+template <int BN, class Epi, int CL = 1, Operand kOp = Operand::kBF16>
 static int launch_gemm(const void* a, int64_t lda, const void* b, int64_t ldb, int M, int N, int K,
                        const typename Epi::Params& ep, cudaStream_t stream, int cat = kCatGemm,
                        TileMap tmap = TileMap()) {
   using Cfg = GemmCfg<BN, Epi::kStagingBytes>;
-  // one 128-byte row segment per box row: 64 bf16 or 128 int8
+  // one 128-byte row segment per box row: 64 bf16, 128 int8 or 1024 bits
+  constexpr bool kS8 = kOp != Operand::kBF16;
   auto make_map = kS8 ? make_tma_2d_u8 : make_tma_2d_bf16;
   const uint32_t box_k = kS8 ? 2 * kGemmBK : kGemmBK;
   CUtensorMap ta, tb;
@@ -25,7 +27,7 @@ static int launch_gemm(const void* a, int64_t lda, const void* b, int64_t ldb, i
   if (rc != SGPT_OK) return rc;
   rc = make_map(&tb, b, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldb), BN, box_k);
   if (rc != SGPT_OK) return rc;
-  auto kern = gemm_bf16_tn_kernel<BN, Epi, CL, kS8>;
+  auto kern = gemm_bf16_tn_kernel<BN, Epi, CL, kOp>;
   static PerDeviceOnce attr_once;
   if (attr_once.first()) {
     SGPT_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
@@ -106,15 +108,12 @@ FilterGeometry filter_geometry(long long tiles, int nq) {
 
 // nq <= 128: one CTA per work unit (M = 128).  128 < nq <= 256: two CTAs per work unit, each with 128 of the queries and
 // the same corpus tile — the second read of the tile is an L2 hit, so one pass over the shard from HBM serves 256 queries.
-template <class Epi>
+template <class Epi, Operand kOp = Operand::kBF16>
 static int launch_filter_gemm(const void* Q, const void* C, int nq, int n, int D, const typename Epi::Params& p,
-                              cudaStream_t stream, TileMap tm, bool s8) {
-  if (s8) {
-    if (nq > kGemmBM) return launch_gemm<kSimBN, Epi, 2, true>(Q, D, C, D, nq, n, D, p, stream, kCatScores, tm);
-    return launch_gemm<kSimBN, Epi, 1, true>(Q, D, C, D, nq, n, D, p, stream, kCatScores, tm);
-  }
-  if (nq > kGemmBM) return launch_gemm<kSimBN, Epi, 2>(Q, D, C, D, nq, n, D, p, stream, kCatScores, tm);
-  return launch_gemm<kSimBN, Epi, 1>(Q, D, C, D, nq, n, D, p, stream, kCatScores, tm);
+                              cudaStream_t stream, TileMap tm) {
+  const int K = kOp == Operand::kB1 ? D / 8 : D;  // TMA elements per row
+  if (nq > kGemmBM) return launch_gemm<kSimBN, Epi, 2, kOp>(Q, K, C, K, nq, n, K, p, stream, kCatScores, tm);
+  return launch_gemm<kSimBN, Epi, 1, kOp>(Q, K, C, K, nq, n, K, p, stream, kCatScores, tm);
 }
 
 int check_doc_mask(const char* fn, long long n, DocMask mask) {
@@ -126,20 +125,64 @@ int check_doc_mask(const char* fn, long long n, DocMask mask) {
   return SGPT_OK;
 }
 
+int shard_operand(const char* fn, int dtype, Operand* op) {
+  SGPT_REQUIRE(dtype == SGPT_DTYPE_BF16 || dtype == SGPT_DTYPE_I8 || dtype == SGPT_DTYPE_B1, "%s: unknown shard dtype %d",
+               fn, dtype);
+  *op = dtype == SGPT_DTYPE_I8 ? Operand::kS8 : dtype == SGPT_DTYPE_B1 ? Operand::kB1 : Operand::kBF16;
+  return SGPT_OK;
+}
+
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+int check_operands(const char* fn, Operand op, const void* Q, const void* C, const float* q_scale, const float* c_scale,
+                   int nq, int D) {
+  switch (op) {
+    case Operand::kS8:
+      SGPT_REQUIRE(D > 0 && D % 16 == 0 && D <= kMaxDimI8, "%s: int8 D=%d must be a positive multiple of 16, at most %d",
+                   fn, D, kMaxDimI8);
+      return SGPT_OK;
+    case Operand::kB1:
+      SGPT_REQUIRE(D > 0 && D % 128 == 0 && D <= kMaxDimB1,
+                   "%s: binary D=%d must be a positive multiple of 128, at most %d", fn, D, kMaxDimB1);
+      if (nq == 0) return SGPT_OK;
+      SGPT_REQUIRE(q_scale != nullptr && c_scale != nullptr, "%s: binary rows need their popcounts (q_scale, c_scale)", fn);
+      SGPT_REQUIRE(aligned16(Q) && aligned16(C) && aligned16(c_scale),
+                   "%s: binary Q, C and the document popcounts must be 16-byte aligned", fn);
+      return SGPT_OK;
+    default:
+      SGPT_REQUIRE(D > 0 && D % 8 == 0, "%s: D=%d must be a positive multiple of 8", fn, D);
+      return SGPT_OK;
+  }
+}
+
+size_t operand_row_bytes(Operand op, int D) {
+  return op == Operand::kS8 ? static_cast<size_t>(D) : op == Operand::kB1 ? static_cast<size_t>(D) / 8 : 2 * static_cast<size_t>(D);
+}
+
 // the masked epilogue only when a mask is given: unmasked searches run the unmasked instantiations
 static int launch_filter_any(const void* Q, const void* C, int nq, int n, int D, const EpiFilterRows::Params& p,
-                             DocMask mask, cudaStream_t stream, TileMap tm, bool s8) {
-  if (mask.bits == nullptr) return launch_filter_gemm<EpiFilterRows>(Q, C, nq, n, D, p, stream, tm, s8);
+                             DocMask mask, cudaStream_t stream, TileMap tm, Operand op) {
   FilterRowsParams pm = p;
   pm.mask = mask.bits;
   pm.mask_pitch = mask.pitch;
-  return launch_filter_gemm<EpiFilterRowsMasked>(Q, C, nq, n, D, pm, stream, tm, s8);
+  const bool masked = mask.bits != nullptr;
+  switch (op) {
+    case Operand::kS8:
+      if (!masked) return launch_filter_gemm<EpiFilterRows, Operand::kS8>(Q, C, nq, n, D, p, stream, tm);
+      return launch_filter_gemm<EpiFilterRowsMasked, Operand::kS8>(Q, C, nq, n, D, pm, stream, tm);
+    case Operand::kB1:
+      if (!masked) return launch_filter_gemm<EpiFilterRowsB1, Operand::kB1>(Q, C, nq, n, D, p, stream, tm);
+      return launch_filter_gemm<EpiFilterRowsB1Masked, Operand::kB1>(Q, C, nq, n, D, pm, stream, tm);
+    default:
+      if (!masked) return launch_filter_gemm<EpiFilterRows>(Q, C, nq, n, D, p, stream, tm);
+      return launch_filter_gemm<EpiFilterRowsMasked>(Q, C, nq, n, D, pm, stream, tm);
+  }
 }
 
 int launch_filter_candidates(const void* Q, const void* C, const float* q_scale, const float* c_scale,
                              const float* tau, const float* tau_hi, uint2* cand, int* counts, int* counts_back,
                              long long stride_q, int L, int group0, int nq, int n, int D, int tile_mode, int tile_stride,
-                             DocMask mask, bool s8, cudaStream_t stream) {
+                             DocMask mask, Operand op, cudaStream_t stream) {
   SGPT_REQUIRE(nq <= 2 * kGemmBM, "filter GEMM: at most %d queries per launch (got %d)", 2 * kGemmBM, nq);
   TileMap tm;
   tm.mode = tile_mode;
@@ -149,11 +192,11 @@ int launch_filter_candidates(const void* Q, const void* C, const float* q_scale,
                g.L);
   FilterRowsParams p{q_scale, c_scale, tau, tau_hi, cand, counts, counts_back, stride_q, L, group0, nq, nullptr, 0, 0,
                      nq > kGemmBM ? 1 : 0};
-  return launch_filter_any(Q, C, nq, n, D, p, mask, stream, tm, s8);
+  return launch_filter_any(Q, C, nq, n, D, p, mask, stream, tm, op);
 }
 
 int launch_sample_maxima(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* pool,
-                         long long stride_p, int Lp, int nq, int n, int D, int tile_stride, DocMask mask, bool s8,
+                         long long stride_p, int Lp, int nq, int n, int D, int tile_stride, DocMask mask, Operand op,
                          cudaStream_t stream) {
   SGPT_REQUIRE(nq <= 2 * kGemmBM, "sample GEMM: at most %d queries per launch (got %d)", 2 * kGemmBM, nq);
   TileMap tm;
@@ -164,19 +207,20 @@ int launch_sample_maxima(const void* Q, const void* C, const float* q_scale, con
                "sample GEMM: maxima lists too small (Lp=%d < %d)", Lp, g.L / 4);
   FilterRowsParams p{q_scale, c_scale, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, 0, nq, pool, stride_p, Lp,
                      nq > kGemmBM ? 1 : 0};
-  return launch_filter_any(Q, C, nq, n, D, p, mask, stream, tm, s8);
+  return launch_filter_any(Q, C, nq, n, D, p, mask, stream, tm, op);
 }
 
 template <class Epi>
 static int launch_ivf_units(const CUtensorMap& ta, const CUtensorMap& tb, int rows, int n, int D,
                             const typename Epi::Params& p, bool s8, cudaStream_t stream) {
   using Cfg = GemmCfg<kSimBN, Epi::kStagingBytes>;
-  auto kern = s8 ? gemm_bf16_tn_kernel<kSimBN, Epi, 1, true, true> : gemm_bf16_tn_kernel<kSimBN, Epi, 1, false, true>;
+  auto kern = s8 ? gemm_bf16_tn_kernel<kSimBN, Epi, 1, Operand::kS8, true>
+                 : gemm_bf16_tn_kernel<kSimBN, Epi, 1, Operand::kBF16, true>;
   static PerDeviceOnce attr_once;
   if (attr_once.first()) {
-    SGPT_CHECK_CUDA(cudaFuncSetAttribute(gemm_bf16_tn_kernel<kSimBN, Epi, 1, true, true>,
+    SGPT_CHECK_CUDA(cudaFuncSetAttribute(gemm_bf16_tn_kernel<kSimBN, Epi, 1, Operand::kS8, true>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    SGPT_CHECK_CUDA(cudaFuncSetAttribute(gemm_bf16_tn_kernel<kSimBN, Epi, 1, false, true>,
+    SGPT_CHECK_CUDA(cudaFuncSetAttribute(gemm_bf16_tn_kernel<kSimBN, Epi, 1, Operand::kBF16, true>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
   }
   // the unit count is only known on the device: one persistent CTA per SM, at most one per possible unit
@@ -209,16 +253,26 @@ int launch_ivf_scan(const void* A, int rows, const void* C, int n, int D, const 
 }
 
 int launch_scores(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* scores, long long lds,
-                  int nq, int n, int D, DocMask mask, bool s8, cudaStream_t stream) {
+                  int nq, int n, int D, DocMask mask, Operand op, cudaStream_t stream) {
   if (nq == 0 || n == 0) return SGPT_OK;
+  constexpr Operand kS8 = Operand::kS8, kB1 = Operand::kB1;
+  if (op == kB1) {  // K in bytes of packed bits
+    const int K = D / 8;
+    if (mask.bits == nullptr) {
+      EpiScoresB1::Params p{scores, q_scale, c_scale, lds, nullptr, 0};
+      return launch_gemm<128, EpiScoresB1, 1, kB1>(Q, K, C, K, nq, n, K, p, stream, kCatScores);
+    }
+    EpiScoresB1Masked::Params p{scores, q_scale, c_scale, lds, mask.bits, mask.pitch};
+    return launch_gemm<128, EpiScoresB1Masked, 1, kB1>(Q, K, C, K, nq, n, K, p, stream, kCatScores);
+  }
   if (mask.bits == nullptr) {
     EpiScoresF32::Params p{scores, q_scale, c_scale, lds, nullptr, 0};
     // lanes = queries (A operand), columns = corpus rows (B operand, streamed once from HBM)
-    if (s8) return launch_gemm<128, EpiScoresF32, 1, true>(Q, D, C, D, nq, n, D, p, stream, kCatScores);
+    if (op == kS8) return launch_gemm<128, EpiScoresF32, 1, kS8>(Q, D, C, D, nq, n, D, p, stream, kCatScores);
     return launch_gemm<128, EpiScoresF32>(Q, D, C, D, nq, n, D, p, stream, kCatScores);
   }
   EpiScoresF32Masked::Params p{scores, q_scale, c_scale, lds, mask.bits, mask.pitch};
-  if (s8) return launch_gemm<128, EpiScoresF32Masked, 1, true>(Q, D, C, D, nq, n, D, p, stream, kCatScores);
+  if (op == kS8) return launch_gemm<128, EpiScoresF32Masked, 1, kS8>(Q, D, C, D, nq, n, D, p, stream, kCatScores);
   return launch_gemm<128, EpiScoresF32Masked>(Q, D, C, D, nq, n, D, p, stream, kCatScores);
 }
 
@@ -313,7 +367,7 @@ extern "C" int sgpt_scores(const void* Q, const void* C, const float* q_scale, c
                (long long)n, D);
   SGPT_REQUIRE(n < (1ll << 31), "sgpt_scores: shard too large for one launch (n=%lld)", (long long)n);
   SGPT_REQUIRE(lds >= n, "sgpt_scores: lds < n");
-  return launch_scores(Q, C, q_scale, c_scale, scores, lds, nq, static_cast<int>(n), D, DocMask(), false, stream);
+  return launch_scores(Q, C, q_scale, c_scale, scores, lds, nq, static_cast<int>(n), D, DocMask(), Operand::kBF16, stream);
 }
 
 extern "C" int sgpt_scores_i8(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* scores,
@@ -325,5 +379,5 @@ extern "C" int sgpt_scores_i8(const void* Q, const void* C, const float* q_scale
   SGPT_REQUIRE(n < (1ll << 31), "sgpt_scores_i8: shard too large for one launch (n=%lld)", (long long)n);
   SGPT_REQUIRE(lds >= n, "sgpt_scores_i8: lds < n");
   SGPT_REQUIRE(nq == 0 || n == 0 || scores != nullptr, "sgpt_scores_i8: null output");
-  return launch_scores(Q, C, q_scale, c_scale, scores, lds, nq, static_cast<int>(n), D, DocMask(), true, stream);
+  return launch_scores(Q, C, q_scale, c_scale, scores, lds, nq, static_cast<int>(n), D, DocMask(), Operand::kS8, stream);
 }

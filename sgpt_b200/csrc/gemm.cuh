@@ -1,5 +1,5 @@
-// Persistent, warp-specialised wgmma GEMM for sm_90a:  C[M,N] = A[M,K] * B[N,K]^T  (bf16 in, fp32 accumulate; int8 in,
-// s32 accumulate for the similarity kernels, see kS8).
+// Persistent, warp-specialised wgmma GEMM for sm_90a:  C[M,N] = A[M,K] * B[N,K]^T  (bf16 in, fp32 accumulate; int8 or
+// single-bit in, s32 accumulate for the similarity kernels, see kOp).
 //
 //   A : activations / queries, row-major [M,K]  -> K-major wgmma operand A
 //   B : nn.Linear weight [out,in] / corpus shard [n,D], row-major [N,K] -> K-major wgmma operand B
@@ -94,10 +94,17 @@ __device__ __forceinline__ void wgmma_mma(int32_t (&d)[BN / 2], uint64_t da, uin
   if constexpr (BN == 128) wgmma_s8_m64n128(d, da, db, scale_d);
   else wgmma_s8_m64n256(d, da, db, scale_d);
 }
+template <int BN>
+__device__ __forceinline__ void wgmma_mma_b1(int32_t (&d)[BN / 2], uint64_t da, uint64_t db, int scale_d) {
+  if constexpr (BN == 128) wgmma_b1_m64n128(d, da, db, scale_d);
+  else wgmma_b1_m64n256(d, da, db, scale_d);
+}
 
 // accumulator element -> the fp32 bits parked in shared memory (an s32 dot product is rounded to nearest: cvt.rn.f32.s32)
 __device__ __forceinline__ uint32_t acc_bits(float x) { return __float_as_uint(x); }
 __device__ __forceinline__ uint32_t acc_bits(int32_t x) { return __float_as_uint(__int2float_rn(x)); }
+// single-bit operands: a = popc(q AND d) -> 4 a + D, an exact fp32 integer (D <= 65536); the epilogue adds the row terms
+__device__ __forceinline__ uint32_t acc_bits_b1(int32_t a, int dims) { return __float_as_uint(__int2float_rn(4 * a + dims)); }
 
 // Optional selection of N-tiles: the similarity search scans a strided sample of corpus tiles first (to establish
 // per-query thresholds) and the remaining tiles afterwards.
@@ -144,20 +151,25 @@ struct TileMap {
 // CL = 2: two CTAs per work unit on the same N-tile and adjacent M-tiles (CTA r of the unit owns rows [128 r, 128 r + 128)
 //   of a 256 x BN tile group): the similarity search scans up to 256 queries per pass over the corpus this way, and both
 //   CTAs of a unit share the candidate-list group of the unit (EpiFilterRows).
-// kS8: int8 operands (int8 corpus shards, similarity epilogues only).  A K-block is then 128 int8 = the same 128 bytes per
-//   row as 64 bf16, so the stage layout, TMA boxes, descriptor steps and ring are unchanged; wgmma k32 accumulates in s32,
-//   exact for |dot| < 2^31, and the accumulator is converted to fp32 where it is parked in shared memory, so every
-//   epilogue runs unchanged.
+// kOp: the operand type (gemm_api.h Operand).  kS8: int8 operands (int8 corpus shards, similarity epilogues only).  A
+//   K-block is then 128 int8 = the same 128 bytes per row as 64 bf16, so the stage layout, TMA boxes, descriptor steps
+//   and ring are unchanged; wgmma k32 accumulates in s32, exact for |dot| < 2^31, and the accumulator is converted to
+//   fp32 where it is parked in shared memory, so every epilogue runs unchanged.
+//   kB1: packed sign bits (binary corpus shards), K counted in bytes (D / 8).  A K-block is again 128 bytes = 1024 bits
+//   per row and a wgmma k256 (.and.popc) takes 32 bytes, the s8 geometry exactly; TMA zero fill of a ragged last k-block
+//   adds no AND bits.  The s32 a = popc(q AND d) is parked as the fp32 integer 4 a + D, and the b1 epilogues
+//   (kB1 of EpiFilterRowsT / OpScoresF32T) add the query and document terms -2 popc(q), -2 popc(d) to it.
 // kUnits: the work units are read from a table in device memory instead of being derived from (M, N) and the TileMap:
 //   unit u is ep.units[u] = (m0, m_end, n0, n_end), one 128 x BN tile at rows m0 / columns n0 whose epilogue sees only
 //   rows < m_end and columns < n_end (passed to it as M and N), and min(*ep.n_units, ep.max_units) units exist.  The
 //   count is read on the device, so the grid is fixed at launch and nothing waits for the host (the grouped IVF scan,
 //   ivf.cu).  CL = 1 and no split-K; M and N bound the tensor maps only.
-template <int BN, class Epi, int CL = 1, bool kS8 = false, bool kUnits = false>
+template <int BN, class Epi, int CL = 1, Operand kOp = Operand::kBF16, bool kUnits = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, int M,
                     int N, int K, const __grid_constant__ typename Epi::Params ep, TileMap tmap) {
   using Cfg = GemmCfg<BN, Epi::kStagingBytes>;
+  constexpr bool kS8 = kOp != Operand::kBF16;      // 1-byte K elements (int8, or 8 packed bits)
   using Acc = typename std::conditional<kS8, int32_t, float>::type;
   constexpr int kBK = kS8 ? 2 * kGemmBK : kGemmBK;  // K elements per k-block (128 bytes per row either way)
   constexpr int kMmaK = kS8 ? 32 : 16;              // K elements per wgmma
@@ -283,7 +295,10 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
         wgmma_fence_acc(acc);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < kBK / kMmaK; ++k) wgmma_mma<BN>(acc, da + 2 * k, db + 2 * k, (kb > kb_begin || k > 0) ? 1 : 0);
+        for (int k = 0; k < kBK / kMmaK; ++k) {
+          if constexpr (kOp == Operand::kB1) wgmma_mma_b1<BN>(acc, da + 2 * k, db + 2 * k, (kb > kb_begin || k > 0) ? 1 : 0);
+          else wgmma_mma<BN>(acc, da + 2 * k, db + 2 * k, (kb > kb_begin || k > 0) ? 1 : 0);
+        }
         wgmma_commit();
         wgmma_fence_acc(acc);
         if constexpr (BN == 128) {
@@ -317,7 +332,11 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
             const uint32_t col = 8 * j + 2 * (t & 3);
             const uint32_t chunk = col >> 2;
             const uint32_t phys = (chunk & ~7u) | ((chunk & 7u) ^ sw);
-            sts_v2(rbase + phys * 16 + (col & 3u) * 4, acc_bits(acc[4 * j + 2 * h]), acc_bits(acc[4 * j + 2 * h + 1]));
+            if constexpr (kOp == Operand::kB1)
+              sts_v2(rbase + phys * 16 + (col & 3u) * 4, acc_bits_b1(acc[4 * j + 2 * h], 8 * K),
+                     acc_bits_b1(acc[4 * j + 2 * h + 1], 8 * K));
+            else
+              sts_v2(rbase + phys * 16 + (col & 3u) * 4, acc_bits(acc[4 * j + 2 * h]), acc_bits(acc[4 * j + 2 * h + 1]));
           }
         }
       }
@@ -700,9 +719,21 @@ __device__ __forceinline__ const uint32_t* mask_row(const uint32_t* mask, long l
 // (topk.cu) treat the document as absent, exactly like an empty slot.
 constexpr uint32_t kMaskedScoreBits = 0xffffffffu;
 
+// Score of a parked accumulator v with the query term r and the document term c.  bf16 / int8 operands: v * r * c (the
+// scales, in this order).  kB1 (binary shards): v = 4 a + D, r = -2 popc(q), c = -2 popc(d) and the score is
+// (v + r) + c = D - 2 hamming(q, d), every step an exact fp32 integer.
+template <bool kB1>
+__device__ __forceinline__ float epi_score(float v, float r, float c) {
+  if constexpr (kB1) return (v + r) + c;
+  else return v * r * c;
+}
+// kB1: the int32 popcount p read through a scale pointer -> the term -2 p
+__device__ __forceinline__ float b1_term(float bits) { return __int2float_rn(-2 * __float_as_int(bits)); }
+
 // scores_f32[q, doc] = fixnan(acc * row_scale[q] * col_scale[doc])       (cos_sim / dot_score, NaN -> -1)
 // kMasked: masked documents get kMaskedScoreBits instead (the dense plan of the masked search).
-template <bool kMasked>
+// kB1: row_scale / col_scale hold int32 popcounts and the score is epi_score<true> (binary shards).
+template <bool kMasked, bool kB1 = false>
 struct OpScoresF32T {
   struct Params {
     float* out;
@@ -720,10 +751,15 @@ struct OpScoresF32T {
       if (ok0) c0 = __ldg(p.col_scale + col);
       if (ok1) c1 = __ldg(p.col_scale + col + 1);
     }
+    if constexpr (kB1) {
+      c0 = b1_term(c0);
+      c1 = b1_term(c1);
+    }
     const bool vec = ok1 && ((p.ldc & 1) == 0);
     float* dst = p.out + static_cast<size_t>(m0) * p.ldc + col;
     float my_rs = 1.f;  // lane r keeps row m0 + r's scale; broadcast per row with a shuffle
     if (p.row_scale && lane < rows) my_rs = __ldg(p.row_scale + m0 + lane);
+    if constexpr (kB1) my_rs = b1_term(my_rs);
     // (col is even: both columns of the lane sit in one mask word)
     const uint32_t shared_word = (kMasked && p.mask_pitch == 0 && ok0) ? __ldg(p.mask + (col >> 5)) : 0u;
     auto masked = [&](int row, float& x, float& y) {
@@ -742,7 +778,7 @@ struct OpScoresF32T {
 #pragma unroll
       for (int u = 0; u < 8; ++u) {
         const float rs = __shfl_sync(0xffffffffu, my_rs, r + u);
-        float x = a[u].x * rs * c0, y = a[u].y * rs * c1;
+        float x = epi_score<kB1>(a[u].x, rs, c0), y = epi_score<kB1>(a[u].y, rs, c1);
         x = (x != x) ? -1.f : x;
         y = (y != y) ? -1.f : y;
         masked(m0 + r + u, x, y);
@@ -757,7 +793,7 @@ struct OpScoresF32T {
     for (; r < rows; ++r) {
       const float rs = __shfl_sync(0xffffffffu, my_rs, r);
       const float2 a = slab_read(slab, r, lane);
-      float x = a.x * rs * c0, y = a.y * rs * c1;
+      float x = epi_score<kB1>(a.x, rs, c0), y = epi_score<kB1>(a.y, rs, c1);
       x = (x != x) ? -1.f : x;
       y = (y != y) ? -1.f : y;
       masked(m0 + r, x, y);
@@ -796,6 +832,10 @@ struct OpScoresF32T {
 // allowed score (-inf, i.e. admit every allowed document, when the sample holds fewer than k maxima).  The four mask
 // words of the warp's half tile are fetched in pre_tile with the document scales.  The unmasked instantiation compiles
 // to the code it had before the mask existed.
+//
+// kB1 (binary shards): row_scale / col_scale hold int32 popcounts; pre_tile turns them into the terms -2 popc of the
+// query and of the tile's documents (b1_term) where it stages the scales, and every score is epi_score<true>.  Masks,
+// thresholds, sample maxima and lists act on that score exactly as on a scaled one.
 struct FilterRowsParams {
   const float* row_scale;  // [M] or null
   const float* col_scale;  // [N] or null
@@ -817,7 +857,7 @@ struct FilterRowsParams {
   long long mask_pitch;    // kMasked: words between consecutive queries' bitmaps (0 = one bitmap for all)
 };
 
-template <bool kMasked>
+template <bool kMasked, bool kB1 = false>
 struct EpiFilterRowsT {
   using Params = FilterRowsParams;
   struct State {
@@ -865,6 +905,10 @@ struct EpiFilterRowsT {
         st.cs.w = __ldg(p.col_scale + min(c + 3, N - 1));
       }
     }
+    if constexpr (kB1) {
+      st.rs = b1_term(st.rs);
+      st.cs = make_float4(b1_term(st.cs.x), b1_term(st.cs.y), b1_term(st.cs.z), b1_term(st.cs.w));
+    }
     if constexpr (kMasked) {
       // Only an L1 prefetch here: four words held in registers across the mainloop would push the 168-register kernel
       // into spills.  tile() loads them from L1 (the 16 bytes may straddle two lines when the pitch is not a multiple of 4)
@@ -897,7 +941,8 @@ struct EpiFilterRowsT {
     const float rs = st.rs;
     const bool pooled = (p.pool != nullptr);
     const float tau = st.tau, tau_hi = st.tau_hi;
-    const bool nan_path = __any_sync(0xffffffffu, !pooled && tau <= -1.0f) != 0;  // warp-uniform
+    // warp-uniform; a b1 score is an integer, never NaN
+    const bool nan_path = !kB1 && __any_sync(0xffffffffu, !pooled && tau <= -1.0f) != 0;
     const float csv[4] = {st.cs.x, st.cs.y, st.cs.z, st.cs.w};
     uint2* dst = p.cand + static_cast<long long>(qok ? q : 0) * p.stride_q + static_cast<long long>(group_of(p)) * p.L;
     int cnt = st.cnt, cnt_b = st.cnt_b;
@@ -927,12 +972,12 @@ struct EpiFilterRowsT {
       if (nan_path) {
 #pragma unroll
         for (int i = 0; i < 32; ++i) {
-          const float s = __uint_as_float(v[i]) * rs * cs[i];
+          const float s = epi_score<kB1>(__uint_as_float(v[i]), rs, cs[i]);
           x[i] = (s != s) ? -1.f : s;
         }
       } else {
 #pragma unroll
-        for (int i = 0; i < 32; ++i) x[i] = __uint_as_float(v[i]) * rs * cs[i];
+        for (int i = 0; i < 32; ++i) x[i] = epi_score<kB1>(__uint_as_float(v[i]), rs, cs[i]);
       }
       if (pooled) {
         // sample pass: maxima of 4 consecutive documents, two 16-byte stores (cnt is a multiple of 8, the lists 32-byte
@@ -986,6 +1031,8 @@ struct EpiFilterRowsT {
 };
 using EpiFilterRows = EpiFilterRowsT<false>;
 using EpiFilterRowsMasked = EpiFilterRowsT<true>;
+using EpiFilterRowsB1 = EpiFilterRowsT<false, true>;
+using EpiFilterRowsB1Masked = EpiFilterRowsT<true, true>;
 
 // Grouped scan of the IVF search (ivf.cu), run with kUnits: A row r is one (query, probe) pair of the query block, all
 // rows of a unit probe the same list, and the unit's columns are one 256-document tile of that list (the unit's M / N
@@ -1139,5 +1186,7 @@ struct EpiDebugNull {
 };
 using EpiScoresF32 = EpiStaged<OpScoresF32T<false>>;
 using EpiScoresF32Masked = EpiStaged<OpScoresF32T<true>>;
+using EpiScoresB1 = EpiStaged<OpScoresF32T<false, true>>;
+using EpiScoresB1Masked = EpiStaged<OpScoresF32T<true, true>>;
 
 }  // namespace sgpt

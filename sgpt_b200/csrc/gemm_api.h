@@ -8,6 +8,12 @@ namespace sgpt {
 constexpr int kSimBN = 256;  // corpus rows per similarity tile (N-tile width of the query x corpus GEMM)
 // int8 operands: at most this many dimensions, so that no s32 dot product can overflow (2^16 x 128 x 128 = 2^30)
 constexpr int kMaxDimI8 = 65536;
+// packed sign bits: at most this many dimensions (the parked 4 a + D <= 5 D stays an exact fp32 integer)
+constexpr int kMaxDimB1 = 65536;
+
+// Operand type of the similarity GEMM (gemm.cuh gemm_bf16_tn_kernel): bf16 rows, int8 rows, or packed sign bits (D / 8
+// bytes per row, include/sgpt_b200.h binary corpus shards).  Functions below take D in dimensions for every type.
+enum class Operand : int { kBF16 = 0, kS8 = 1, kB1 = 2 };
 
 // Geometry of the candidate lists the filter GEMM writes for a launch over `tiles` corpus tiles: every (CTA, column
 // half) is a group with a private list of `L` entries per query (worst case: every score of every visited tile).
@@ -27,28 +33,38 @@ struct DocMask {
 // bitmap (no CUDA call)
 int check_doc_mask(const char* fn, long long n, DocMask mask);
 
+// The `dtype` argument of the masked entry points -> operand type; SGPT_ERR_INVALID with the message set for an unknown
+// dtype (no CUDA call)
+int shard_operand(const char* fn, int dtype, Operand* op);
+// The D rules of the operand type and, for kB1 with nq > 0, non-null popcounts and 16-byte aligned Q, C and document
+// popcounts: SGPT_OK, or SGPT_ERR_INVALID with the message set (no CUDA call)
+int check_operands(const char* fn, Operand op, const void* Q, const void* C, const float* q_scale, const float* c_scale,
+                   int nq, int D);
+// bytes per row of D dimensions
+size_t operand_row_bytes(Operand op, int D);
+
 // Similarity GEMM whose epilogue appends every score >= tau[q] (tau == nullptr: every score) as (score bits, local doc
 // index) to the list cand[q * stride_q + (group0 + g) * L + ...] — scores >= tau_hi[q] at its front, the others at its
 // back (tau_hi == nullptr: all at the front) — and writes counts / counts_back[(group0 + g) * nq + q] for the groups g of
 // this launch (filter_geometry of the visited tile count).  tile_mode/tile_stride select the corpus tiles visited
-// (gemm.cuh TileMap).  nq <= 256 (above 128: CTA pairs, M = 256).  s8: Q and C are int8 rows (gemm.cuh kS8), else bf16.
-// Documents the mask excludes are never admitted.
+// (gemm.cuh TileMap).  nq <= 256 (above 128: CTA pairs, M = 256).  op: the type of the Q and C rows (gemm.cuh; kB1: the
+// scales are the int32 popcounts of the rows).  Documents the mask excludes are never admitted.
 int launch_filter_candidates(const void* Q, const void* C, const float* q_scale, const float* c_scale,
                              const float* tau, const float* tau_hi, uint2* cand, int* counts, int* counts_back,
                              long long stride_q, int L, int group0, int nq, int n, int D, int tile_mode, int tile_stride,
-                             DocMask mask, bool s8, cudaStream_t stream);
+                             DocMask mask, Operand op, cudaStream_t stream);
 
 // The same GEMM over every tile_stride-th corpus tile in sample mode: pool[q * stride_p + g * Lp + ...] receives the
 // maximum score of every 4 consecutive (allowed) documents the group visited (filter_geometry(sampled tiles).L / 4 floats
 // per list, unused slots = 0xffffffff).  Input of launch_tau_select (topk.cuh).
 int launch_sample_maxima(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* pool,
-                         long long stride_p, int Lp, int nq, int n, int D, int tile_stride, DocMask mask, bool s8,
+                         long long stride_p, int Lp, int nq, int n, int D, int tile_stride, DocMask mask, Operand op,
                          cudaStream_t stream);
 
 // Dense scores [nq, lds] (sgpt_scores / sgpt_scores_i8); with a mask, masked documents get score bits 0xffffffff, which
 // the selection kernels treat as absent (topk.cu score_key: invalid key 0).
 int launch_scores(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* scores, long long lds,
-                  int nq, int n, int D, DocMask mask, bool s8, cudaStream_t stream);
+                  int nq, int n, int D, DocMask mask, Operand op, cudaStream_t stream);
 
 // Grouped scan of the IVF search (ivf.cu; gemm.cuh EpiIvfRows): the filter GEMM's mainloop (BN = kSimBN, bf16 or s8)
 // over the work units of p.units, A = rows x D gathered query rows, C = the n x D list-ordered corpus.  Launches

@@ -15,6 +15,7 @@
 // inconsistent inputs give wrong results, never an out-of-bounds access.
 #include "../../include/sgpt_b200.h"
 #include "common.cuh"
+#include "gemm_api.h"
 #include "host_utils.h"
 #include "ivf.cuh"
 #include "topk.cuh"
@@ -333,6 +334,54 @@ __global__ void __launch_bounds__(kThreads) rerank_kernel(const uint8_t* __restr
   if (lane == 0) out[w] = make_uint2(__float_as_uint(x), static_cast<uint32_t>(static_cast<int32_t>(id)));
 }
 
+// Binary shards: Q fp32 [nq, D] rows, C packed sign bits [n, D / 8] (np.packbits order: dimension j at bit 7 - (j & 7) of
+// byte j / 8).  The asymmetric score sum_j q_j s_j, s_j = +1 for a set bit and -1 otherwise, in a fixed order: lane l
+// takes the 16-byte bit units l, l + 32, ... (128 dimensions each) in order and the 128 dimensions of a unit in
+// ascending order, acc += bit ? q : -q (one rounding per add); then the xor butterfly of the bf16 rerank and x q_scale.
+__global__ void __launch_bounds__(kThreads) rerank_b1_kernel(const float* __restrict__ Q, const uint8_t* __restrict__ C,
+                                                             const float* __restrict__ q_scale, int nq, int n, int D,
+                                                             long long id_base, const int64_t* __restrict__ cand, int kc,
+                                                             uint2* __restrict__ out) {
+  pdl_sync();
+  const int lane = threadIdx.x & 31;
+  const long long w = (static_cast<long long>(blockIdx.x) * kThreads + threadIdx.x) >> 5;  // warp-uniform
+  if (w >= static_cast<long long>(nq) * kc) return;
+  const long long q = w / kc;
+  const long long id = __ldg(reinterpret_cast<const long long*>(cand) + w);
+  if (id < 0 || id < id_base || id >= id_base + n) {
+    if (lane == 0) out[w] = make_uint2(__float_as_uint(-INFINITY), 0xffffffffu);
+    return;
+  }
+  const long long row = id - id_base;
+  const float4* qp = reinterpret_cast<const float4*>(Q + q * D);
+  const uint4* cp = reinterpret_cast<const uint4*>(C + row * (D / 8));
+  const int units = D / 128;
+  float acc = 0.f;
+  for (int u = lane; u < units; u += 32) {
+    const uint4 b = __ldg(cp + u);
+    const uint32_t words[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {  // word i: dimensions 128 u + 32 i + t, t = 0 .. 31, at bit 8 (t / 8) + 7 - (t & 7)
+#pragma unroll
+      for (int f = 0; f < 8; ++f) {
+        const float4 v = __ldg(qp + 32 * u + 8 * i + f);
+        const float vs[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int t = 4 * f + e;
+          const bool bit = (words[i] >> (8 * (t >> 3) + 7 - (t & 7))) & 1u;
+          acc += bit ? vs[e] : -vs[e];
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  float x = acc * (q_scale != nullptr ? __ldg(q_scale + q) : 1.f);
+  x = (x != x) ? -1.f : x;
+  if (lane == 0) out[w] = make_uint2(__float_as_uint(x), static_cast<uint32_t>(static_cast<int32_t>(id)));
+}
+
 // ---- argument checks (no CUDA call) ---------------------------------------------------------------------------------
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
@@ -552,10 +601,13 @@ extern "C" int sgpt_rerank(int dtype, const void* Q, const void* C, const float*
                            float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream_) {
   const char* fn = "sgpt_rerank";
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SGPT_REQUIRE(dtype_known(dtype), "%s: unknown shard dtype %d", fn, dtype);
+  SGPT_REQUIRE(dtype_known(dtype) || dtype == SGPT_DTYPE_B1, "%s: unknown shard dtype %d", fn, dtype);
   if (check_rerank_sizes(fn, nq, kc) != SGPT_OK) return SGPT_ERR_INVALID;
-  const bool s8 = dtype == SGPT_DTYPE_I8;
-  if (s8)
+  const bool s8 = dtype == SGPT_DTYPE_I8, b1 = dtype == SGPT_DTYPE_B1;
+  if (b1)
+    SGPT_REQUIRE(D > 0 && D % 128 == 0 && D <= kMaxDimB1, "%s: binary D=%d must be a positive multiple of 128, at most %d",
+                 fn, D, kMaxDimB1);
+  else if (s8)
     SGPT_REQUIRE(D > 0 && D % 16 == 0 && D <= 65536, "%s: int8 D=%d must be a positive multiple of 16, at most %d", fn,
                  D, 65536);
   else
@@ -577,7 +629,11 @@ extern "C" int sgpt_rerank(int dtype, const void* Q, const void* C, const float*
   const dim3 grid(static_cast<unsigned>((warps * 32 + kThreads - 1) / kThreads));
   {
     LaunchScope _ls(kCatScores, stream);
-    if (s8)
+    if (b1)
+      SGPT_CHECK_CUDA(launch_kernel(rerank_b1_kernel, grid, dim3(kThreads), 0, stream, static_cast<const float*>(Q),
+                                    static_cast<const uint8_t*>(C), q_scale, nq, static_cast<int>(n), D,
+                                    static_cast<long long>(id_base), cand_ids, static_cast<int>(kc), packed));
+    else if (s8)
       SGPT_CHECK_CUDA(launch_kernel(rerank_kernel<true>, grid, dim3(kThreads), 0, stream,
                                     static_cast<const uint8_t*>(Q), static_cast<const uint8_t*>(C), q_scale, c_scale, nq,
                                     static_cast<int>(n), D, static_cast<long long>(id_base), cand_ids,

@@ -1,5 +1,6 @@
 // Row quantization for int8 corpus shards and their queries (include/sgpt_b200.h sgpt_quantize_rows_i8): one warp per
 // row, two passes over the row (absolute maximum, then quantize and sum the squares; the second pass hits L1/L2).
+// Sign bits for binary corpus shards (sgpt_quantize_rows_b1): one warp per row, one ballot per 32 dimensions.
 #include "../../include/sgpt_b200.h"
 #include "common.cuh"
 #include "gemm_api.h"
@@ -80,7 +81,67 @@ __global__ void __launch_bounds__(kQuantThreads) quantize_rows_i8_kernel(const v
   }
 }
 
+// Ballot word -> the np.packbits layout of its 32 dimensions.  The ballot has dimension j0 + l at bit l (lane order);
+// np.packbits puts dimension j at bit 7 - (j & 7) of byte j / 8, i.e. byte i of the word holds dimensions j0 + 8 i ..
+// j0 + 8 i + 7 with the first one at its MOST significant bit.  __brev reverses all 32 bits (bit l -> 31 - l), which
+// reverses the bits inside every byte but also the byte order; the byte permutation 0x0123 restores the byte order.
+__device__ __forceinline__ uint32_t packbits_order(uint32_t ballot) { return __byte_perm(__brev(ballot), 0, 0x0123); }
+
+// Row `row`: lane c of the warp holds the word of dimensions base + 32 c .. + 31 for every 1024-dimension step; the word
+// store is then one coalesced 128-byte row segment per step.  popc = the row's number of set bits.
+__global__ void __launch_bounds__(kQuantThreads) quantize_rows_b1_kernel(const void* __restrict__ x, int x_bf16,
+                                                                          const float* __restrict__ thresholds,
+                                                                          uint32_t* __restrict__ bits,
+                                                                          int32_t* __restrict__ popc, long long n, int D) {
+  pdl_sync();
+  const long long row = static_cast<long long>(blockIdx.x) * kQuantRows + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (row >= n) return;  // warp-uniform
+  const long long base = row * D;
+  uint32_t* out = bits + row * (D / 32);
+  int count = 0;
+  for (int j0 = 0; j0 < D; j0 += 1024) {
+    uint32_t mine = 0;
+#pragma unroll 4
+    for (int c = 0; c < 32; ++c) {
+      const int j = j0 + 32 * c + lane;
+      if (j0 + 32 * c >= D) break;  // warp-uniform (D % 128 == 0)
+      const float v = x_bf16 ? bf16_lo(static_cast<uint32_t>(__ldg(static_cast<const uint16_t*>(x) + base + j)))
+                             : __ldg(static_cast<const float*>(x) + base + j);
+      const float t = thresholds != nullptr ? __ldg(thresholds + j) : 0.f;
+      const uint32_t w = __ballot_sync(0xffffffffu, v > t);  // strict; a NaN on either side gives 0
+      if (lane == c) mine = packbits_order(w);
+    }
+    if (j0 + 32 * lane < D) {
+      out[(j0 >> 5) + lane] = mine;
+      count += __popc(mine);
+    }
+  }
+  count = __reduce_add_sync(0xffffffffu, count);
+  if (lane == 0) popc[row] = count;
+}
+
 }  // namespace
+
+extern "C" int sgpt_quantize_rows_b1(const void* x, int x_bf16, const float* thresholds, void* bits_out,
+                                     int32_t* popc_out, int64_t n, int D, sgpt_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  SGPT_REQUIRE(n >= 0, "sgpt_quantize_rows_b1: bad row count n=%lld", (long long)n);
+  SGPT_REQUIRE(D > 0 && D % 128 == 0 && D <= kMaxDimB1,
+               "sgpt_quantize_rows_b1: D=%d must be a positive multiple of 128, at most %d", D, kMaxDimB1);
+  if (n == 0) return SGPT_OK;
+  SGPT_REQUIRE(x != nullptr && bits_out != nullptr && popc_out != nullptr, "sgpt_quantize_rows_b1: null argument");
+  SGPT_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(bits_out) & 15) == 0 &&
+                   (reinterpret_cast<uintptr_t>(popc_out) & 3) == 0 && (reinterpret_cast<uintptr_t>(thresholds) & 3) == 0,
+               "sgpt_quantize_rows_b1: x and bits_out must be 16-byte aligned, popc_out and thresholds 4-byte aligned");
+  const long long blocks = (n + kQuantRows - 1) / kQuantRows;
+  SGPT_REQUIRE(blocks < (1ll << 31), "sgpt_quantize_rows_b1: too many rows");
+  LaunchScope _ls(kCatMisc, stream);
+  SGPT_CHECK_CUDA(launch_kernel(quantize_rows_b1_kernel, dim3(static_cast<unsigned>(blocks)), dim3(kQuantThreads), 0,
+                                stream, x, x_bf16, thresholds, static_cast<uint32_t*>(bits_out), popc_out,
+                                static_cast<long long>(n), D));
+  return SGPT_OK;
+}
 
 extern "C" int sgpt_quantize_rows_i8(const void* x, int x_bf16, void* q_out, float* scale_out, float* cos_scale_out,
                                      int64_t n, int D, sgpt_stream_t stream_) {

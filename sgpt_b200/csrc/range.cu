@@ -193,19 +193,15 @@ extern "C" int64_t sgpt_range_search_workspace_bytes(int nq, int64_t n) {
   return kHeadBytes + b;
 }
 
-// s8: Q and C are int8 rows (gemm.cuh kS8); everything after the filter GEMM is the same.  mask: the filter admits allowed
+// op: the type of the Q and C rows (gemm_api.h Operand); everything after the filter GEMM is the same.  mask: the filter admits allowed
 // documents only, so the lists stay ascending in document index and the run / offset / fill kernels are unchanged.
 static int range_search(const void* Q, const void* Cm, const float* q_scale, const float* c_scale, int nq, int64_t n, int D,
                         float threshold, int64_t id_base, int64_t* out_counts, int64_t cap, float* out_scores,
-                        int64_t* out_ids, void* ws, int64_t ws_bytes, DocMask mask, bool s8, cudaStream_t stream) {
+                        int64_t* out_ids, void* ws, int64_t ws_bytes, DocMask mask, Operand op, cudaStream_t stream) {
   SGPT_REQUIRE(threshold == threshold, "sgpt_range_search: threshold is NaN");
   if (check_doc_mask("sgpt_range_search", n, mask) != SGPT_OK) return SGPT_ERR_INVALID;
-  if (s8)
-    SGPT_REQUIRE(D > 0 && D % 16 == 0 && D <= kMaxDimI8,
-                 "sgpt_range_search: int8 D=%d must be a positive multiple of 16, at most %d", D, kMaxDimI8);
-  else
-    SGPT_REQUIRE(D > 0 && D % 8 == 0, "sgpt_range_search: D=%d must be a positive multiple of 8", D);
-  const size_t row_bytes = static_cast<size_t>(D) * (s8 ? 1 : 2);
+  if (check_operands("sgpt_range_search", op, Q, Cm, q_scale, c_scale, nq, D) != SGPT_OK) return SGPT_ERR_INVALID;
+  const size_t row_bytes = operand_row_bytes(op, D);
   SGPT_REQUIRE(n >= 0 && n < (1ll << 31), "sgpt_range_search: shard size n=%lld outside [0, 2^31)", (long long)n);
   SGPT_REQUIRE(nq >= 0 && cap >= 0, "sgpt_range_search: bad sizes nq=%d cap=%lld", nq, (long long)cap);
   SGPT_REQUIRE(nq == 0 || out_counts != nullptr, "sgpt_range_search: null out_counts");
@@ -247,7 +243,7 @@ static int range_search(const void* Q, const void* Cm, const float* q_scale, con
     if (mb.bits != nullptr) mb.bits += q0 * mb.pitch;
     if (n > 0) {
       int rc = launch_filter_candidates(Qb, Cm, qs, c_scale, tau, nullptr, cand, cnt, nullptr, l.stride_q, l.g.L, 0, nb,
-                                        static_cast<int>(n), D, /*tile_mode=*/0, 1, mb, s8, stream);
+                                        static_cast<int>(n), D, /*tile_mode=*/0, 1, mb, op, stream);
       if (rc != SGPT_OK) return rc;
     }
     LaunchScope _ls(kCatTopk, stream);
@@ -274,7 +270,7 @@ extern "C" int sgpt_range_search(const void* Q, const void* Cm, const float* q_s
                                  float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes,
                                  sgpt_stream_t stream_) {
   return range_search(Q, Cm, q_scale, c_scale, nq, n, D, threshold, id_base, out_counts, cap, out_scores, out_ids, ws,
-                      ws_bytes, DocMask(), false, static_cast<cudaStream_t>(stream_));
+                      ws_bytes, DocMask(), Operand::kBF16, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int sgpt_range_search_i8(const void* Q, const void* Cm, const float* q_scale, const float* c_scale, int nq,
@@ -282,7 +278,7 @@ extern "C" int sgpt_range_search_i8(const void* Q, const void* Cm, const float* 
                                     float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes,
                                     sgpt_stream_t stream_) {
   return range_search(Q, Cm, q_scale, c_scale, nq, n, D, threshold, id_base, out_counts, cap, out_scores, out_ids, ws,
-                      ws_bytes, DocMask(), true, static_cast<cudaStream_t>(stream_));
+                      ws_bytes, DocMask(), Operand::kS8, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int sgpt_range_search_masked(int dtype, const void* Q, const void* Cm, const float* q_scale,
@@ -290,9 +286,8 @@ extern "C" int sgpt_range_search_masked(int dtype, const void* Q, const void* Cm
                                         const uint32_t* mask, int64_t mask_pitch_words, int64_t* out_counts, int64_t cap,
                                         float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes,
                                         sgpt_stream_t stream_) {
-  SGPT_REQUIRE(dtype == SGPT_DTYPE_BF16 || dtype == SGPT_DTYPE_I8, "sgpt_range_search_masked: unknown shard dtype %d",
-               dtype);
+  Operand op;
+  if (shard_operand("sgpt_range_search_masked", dtype, &op) != SGPT_OK) return SGPT_ERR_INVALID;
   return range_search(Q, Cm, q_scale, c_scale, nq, n, D, threshold, id_base, out_counts, cap, out_scores, out_ids, ws,
-                      ws_bytes, DocMask{mask, mask_pitch_words}, dtype == SGPT_DTYPE_I8,
-                      static_cast<cudaStream_t>(stream_));
+                      ws_bytes, DocMask{mask, mask_pitch_words}, op, static_cast<cudaStream_t>(stream_));
 }

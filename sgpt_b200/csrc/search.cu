@@ -98,21 +98,17 @@ extern "C" int64_t sgpt_search_workspace_bytes(int nq, int64_t n, int k) {
 }
 
 // One shard, all query blocks.  `fin` carries the packed destinations of the final selection (TopkExtra::dst/flag:
-// this rank's buffer and/or peer gather buffers); out_scores / out_ids may be null when only those are wanted.  s8: Q and
-// C are int8 rows (the plan, thresholds, candidate lists and selection do not depend on the operand type).  mask: the
-// allowed documents (bits == nullptr: all); the plan and the workspace do not depend on it.
+// this rank's buffer and/or peer gather buffers); out_scores / out_ids may be null when only those are wanted.  op: the
+// type of the Q and C rows, bf16, int8 or packed bits (the plan, thresholds, candidate lists and selection do not depend
+// on it).  mask: the allowed documents (bits == nullptr: all); the plan and the workspace do not depend on it.
 static int search_impl(const void* Q, const void* Cm, const float* q_scale, const float* c_scale, int nq, int64_t n, int D,
                        int k, int64_t id_base, float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes,
-                       const TopkExtra& fin, DocMask mask, bool s8, cudaStream_t stream) {
+                       const TopkExtra& fin, DocMask mask, Operand op, cudaStream_t stream) {
   SGPT_REQUIRE(nq >= 0 && n >= 0 && k > 0, "sgpt_search: bad sizes nq=%d n=%lld k=%d", nq, (long long)n, k);
   SGPT_REQUIRE(n < (1ll << 31), "sgpt_search: shard too large for one launch (n=%lld)", (long long)n);
   if (check_doc_mask("sgpt_search", n, mask) != SGPT_OK) return SGPT_ERR_INVALID;
-  if (s8)
-    SGPT_REQUIRE(D > 0 && D % 16 == 0 && D <= kMaxDimI8, "sgpt_search: int8 D=%d must be a positive multiple of 16, at most %d",
-                 D, kMaxDimI8);
-  else
-    SGPT_REQUIRE(D > 0 && D % 8 == 0, "sgpt_search: D=%d must be a positive multiple of 8", D);
-  const size_t row_bytes = static_cast<size_t>(D) * (s8 ? 1 : 2);
+  if (check_operands("sgpt_search", op, Q, Cm, q_scale, c_scale, nq, D) != SGPT_OK) return SGPT_ERR_INVALID;
+  const size_t row_bytes = operand_row_bytes(op, D);
   SGPT_REQUIRE(ws != nullptr && ws_bytes >= sgpt_search_workspace_bytes(nq, n, k),
                "sgpt_search: workspace too small (%lld < %lld bytes)", (long long)ws_bytes,
                (long long)sgpt_search_workspace_bytes(nq, n, k));
@@ -130,7 +126,7 @@ static int search_impl(const void* Q, const void* Cm, const float* q_scale, cons
       int rc = search_impl(static_cast<const uint8_t*>(Q) + static_cast<size_t>(q0) * row_bytes, Cm,
                            q_scale ? q_scale + q0 : nullptr, c_scale, nb, n, D, k, id_base,
                            out_scores ? out_scores + static_cast<size_t>(q0) * k : nullptr,
-                           out_ids ? out_ids + static_cast<size_t>(q0) * k : nullptr, ws, ws_bytes, f, m, s8, stream);
+                           out_ids ? out_ids + static_cast<size_t>(q0) * k : nullptr, ws, ws_bytes, f, m, op, stream);
       if (rc != SGPT_OK) return rc;
     }
     return SGPT_OK;
@@ -139,7 +135,7 @@ static int search_impl(const void* Q, const void* Cm, const float* q_scale, cons
   if (!p.two_pass) {
     float* scores = static_cast<float*>(ws);
     const int64_t lds = padded_cols(n);
-    int rc = launch_scores(Q, Cm, q_scale, c_scale, scores, lds, nq, static_cast<int>(n), D, mask, s8, stream);
+    int rc = launch_scores(Q, Cm, q_scale, c_scale, scores, lds, nq, static_cast<int>(n), D, mask, op, stream);
     if (rc != SGPT_OK) return rc;
     TopkSrc src{};
     src.scores = scores;
@@ -169,13 +165,13 @@ static int search_impl(const void* Q, const void* Cm, const float* q_scale, cons
 
   // pass A: block maxima of the sampled tiles -> admission thresholds
   int rc = launch_sample_maxima(Q, Cm, q_scale, c_scale, pool, p.stride_p, p.Lp, nq, static_cast<int>(n), D, p.stride, mask,
-                                s8, stream);
+                                op, stream);
   if (rc != SGPT_OK) return rc;
   rc = launch_tau_select(pool, p.stride_p, static_cast<int>(p.stride_p), nq, k, p.k_hi, tau, tau_hi, stream);
   if (rc != SGPT_OK) return rc;
   // pass B: the whole shard, admission threshold tau[q], front / back split at tau_hi[q]
   rc = launch_filter_candidates(Q, Cm, q_scale, c_scale, tau, tau_hi, cand, cnt, cnt_back, p.stride_b, p.gb.L, 0, nq,
-                                static_cast<int>(n), D, /*tile_mode=*/0, 1, mask, s8, stream);
+                                static_cast<int>(n), D, /*tile_mode=*/0, 1, mask, op, stream);
   if (rc != SGPT_OK) return rc;
   // final exact selection over the candidates
   TopkSrc src{};
@@ -198,15 +194,15 @@ static int search_impl(const void* Q, const void* Cm, const float* q_scale, cons
 
 static int search_unpacked(const void* Q, const void* Cm, const float* q_scale, const float* c_scale, int nq, int64_t n,
                            int D, int k, int64_t id_base, float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes,
-                           DocMask mask, bool s8, cudaStream_t stream) {
+                           DocMask mask, Operand op, cudaStream_t stream) {
   SGPT_REQUIRE(nq == 0 || (out_scores != nullptr && out_ids != nullptr), "sgpt_search: null output");
   return search_impl(Q, Cm, q_scale, c_scale, nq, n, D, k, id_base, out_scores, out_ids, ws, ws_bytes, TopkExtra(), mask,
-                     s8, stream);
+                     op, stream);
 }
 
 static int search_packed(const void* Q, const void* Cm, const float* q_scale, const float* c_scale, int nq, int64_t n,
                          int D, int k, int64_t id_base, uint64_t* out_packed, void* ws, int64_t ws_bytes, DocMask mask,
-                         bool s8, cudaStream_t stream) {
+                         Operand op, cudaStream_t stream) {
   SGPT_REQUIRE(nq == 0 || out_packed != nullptr, "sgpt_search_packed: null output");
   SGPT_REQUIRE(id_base >= 0 && id_base + n < (1ll << 31), "sgpt_search_packed: global ids must fit 31 bits (id_base=%lld n=%lld)",
                (long long)id_base, (long long)n);
@@ -215,51 +211,44 @@ static int search_packed(const void* Q, const void* Cm, const float* q_scale, co
   fin.n_dst = 1;
   fin.dst_slot = 0;
   fin.dst_nq = nq;
-  return search_impl(Q, Cm, q_scale, c_scale, nq, n, D, k, id_base, nullptr, nullptr, ws, ws_bytes, fin, mask, s8, stream);
-}
-
-// dtype argument of the masked entry points -> int8 operands?
-static int shard_dtype_s8(const char* fn, int dtype, bool* s8) {
-  SGPT_REQUIRE(dtype == SGPT_DTYPE_BF16 || dtype == SGPT_DTYPE_I8, "%s: unknown shard dtype %d", fn, dtype);
-  *s8 = dtype == SGPT_DTYPE_I8;
-  return SGPT_OK;
+  return search_impl(Q, Cm, q_scale, c_scale, nq, n, D, k, id_base, nullptr, nullptr, ws, ws_bytes, fin, mask, op, stream);
 }
 
 extern "C" int sgpt_search(const void* Q, const void* Cm, const float* q_scale, const float* c_scale, int nq,
                            int64_t n, int D, int k, int64_t id_base, float* out_scores, int64_t* out_ids, void* ws,
                            int64_t ws_bytes, sgpt_stream_t stream_) {
   return search_unpacked(Q, Cm, q_scale, c_scale, nq, n, D, k, id_base, out_scores, out_ids, ws, ws_bytes, DocMask(),
-                         false, static_cast<cudaStream_t>(stream_));
+                         Operand::kBF16, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int sgpt_search_i8(const void* Q, const void* Cm, const float* q_scale, const float* c_scale, int nq,
                               int64_t n, int D, int k, int64_t id_base, float* out_scores, int64_t* out_ids, void* ws,
                               int64_t ws_bytes, sgpt_stream_t stream_) {
   return search_unpacked(Q, Cm, q_scale, c_scale, nq, n, D, k, id_base, out_scores, out_ids, ws, ws_bytes, DocMask(),
-                         true, static_cast<cudaStream_t>(stream_));
+                         Operand::kS8, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int sgpt_search_masked(int dtype, const void* Q, const void* Cm, const float* q_scale, const float* c_scale,
                                   int nq, int64_t n, int D, int k, int64_t id_base, const uint32_t* mask,
                                   int64_t mask_pitch_words, float* out_scores, int64_t* out_ids, void* ws,
                                   int64_t ws_bytes, sgpt_stream_t stream_) {
-  bool s8 = false;
-  if (shard_dtype_s8("sgpt_search_masked", dtype, &s8) != SGPT_OK) return SGPT_ERR_INVALID;
+  Operand op;
+  if (shard_operand("sgpt_search_masked", dtype, &op) != SGPT_OK) return SGPT_ERR_INVALID;
   return search_unpacked(Q, Cm, q_scale, c_scale, nq, n, D, k, id_base, out_scores, out_ids, ws, ws_bytes,
-                         DocMask{mask, mask_pitch_words}, s8, static_cast<cudaStream_t>(stream_));
+                         DocMask{mask, mask_pitch_words}, op, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int sgpt_search_packed(const void* Q, const void* Cm, const float* q_scale, const float* c_scale, int nq,
                                   int64_t n, int D, int k, int64_t id_base, uint64_t* out_packed, void* ws,
                                   int64_t ws_bytes, sgpt_stream_t stream_) {
-  return search_packed(Q, Cm, q_scale, c_scale, nq, n, D, k, id_base, out_packed, ws, ws_bytes, DocMask(), false,
+  return search_packed(Q, Cm, q_scale, c_scale, nq, n, D, k, id_base, out_packed, ws, ws_bytes, DocMask(), Operand::kBF16,
                        static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int sgpt_search_packed_i8(const void* Q, const void* Cm, const float* q_scale, const float* c_scale, int nq,
                                      int64_t n, int D, int k, int64_t id_base, uint64_t* out_packed, void* ws,
                                      int64_t ws_bytes, sgpt_stream_t stream_) {
-  return search_packed(Q, Cm, q_scale, c_scale, nq, n, D, k, id_base, out_packed, ws, ws_bytes, DocMask(), true,
+  return search_packed(Q, Cm, q_scale, c_scale, nq, n, D, k, id_base, out_packed, ws, ws_bytes, DocMask(), Operand::kS8,
                        static_cast<cudaStream_t>(stream_));
 }
 
@@ -267,10 +256,10 @@ extern "C" int sgpt_search_packed_masked(int dtype, const void* Q, const void* C
                                          const float* c_scale, int nq, int64_t n, int D, int k, int64_t id_base,
                                          const uint32_t* mask, int64_t mask_pitch_words, uint64_t* out_packed, void* ws,
                                          int64_t ws_bytes, sgpt_stream_t stream_) {
-  bool s8 = false;
-  if (shard_dtype_s8("sgpt_search_packed_masked", dtype, &s8) != SGPT_OK) return SGPT_ERR_INVALID;
+  Operand op;
+  if (shard_operand("sgpt_search_packed_masked", dtype, &op) != SGPT_OK) return SGPT_ERR_INVALID;
   return search_packed(Q, Cm, q_scale, c_scale, nq, n, D, k, id_base, out_packed, ws, ws_bytes,
-                       DocMask{mask, mask_pitch_words}, s8, static_cast<cudaStream_t>(stream_));
+                       DocMask{mask, mask_pitch_words}, op, static_cast<cudaStream_t>(stream_));
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -350,7 +339,7 @@ extern "C" void sgpt_gather_destroy(sgpt_gather_t g) {
 
 static int search_gather(sgpt_gather_t g, const void* Q, const void* Cm, const float* q_scale, const float* c_scale, int nq,
                          int64_t n, int D, int k, int64_t id_base, const int64_t* exclude_ids, float* out_scores,
-                         int64_t* out_ids, void* ws, int64_t ws_bytes, DocMask mask, bool s8, cudaStream_t stream) {
+                         int64_t* out_ids, void* ws, int64_t ws_bytes, DocMask mask, Operand op, cudaStream_t stream) {
   SGPT_REQUIRE(g != nullptr, "sgpt_search_gather: null gather context");
   if (check_doc_mask("sgpt_search_gather", n, mask) != SGPT_OK) return SGPT_ERR_INVALID;
   SGPT_REQUIRE(nq >= 0 && nq <= g->nq_cap && k == g->k, "sgpt_search_gather: nq=%d k=%d do not fit the context (nq<=%d, k=%d)",
@@ -371,7 +360,7 @@ static int search_gather(sgpt_gather_t g, const void* Q, const void* Cm, const f
     fin.dst[r] = reinterpret_cast<uint2*>(g->peers[r] + static_cast<size_t>(par) * g->parity_bytes);
     fin.flag[r] = reinterpret_cast<unsigned int*>(g->peers[r] + flag_off);
   }
-  int rc = search_impl(Q, Cm, q_scale, c_scale, nq, n, D, k, id_base, nullptr, nullptr, ws, ws_bytes, fin, mask, s8,
+  int rc = search_impl(Q, Cm, q_scale, c_scale, nq, n, D, k, id_base, nullptr, nullptr, ws, ws_bytes, fin, mask, op,
                        stream);
   // the counters of this parity are consumed whether or not the merge below is launched
   g->uses[par] += 1;
@@ -397,7 +386,7 @@ extern "C" int sgpt_search_gather(sgpt_gather_t g, const void* Q, const void* Cm
                                   const int64_t* exclude_ids, float* out_scores, int64_t* out_ids, void* ws,
                                   int64_t ws_bytes, sgpt_stream_t stream_) {
   return search_gather(g, Q, Cm, q_scale, c_scale, nq, n, D, k, id_base, exclude_ids, out_scores, out_ids, ws, ws_bytes,
-                       DocMask(), false, static_cast<cudaStream_t>(stream_));
+                       DocMask(), Operand::kBF16, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int sgpt_search_gather_i8(sgpt_gather_t g, const void* Q, const void* Cm, const float* q_scale,
@@ -405,7 +394,7 @@ extern "C" int sgpt_search_gather_i8(sgpt_gather_t g, const void* Q, const void*
                                      const int64_t* exclude_ids, float* out_scores, int64_t* out_ids, void* ws,
                                      int64_t ws_bytes, sgpt_stream_t stream_) {
   return search_gather(g, Q, Cm, q_scale, c_scale, nq, n, D, k, id_base, exclude_ids, out_scores, out_ids, ws, ws_bytes,
-                       DocMask(), true, static_cast<cudaStream_t>(stream_));
+                       DocMask(), Operand::kS8, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int sgpt_search_gather_masked(int dtype, sgpt_gather_t g, const void* Q, const void* Cm, const float* q_scale,
@@ -413,10 +402,10 @@ extern "C" int sgpt_search_gather_masked(int dtype, sgpt_gather_t g, const void*
                                          const uint32_t* mask, int64_t mask_pitch_words, const int64_t* exclude_ids,
                                          float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes,
                                          sgpt_stream_t stream_) {
-  bool s8 = false;
-  if (shard_dtype_s8("sgpt_search_gather_masked", dtype, &s8) != SGPT_OK) return SGPT_ERR_INVALID;
+  Operand op;
+  if (shard_operand("sgpt_search_gather_masked", dtype, &op) != SGPT_OK) return SGPT_ERR_INVALID;
   return search_gather(g, Q, Cm, q_scale, c_scale, nq, n, D, k, id_base, exclude_ids, out_scores, out_ids, ws, ws_bytes,
-                       DocMask{mask, mask_pitch_words}, s8, static_cast<cudaStream_t>(stream_));
+                       DocMask{mask, mask_pitch_words}, op, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int sgpt_topk_merge_packed(const uint64_t* in_packed, int G, int nq, int k, float* out_scores,

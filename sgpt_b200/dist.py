@@ -131,6 +131,8 @@ class ShardedDenseRetrievalExactSearch:
     def __init__(self, model, batch_size: int = 128, corpus_chunk_size: int = 50000, group=None,
                  shard_factory: Optional[Callable] = None, merge: Optional[Callable] = None, peer_gather: bool = False,
                  shard_dtype: str = "bf16", **kwargs):
+        if shard_dtype == "binary":
+            raise ValueError("shard_dtype 'binary' is not supported by the sharded exact search: use bf16 or int8")
         self.model, self.batch_size, self.corpus_chunk_size = model, batch_size, corpus_chunk_size
         self.group, self.shard_factory, self.merge = group, shard_factory, merge
         self.shard_dtype = shard_dtype

@@ -12,10 +12,16 @@ Every search takes an optional document filter ``allow=`` (a boolean device tens
 with one row per query), and ``CorpusShard.remove`` deletes documents from a built shard.  Both become one document
 bitmap per search (``pack_mask``; include/sgpt_b200.h, masked searches): the result is exactly the search over the
 allowed, undeleted documents.
+
+A binary shard (``dtype="binary"``) holds the sign bits of every document, D / 8 bytes (sentence-transformers'
+``quantize_embeddings(..., precision="ubinary")``), searched exactly by their integer scores: s = D - 2 hamming for
+"dot", s / D for "cos_sim" (include/sgpt_b200.h, binary corpus shards).  ``search(..., rescore=kc)`` rescores the best kc
+by the float query, ``refine=shard`` with the exact scores of a bf16 / int8 shard of the same documents.
 """
 from __future__ import annotations
 
 import json
+import math
 import os
 from typing import Dict, List, Optional, Tuple, Union
 
@@ -25,7 +31,7 @@ import torch
 from . import _lib
 
 SCORE_FUNCTIONS = ("cos_sim", "dot")
-SHARD_DTYPES = ("bf16", "int8")
+SHARD_DTYPES = ("bf16", "int8", "binary")
 
 
 def _check_score_function(score_function: str) -> None:
@@ -69,6 +75,69 @@ def quantize_rows_i8(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch
                                                     scale.data_ptr(), cos_scale.data_ptr(), n, D, _lib.current_stream()),
                    "sgpt_quantize_rows_i8")
     return q, scale, cos_scale
+
+
+def quantize_rows_b1(x: torch.Tensor, thresholds: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """fp32 or bf16 [n, D] (device) -> (sign bits uint8 [n, D / 8] in np.packbits order, popcounts int32 [n]) with the
+    library's quantizer: bit j is x_j > thresholds[j] (None: 0), strict, NaN -> 0."""
+    if x.dtype != torch.bfloat16:
+        x = x.float()
+    x = x.contiguous()
+    n, D = x.shape
+    bits = torch.empty((n, D // 8), dtype=torch.uint8, device=x.device)
+    popc = torch.empty(n, dtype=torch.int32, device=x.device)
+    t = None if thresholds is None else thresholds.to(x.device, torch.float32).contiguous()
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.lib().sgpt_quantize_rows_b1(x.data_ptr(), int(x.dtype == torch.bfloat16), _lib.ptr(t),
+                                                    bits.data_ptr(), popc.data_ptr(), n, D, _lib.current_stream()),
+                   "sgpt_quantize_rows_b1")
+    return bits, popc
+
+
+def binary_thresholds(sample: torch.Tensor) -> torch.Tensor:
+    """Per-dimension thresholds of a binary shard from a sample of embeddings [m, D]: the lower median of every
+    dimension, fp32 [D].  Mean-pooled GPT embeddings are anisotropic (a large common offset), so with zero thresholds
+    some bits may hardly vary; median thresholds split every dimension of the sample in half."""
+    sample = torch.as_tensor(sample)
+    if sample.dim() != 2 or sample.shape[0] == 0:
+        raise ValueError(f"binary_thresholds needs a sample [m, D] with m >= 1, got {tuple(sample.shape)}")
+    return sample.float().median(dim=0).values.contiguous()  # torch.median: the lower of the two middle values
+
+
+_POPC8 = [bin(i).count("1") for i in range(256)]
+
+
+def _popcounts(bits: torch.Tensor) -> torch.Tensor:
+    """Number of set bits of every packed row, uint8 [n, B] -> int32 [n] (loading stored bits)."""
+    lut = torch.tensor(_POPC8, dtype=torch.int32, device=bits.device)
+    out = torch.empty(bits.shape[0], dtype=torch.int32, device=bits.device)
+    step = max(1, (16 << 20) // max(1, bits.shape[1]))
+    for i in range(0, bits.shape[0], step):
+        out[i:i + step] = lut[bits[i:i + step].long()].sum(1, dtype=torch.int32)
+    return out
+
+
+def _b1_cos(scores: torch.Tensor, dim: int) -> torch.Tensor:
+    """cos_sim of the +-1 vectors from the sign dot products s: s / D, one correctly rounded fp32 division per score
+    (a tensor divisor: torch turns division by a Python scalar into a multiplication by its reciprocal)."""
+    return scores / torch.full((), float(dim), dtype=torch.float32, device=scores.device)
+
+
+def _b1_threshold(threshold: float, score_function: str, dim: int) -> float:
+    """A range-search threshold on the shard's scores -> the threshold on s: for cos_sim the smallest integer s0 with
+    fl(s0 / D) >= threshold (fl(s / D) is monotone in s), D + 1 when no s qualifies.  -inf admits every document
+    (-D), +inf none (D + 1); NaN is passed on for the library to reject."""
+    if score_function != "cos_sim" or math.isnan(threshold):
+        return float(threshold)
+    if math.isinf(threshold):
+        return float(-dim if threshold < 0 else dim + 1)
+    t, d = np.float32(threshold), np.float32(dim)
+    s0 = min(max(math.ceil(float(threshold) * dim), -dim), dim + 1)
+    while s0 > -dim and np.float32(s0 - 1) / d >= t:
+        s0 -= 1
+    while s0 <= dim and np.float32(s0) / d < t:
+        s0 += 1
+    return float(s0)
 
 
 def row_inv_norms(x_bf16: torch.Tensor) -> torch.Tensor:
@@ -152,6 +221,11 @@ def _grown_range(nq: int, device, run, capacity: Optional[int] = None
 def _check_dtype(dtype: str, dim: int) -> None:
     if dtype not in SHARD_DTYPES:
         raise ValueError(f"shard dtype {dtype!r} must be one of {SHARD_DTYPES}")
+    if dtype == "binary":
+        if dim % 128 != 0 or not 0 < dim <= 65536:
+            raise ValueError(f"binary shards need a positive embedding dimension that is a multiple of 128, at most "
+                             f"65536 (got {dim})")
+        return
     if dim % (16 if dtype == "int8" else 8) != 0:
         raise ValueError(f"embedding dimension must be a multiple of {16 if dtype == 'int8' else 8} for {dtype} shards")
     if dtype == "int8" and dim > 65536:
@@ -162,17 +236,30 @@ class CorpusShard:
     """Documents [id_base, id_base + n) of a corpus, resident in the HBM of one GPU.
 
     ``dtype="bf16"``: ``vectors`` bf16 [capacity, D] and ``inv_norms`` fp32.  ``dtype="int8"``: ``vectors`` int8
-    [capacity, D], ``scales`` and ``cos_scales`` fp32 (include/sgpt_b200.h, int8 corpus shards).
+    [capacity, D], ``scales`` and ``cos_scales`` fp32 (include/sgpt_b200.h, int8 corpus shards).  ``dtype="binary"``:
+    ``vectors`` uint8 [capacity, D / 8] (sign bits in np.packbits order), ``popcounts`` int32 and the ``thresholds``
+    fp32 [D] that documents and queries are quantized with (``thresholds=None``: zeros, ST's "ubinary"; see
+    ``binary_thresholds``).
 
     Deleted documents (``remove``) are bits of a device bitmap int32 [capacity / 32 + 1] that the shard and its views
     share (``_deleted``: the words and whether any bit was ever set; ``_deleted_at``: the bit of this shard's row 0).
     Every search leaves them out; ids never change."""
 
-    def __init__(self, dim: int, capacity: int, device="cuda:0", id_base: int = 0, dtype: str = "bf16"):
+    def __init__(self, dim: int, capacity: int, device="cuda:0", id_base: int = 0, dtype: str = "bf16",
+                 thresholds: Optional[torch.Tensor] = None):
         _check_dtype(dtype, dim)
+        if thresholds is not None and dtype != "binary":
+            raise ValueError(f"thresholds apply to binary shards only (dtype {dtype!r})")
         self.dim, self.capacity, self.id_base, self.dtype = int(dim), int(capacity), int(id_base), dtype
         self.device = torch.device(device)
-        if dtype == "int8":
+        if dtype == "binary":
+            t = torch.zeros(self.dim) if thresholds is None else torch.as_tensor(thresholds)
+            if t.shape != (self.dim,):
+                raise ValueError(f"thresholds must be [{self.dim}], got {tuple(t.shape)}")
+            self.thresholds = t.to(self.device, torch.float32).contiguous()
+            self.vectors = torch.empty((self.capacity, self.dim // 8), dtype=torch.uint8, device=self.device)
+            self.popcounts = torch.empty(self.capacity, dtype=torch.int32, device=self.device)
+        elif dtype == "int8":
             self.vectors = torch.empty((self.capacity, self.dim), dtype=torch.int8, device=self.device)
             self.scales = torch.empty(self.capacity, dtype=torch.float32, device=self.device)
             self.cos_scales = torch.empty(self.capacity, dtype=torch.float32, device=self.device)
@@ -186,10 +273,28 @@ class CorpusShard:
         self._deleted_at = 0
 
     @classmethod
-    def from_embeddings(cls, emb: torch.Tensor, device=None, id_base: int = 0, dtype: str = "bf16") -> "CorpusShard":
+    def from_embeddings(cls, emb: torch.Tensor, device=None, id_base: int = 0, dtype: str = "bf16",
+                        thresholds: Optional[torch.Tensor] = None) -> "CorpusShard":
         device = device or emb.device
-        shard = cls(emb.shape[1], emb.shape[0], device=device, id_base=id_base, dtype=dtype)
+        shard = cls(emb.shape[1], emb.shape[0], device=device, id_base=id_base, dtype=dtype, thresholds=thresholds)
         shard.add(emb)
+        return shard
+
+    @classmethod
+    def from_packed_bits(cls, bits, device="cuda:0", id_base: int = 0, thresholds: Optional[torch.Tensor] = None,
+                         capacity: Optional[int] = None) -> "CorpusShard":
+        """A binary shard of sign bits as stored by sentence-transformers' ``quantize_embeddings(...,
+        precision="ubinary")`` (``np.packbits(x > 0, axis=-1)``): uint8 [n, D / 8], numpy or torch, taken as they are.
+        ``thresholds`` [D] are those the queries are quantized with (None: zeros, what "ubinary" used)."""
+        b = torch.as_tensor(np.ascontiguousarray(bits) if isinstance(bits, np.ndarray) else bits)
+        if b.dim() != 2 or b.dtype != torch.uint8:
+            raise ValueError(f"packed bits must be uint8 [n, D / 8], got {b.dtype} {tuple(b.shape)}")
+        n = b.shape[0]
+        shard = cls(8 * b.shape[1], max(n, capacity or n), device=device, id_base=id_base, dtype="binary",
+                    thresholds=thresholds)
+        shard.vectors[:n].copy_(b)
+        shard.popcounts[:n].copy_(_popcounts(shard.vectors[:n]))
+        shard.n = n
         return shard
 
     def add(self, emb: torch.Tensor) -> None:
@@ -198,6 +303,12 @@ class CorpusShard:
         if self.n + m > self.capacity:
             raise ValueError(f"shard capacity {self.capacity} exceeded ({self.n} + {m})")
         emb = emb.to(self.device)
+        if self.dtype == "binary":
+            bits, popc = quantize_rows_b1(emb, self.thresholds)
+            self.vectors[self.n:self.n + m].copy_(bits)
+            self.popcounts[self.n:self.n + m].copy_(popc)
+            self.n += m
+            return
         if self.dtype == "int8":
             q, scale, cos_scale = quantize_rows_i8(emb)
             self.vectors[self.n:self.n + m].copy_(q)
@@ -217,9 +328,13 @@ class CorpusShard:
     def save(self, path: str) -> None:
         """Write the shard as ``path/{vectors.npy, <scales>, meta.json}``; one directory per rank for a sharded corpus.
         bf16: vectors.npy holds the bf16 bit patterns as uint16, inv_norms.npy the fp32 1/||row||.  int8: vectors.npy
-        holds the int8 rows, scales.npy fp32 [n, 2] the (scale, cos_scale) of every row."""
+        holds the int8 rows, scales.npy fp32 [n, 2] the (scale, cos_scale) of every row.  binary: vectors.npy holds the
+        bits uint8 [n, D / 8], thresholds.npy fp32 [D]; the popcounts are recomputed at load."""
         os.makedirs(path, exist_ok=True)
-        if self.dtype == "int8":
+        if self.dtype == "binary":
+            np.save(os.path.join(path, "vectors.npy"), self.stored().cpu().numpy())
+            np.save(os.path.join(path, "thresholds.npy"), self.thresholds.cpu().numpy())
+        elif self.dtype == "int8":
             np.save(os.path.join(path, "vectors.npy"), self.stored().cpu().numpy())
             np.save(os.path.join(path, "scales.npy"),
                     torch.stack([self.scales[:self.n], self.cos_scales[:self.n]], 1).cpu().numpy())
@@ -247,7 +362,12 @@ class CorpusShard:
             raise ValueError(f"{path}: unknown shard dtype {dtype!r} (expected one of {SHARD_DTYPES})")
         n, dim = int(meta["n"]), int(meta["dim"])
         vec = np.load(os.path.join(path, "vectors.npy"), mmap_mode="r")
-        if dtype == "int8":
+        if dtype == "binary":
+            thr = np.load(os.path.join(path, "thresholds.npy"))
+            if (dim % 128 != 0 or vec.shape != (n, dim // 8) or vec.dtype != np.uint8 or thr.shape != (dim,)
+                    or thr.dtype != np.float32):
+                raise ValueError(f"{path}: array shapes {vec.shape}/{thr.shape} do not match meta {meta}")
+        elif dtype == "int8":
             sc = np.load(os.path.join(path, "scales.npy"))
             if vec.shape != (n, dim) or vec.dtype != np.int8 or sc.shape != (n, 2) or sc.dtype != np.float32:
                 raise ValueError(f"{path}: array shapes {vec.shape}/{sc.shape} do not match meta {meta}")
@@ -261,8 +381,12 @@ class CorpusShard:
             if deleted.shape != ((n + 31) // 32,) or deleted.dtype != np.uint32:
                 raise ValueError(f"{path}: deletion bitmap {deleted.shape}/{deleted.dtype} does not match meta {meta} "
                                  f"(expected uint32 [{(n + 31) // 32}])")
-        shard = cls(dim, max(n, capacity or n), device=device, id_base=int(meta["id_base"]), dtype=dtype)
-        if dtype == "int8":
+        shard = cls(dim, max(n, capacity or n), device=device, id_base=int(meta["id_base"]), dtype=dtype,
+                    thresholds=torch.from_numpy(thr) if dtype == "binary" else None)
+        if dtype == "binary":
+            shard.vectors[:n].copy_(torch.from_numpy(np.array(vec)))
+            shard.popcounts[:n].copy_(_popcounts(shard.vectors[:n]))
+        elif dtype == "int8":
             shard.vectors[:n].copy_(torch.from_numpy(np.array(vec)))
             shard.scales[:n].copy_(torch.from_numpy(np.ascontiguousarray(sc[:, 0])))
             shard.cos_scales[:n].copy_(torch.from_numpy(np.ascontiguousarray(sc[:, 1])))
@@ -315,15 +439,19 @@ class CorpusShard:
 
     def _dtype_id(self) -> int:
         """The `dtype` argument of the masked entry points for this shard's format."""
-        return _lib.DTYPE_I8 if self.dtype == "int8" else _lib.DTYPE_BF16
+        return {"int8": _lib.DTYPE_I8, "binary": _lib.DTYPE_B1}.get(self.dtype, _lib.DTYPE_BF16)
 
     def _queries(self, queries: torch.Tensor, score_function: str):
         """Queries -> rows in the shard's format + their scales + the shard's scale pointer.  bf16: bf16 rows, 1/||q||
         of the rounded rows for cos_sim and no scales (None) for dot.  int8: quantized rows, cos_scale (cos_sim) or scale
-        (dot) of queries and documents."""
+        (dot) of queries and documents.  binary: the query bits (the shard's thresholds) and the popcounts of queries and
+        documents, for either score function (cos_sim divides the scores afterwards, ``_b1_cos``)."""
         _check_score_function(score_function)
         q = queries.to(self.device)
         cos = score_function == "cos_sim"
+        if self.dtype == "binary":
+            bits, popc = quantize_rows_b1(q, self.thresholds)
+            return bits, popc, self.popcounts.data_ptr()
         if self.dtype == "int8":
             q8, scale, cos_scale = quantize_rows_i8(q)
             return q8, (cos_scale if cos else scale), (self.cos_scales if cos else self.scales).data_ptr()
@@ -343,7 +471,8 @@ class CorpusShard:
         return qb, q_scale, c_scale
 
     def search(self, queries: torch.Tensor, k: int, score_function: str = "cos_sim",
-               allow: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+               allow: Optional[torch.Tensor] = None, rescore: Optional[int] = None,
+               refine: Optional["CorpusShard"] = None) -> Tuple[torch.Tensor, torch.Tensor]:
         """Exact top-k of this shard for fp32/bf16 queries [Q, D] (device).
 
         Returns (scores fp32 [Q,k] descending, global ids int64 [Q,k]); when the shard has fewer than k documents the
@@ -354,7 +483,17 @@ class CorpusShard:
         ``allow``: boolean device tensor [n] (all queries) or [Q, n] (one row per query) of the documents that may be
         returned; deleted documents (``remove``) never are.  The result is exactly the search over those documents, with
         the tail (-inf, -1) when fewer than k are allowed.
+
+        Binary shards: the queries are quantized with the shard's thresholds and the scores are the sign dot products s
+        (dot) or s / D (cos_sim), exact integers / quotients with many ties (broken by ascending id).  ``rescore=kc``
+        (k <= kc <= 4096) takes the best kc documents by s and returns their top-k by the asymmetric score of the float
+        query against the +-1 documents (``rerank_binary``; cos_sim: F.normalize(q - t) . s / sqrt(D), t the shard's
+        thresholds).  ``refine=shard``: a
+        bf16 or int8 shard holding the same documents (same id_base, n and dim) whose exact scores rank the kc candidates
+        instead, kc = ``rescore`` or min(4096, 10 k).  Both are ValueErrors on bf16 and int8 shards.
         """
+        if rescore is not None or refine is not None:
+            return self._rescored(queries, k, score_function, allow, rescore, refine)
         qb, q_scale, c_scale = self._prepare(queries, k, score_function)
         nq = qb.shape[0]
         mask, pitch = self._mask(allow, nq)
@@ -366,6 +505,63 @@ class CorpusShard:
                                                _lib.ptr(mask), pitch, out_s.data_ptr(), out_i.data_ptr(),
                                                self._ws.data_ptr(), self._ws.numel(), _lib.current_stream())
         _lib.check(rc, "sgpt_search")
+        if self.dtype == "binary" and score_function == "cos_sim":
+            out_s = _b1_cos(out_s, self.dim)
+        return out_s, out_i
+
+    def _rescored(self, queries: torch.Tensor, k: int, score_function: str, allow, rescore: Optional[int],
+                  refine: Optional["CorpusShard"]) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``search(..., rescore=, refine=)`` of a binary shard: kc candidates by s, then their top-k rescored."""
+        if self.dtype != "binary":
+            raise ValueError(f"rescore= and refine= apply to binary shards only (this shard is {self.dtype!r})")
+        _check_score_function(score_function)
+        kc = int(rescore) if rescore is not None else min(4096, 10 * int(k))
+        if not int(k) <= kc <= 4096:
+            raise ValueError(f"rescore={kc} must lie in [k={k}, 4096]")
+        if refine is not None:
+            if not isinstance(refine, CorpusShard) or refine.dtype not in ("bf16", "int8"):
+                raise ValueError("refine must be a bf16 or int8 CorpusShard")
+            if (refine.id_base, refine.n, refine.dim) != (self.id_base, self.n, self.dim):
+                raise ValueError(f"refine shard (id_base={refine.id_base}, n={refine.n}, dim={refine.dim}) does not hold "
+                                 f"this shard's documents (id_base={self.id_base}, n={self.n}, dim={self.dim})")
+        _, cand = self.search(queries, kc, "dot", allow=allow)
+        if refine is not None:
+            from .ivfpq import rerank
+            return rerank(refine, queries, cand, k, score_function)
+        return self.rerank_binary(queries, cand, k, score_function)
+
+    def rerank_binary(self, queries: torch.Tensor, cand_ids: torch.Tensor, k: int, score_function: str = "cos_sim"
+                      ) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Top-k of the candidates (global ids int64 [Q, kc], < 0 = empty, distinct per query) of a binary shard by the
+        asymmetric score of the float queries against the +-1 documents: ``sgpt_rerank`` with SGPT_DTYPE_B1 of the
+        query q - t centered on the shard's thresholds t (zero thresholds: q itself, sentence-transformers' rescoring),
+        in fp32, F.normalize'd and scaled by fp32(1 / sqrt(D)) for cos_sim.  The centering keeps the query's component
+        along a common offset (what median thresholds remove from the bits) out of the score.  Deletions are not
+        consulted."""
+        if self.dtype != "binary":
+            raise ValueError(f"rerank_binary needs a binary shard (this shard is {self.dtype!r})")
+        _check_score_function(score_function)
+        q = queries.to(self.device).float() - self.thresholds
+        q_scale = None
+        if score_function == "cos_sim":
+            q = torch.nn.functional.normalize(q, dim=1)
+            q_scale = torch.full((q.shape[0],), float(np.float32(1.0 / math.sqrt(self.dim))), dtype=torch.float32,
+                                 device=self.device)
+        q = q.contiguous()
+        cand = cand_ids.to(self.device, torch.int64).contiguous()
+        nq, kc = cand.shape
+        lib = _lib.lib()
+        need = lib.sgpt_rerank_workspace_bytes(nq, kc)
+        if need < 0:
+            raise ValueError(f"sgpt_rerank rejects these arguments: {lib.sgpt_last_error().decode()}")
+        ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+        out_s = torch.empty((nq, k), dtype=torch.float32, device=self.device)
+        out_i = torch.empty((nq, k), dtype=torch.int64, device=self.device)
+        with torch.cuda.device(self.device):
+            rc = lib.sgpt_rerank(_lib.DTYPE_B1, q.data_ptr(), self.vectors.data_ptr(), _lib.ptr(q_scale), None, nq,
+                                 self.n, self.dim, self.id_base, cand.data_ptr(), kc, int(k), out_s.data_ptr(),
+                                 out_i.data_ptr(), ws.data_ptr(), ws.numel(), _lib.current_stream())
+        _lib.check(rc, "sgpt_rerank")
         return out_s, out_i
 
     def search_packed(self, queries: torch.Tensor, k: int, score_function: str = "cos_sim",
@@ -383,6 +579,9 @@ class CorpusShard:
                                                       _lib.ptr(mask), pitch, out.data_ptr(), self._ws.data_ptr(),
                                                       self._ws.numel(), _lib.current_stream())
         _lib.check(rc, "sgpt_search_packed")
+        if self.dtype == "binary" and score_function == "cos_sim":
+            halves = out.view(torch.int32).view(nq, k, 2)
+            halves[..., 0] = _b1_cos(halves[..., 0].contiguous().view(torch.float32), self.dim).view(torch.int32)
         return out
 
     def search_gather(self, gather_handle, queries: torch.Tensor, k: int, score_function: str = "cos_sim",
@@ -403,6 +602,8 @@ class CorpusShard:
                                                       _lib.ptr(exclude_ids), out_s.data_ptr(), out_i.data_ptr(),
                                                       self._ws.data_ptr(), self._ws.numel(), _lib.current_stream())
         _lib.check(rc, "sgpt_search_gather")
+        if self.dtype == "binary" and score_function == "cos_sim":
+            out_s = _b1_cos(out_s, self.dim)
         return out_s, out_i
 
     def view(self, start: int, end: int) -> "CorpusShard":
@@ -412,7 +613,10 @@ class CorpusShard:
         v = object.__new__(CorpusShard)
         v.dim, v.capacity, v.id_base, v.device, v.dtype = self.dim, end - start, int(start), self.device, self.dtype
         v.vectors = self.vectors[start:end]
-        if self.dtype == "int8":
+        if self.dtype == "binary":
+            v.popcounts = self.popcounts[start:end].clone()
+            v.thresholds = self.thresholds
+        elif self.dtype == "int8":
             v.scales = self.scales[start:end].clone()
             v.cos_scales = self.cos_scales[start:end].clone()
         else:
@@ -453,9 +657,15 @@ class CorpusShard:
         Returns (offsets int64 [Q+1], scores fp32 [E], global ids int64 [E]) on the device: query q's documents are
         entries offsets[q] .. offsets[q+1], in ascending id order.  Queries are converted and scored exactly as in
         ``search``; a NaN score counts as -1.  The output buffer starts at 64 entries per query and grows once, for the
-        queries that did not fit.  ``allow`` as in ``search``: only allowed, undeleted documents are counted and returned."""
+        queries that did not fit.  ``allow`` as in ``search``: only allowed, undeleted documents are counted and returned.
+        On a binary shard the scores are those of ``search`` (s, or s / D for cos_sim), so a "dot" threshold D - 2 r is
+        the Hamming ball of radius r."""
         qb, q_scale, c_scale = self._queries(queries, score_function)
-        return self._range(qb, q_scale, c_scale, threshold, mask=self._mask(allow, qb.shape[0]))
+        if self.dtype != "binary":
+            return self._range(qb, q_scale, c_scale, threshold, mask=self._mask(allow, qb.shape[0]))
+        offsets, scores, ids = self._range(qb, q_scale, c_scale, _b1_threshold(threshold, score_function, self.dim),
+                                           mask=self._mask(allow, qb.shape[0]))
+        return offsets, (_b1_cos(scores, self.dim) if score_function == "cos_sim" else scores), ids
 
 
 def unpack_topk(packed: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -508,6 +718,8 @@ def semantic_search(query_embeddings: torch.Tensor, corpus_embeddings: Union[tor
         q = q.unsqueeze(0)  # ST/util.py:214-217
     shard = corpus_embeddings if isinstance(corpus_embeddings, CorpusShard) else CorpusShard.from_embeddings(
         torch.as_tensor(corpus_embeddings).to(device))
+    if shard.dtype == "binary":
+        raise ValueError("semantic_search does not take binary shards (dtype 'binary'): use CorpusShard.search")
     k = min(int(top_k), shard.n)
     scores, ids = shard.search(q.to(shard.device), k, score_function)
     scores, ids = scores.cpu().tolist(), ids.cpu().tolist()

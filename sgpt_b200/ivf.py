@@ -111,6 +111,8 @@ class IVFIndex:
     def __init__(self, shard: CorpusShard, centroids: torch.Tensor, offsets: torch.Tensor, ids: torch.Tensor,
                  id_base: int, score_function: str):
         _check_score_function(score_function)
+        if shard.dtype == "binary":
+            raise ValueError("IVF indexes do not take binary shards (dtype 'binary'): use bf16 or int8")
         self.score_function, self.id_base = score_function, int(id_base)
         self.device = shard.device
         self.centroids = centroids.to(self.device, torch.float32).contiguous()
@@ -149,6 +151,8 @@ class IVFIndex:
         Peak device memory: the source plus the index (rows, scales, int32 ids, centroids), plus one batch of dequantized
         rows and its centroid scores (~256 MB) during the assignment."""
         _check_score_function(score_function)
+        if (source.dtype if isinstance(source, CorpusShard) else dtype) == "binary":
+            raise ValueError("IVF indexes do not take binary shards (dtype 'binary'): use bf16 or int8")
         if isinstance(source, CorpusShard):
             if dtype is not None and dtype != source.dtype:
                 raise ValueError(f"dtype {dtype!r} differs from the source shard's {source.dtype!r}")

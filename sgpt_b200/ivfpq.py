@@ -185,6 +185,8 @@ class IVFPQIndex:
         batches.  ``source``: a ``CorpusShard`` (its stored rows; an int8 shard's dequantized with their scales, its
         id_base and deletions carry over) or fp32/bf16 embeddings [n, D] (ids from 0)."""
         if isinstance(source, CorpusShard):
+            if source.dtype == "binary":
+                raise ValueError("IVF-PQ indexes are not built from binary shards (dtype 'binary'): use bf16 or int8")
             src = source
         else:
             src = CorpusShard.from_embeddings(torch.as_tensor(source).float(), device=device)
@@ -310,6 +312,9 @@ class IVFPQIndex:
             kk = min(4096, 10 * k) if k_refine is None else int(k_refine)
             if not k <= kk <= 4096:
                 raise ValueError(f"k_refine={kk} must lie in [k={k}, 4096]")
+            if refine.dtype == "binary":
+                raise ValueError("refine must be a bf16 or int8 shard: a binary shard (dtype 'binary') holds no exact "
+                                 "scores")
             if (refine.id_base, refine.n, refine.dim) != (self.id_base, self.n, self.dim):
                 raise ValueError(f"refine shard (id_base={refine.id_base}, n={refine.n}, dim={refine.dim}) does not hold "
                                  f"the index's documents (id_base={self.id_base}, n={self.n}, dim={self.dim})")
@@ -419,7 +424,11 @@ def rerank(shard: CorpusShard, queries: torch.Tensor, cand_ids: torch.Tensor, k:
            ) -> Tuple[torch.Tensor, torch.Tensor]:
     """``sgpt_rerank``: the top-k of the exact scores of each query's candidates (global ids int64 [Q, kc]; ids < 0 or
     outside the shard are empty slots, a query's ids must be distinct) in ``shard``, with ``shard.search``'s query
-    conversion, score bits and tie rule; tail (-inf, -1).  The shard's deletions are not consulted."""
+    conversion, score bits and tie rule; tail (-inf, -1).  The shard's deletions are not consulted.  bf16 and int8
+    shards only: a binary shard's candidates are rescored with the float query by ``CorpusShard.rerank_binary``."""
+    if shard.dtype == "binary":
+        raise ValueError("rerank takes bf16 or int8 shards; a binary shard (dtype 'binary') is rescored with "
+                         "CorpusShard.rerank_binary")
     qb, q_scale, c_scale = shard._queries(queries, score_function)
     cand = cand_ids.to(shard.device, torch.int64).contiguous()
     nq, kc = cand.shape

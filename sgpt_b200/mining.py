@@ -29,6 +29,8 @@ _COUNT_ROWS = 1 << 16           # stored rows per count-only IVF range pass of c
 def _as_shard(embeddings: Union[torch.Tensor, CorpusShard]) -> CorpusShard:
     """The embeddings as a shard whose ids are row positions 0 .. N-1."""
     if isinstance(embeddings, CorpusShard):
+        if embeddings.dtype == "binary":
+            raise ValueError("mining does not take binary shards (dtype 'binary'): use bf16 or int8")
         if embeddings.n_deleted > 0:
             # deleted rows would still be mined as queries: refuse rather than return pairs of deleted documents
             raise ValueError(f"mining a CorpusShard with deleted documents ({embeddings.n_deleted}) is not supported")
