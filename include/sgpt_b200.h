@@ -214,7 +214,10 @@ int sgpt_forward(sgpt_model_t m, const int32_t* ids, const int32_t* pos, const i
  *     rows `rows` of the batch the last sgpt_forward ran.  lm_head_w bf16[vocab,d] (the tied wte for GPT-Neo / BLOOM,
  *     lm_head.weight for GPT-J), lm_head_bias fp32[vocab] or NULL (GPT-J has one); rows,targets int32[M];
  *     greedy int32[M] or NULL receives argmax(logits) (:229, lowest index on ties).  The [M,vocab] logits exist only in
- *     `ws`, rows_per_chunk rows at a time (ws >= sgpt_lm_logprobs_workspace_bytes(d_model, vocab, rows_per_chunk)). */
+ *     `ws`, rows_per_chunk rows at a time (ws >= sgpt_lm_logprobs_workspace_bytes(d_model, vocab, rows_per_chunk));
+ *     ws must be 16-byte aligned (checked before any CUDA call, for every M).
+ *     The logits are not NaN-fixed like sgpt_scores: a selected row whose hidden state holds a NaN or +-inf gets a NaN
+ *     log-prob and greedy 0, the sgpt_token_logprobs rules for a row of NaN (the reference returns NaN too, :221). */
 int64_t sgpt_lm_logprobs_workspace_bytes(int d_model, int vocab, int rows_per_chunk);
 int sgpt_lm_logprobs(sgpt_model_t m, const void* lm_head_w, const float* lm_head_bias, int vocab, const int32_t* rows,
                      const int32_t* targets, int M, float* token_logprobs, int32_t* greedy, void* ws, int64_t ws_bytes,

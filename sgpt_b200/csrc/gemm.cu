@@ -276,6 +276,13 @@ int launch_scores(const void* Q, const void* C, const float* q_scale, const floa
   return launch_gemm<128, EpiScoresF32Masked>(Q, D, C, D, nq, n, D, p, stream, kCatScores);
 }
 
+int launch_lm_logits(const void* X, const void* W, float* logits, long long lds, int M, int vocab, int d,
+                     cudaStream_t stream) {
+  if (M == 0) return SGPT_OK;
+  EpiLogitsF32::Params p{logits, nullptr, nullptr, lds, nullptr, 0};
+  return launch_gemm<128, EpiLogitsF32>(X, d, W, d, M, vocab, d, p, stream, kCatScores);
+}
+
 }  // namespace sgpt
 
 using namespace sgpt;

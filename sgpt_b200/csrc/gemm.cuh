@@ -733,7 +733,8 @@ __device__ __forceinline__ float b1_term(float bits) { return __int2float_rn(-2 
 // scores_f32[q, doc] = fixnan(acc * row_scale[q] * col_scale[doc])       (cos_sim / dot_score, NaN -> -1)
 // kMasked: masked documents get kMaskedScoreBits instead (the dense plan of the masked search).
 // kB1: row_scale / col_scale hold int32 popcounts and the score is epi_score<true> (binary shards).
-template <bool kMasked, bool kB1 = false>
+// !kFixNaN: a NaN is stored as it is (the LM-head logits, whose NaN must reach the log-softmax).
+template <bool kMasked, bool kB1 = false, bool kFixNaN = true>
 struct OpScoresF32T {
   struct Params {
     float* out;
@@ -779,8 +780,10 @@ struct OpScoresF32T {
       for (int u = 0; u < 8; ++u) {
         const float rs = __shfl_sync(0xffffffffu, my_rs, r + u);
         float x = epi_score<kB1>(a[u].x, rs, c0), y = epi_score<kB1>(a[u].y, rs, c1);
-        x = (x != x) ? -1.f : x;
-        y = (y != y) ? -1.f : y;
+        if constexpr (kFixNaN) {
+          x = (x != x) ? -1.f : x;
+          y = (y != y) ? -1.f : y;
+        }
         masked(m0 + r + u, x, y);
         if (vec) *reinterpret_cast<float2*>(dst) = make_float2(x, y);
         else {
@@ -794,8 +797,10 @@ struct OpScoresF32T {
       const float rs = __shfl_sync(0xffffffffu, my_rs, r);
       const float2 a = slab_read(slab, r, lane);
       float x = epi_score<kB1>(a.x, rs, c0), y = epi_score<kB1>(a.y, rs, c1);
-      x = (x != x) ? -1.f : x;
-      y = (y != y) ? -1.f : y;
+      if constexpr (kFixNaN) {
+        x = (x != x) ? -1.f : x;
+        y = (y != y) ? -1.f : y;
+      }
       masked(m0 + r, x, y);
       if (vec) *reinterpret_cast<float2*>(dst) = make_float2(x, y);
       else {
@@ -1188,5 +1193,6 @@ using EpiScoresF32 = EpiStaged<OpScoresF32T<false>>;
 using EpiScoresF32Masked = EpiStaged<OpScoresF32T<true>>;
 using EpiScoresB1 = EpiStaged<OpScoresF32T<false, true>>;
 using EpiScoresB1Masked = EpiStaged<OpScoresF32T<true, true>>;
+using EpiLogitsF32 = EpiStaged<OpScoresF32T<false, false, false>>;  // LM-head logits: acc stored unchanged, NaN kept
 
 }  // namespace sgpt

@@ -66,6 +66,13 @@ int launch_sample_maxima(const void* Q, const void* C, const float* q_scale, con
 int launch_scores(const void* Q, const void* C, const float* q_scale, const float* c_scale, float* scores, long long lds,
                   int nq, int n, int D, DocMask mask, Operand op, cudaStream_t stream);
 
+// LM-head logits of sgpt_lm_logprobs (model.cu): logits[m, j] = <X[m,:], W[j,:]> as the fp32 accumulator holds it,
+// fp32 [M, lds], with X bf16 [M, d] and W bf16 [vocab, d].  Unlike launch_scores a NaN stays NaN (gemm.cuh
+// EpiLogitsF32), so a broken hidden state reaches the log-softmax.  d % 8 == 0, lds >= vocab; X, W and logits 16-byte
+// aligned.
+int launch_lm_logits(const void* X, const void* W, float* logits, long long lds, int M, int vocab, int d,
+                     cudaStream_t stream);
+
 // Grouped scan of the IVF search (ivf.cu; gemm.cuh EpiIvfRows): the filter GEMM's mainloop (BN = kSimBN, bf16 or s8)
 // over the work units of p.units, A = rows x D gathered query rows, C = the n x D list-ordered corpus.  Launches
 // min(p.max_units, SMs) persistent CTAs; the unit count is read on the device.

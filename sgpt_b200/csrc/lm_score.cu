@@ -1,7 +1,7 @@
 // Continuation log-likelihood scoring on top of the encoder (SURVEY.md §8f row 4: the SGPT cross-encoder,
 // crossencoder/beir/sgptce.py:150-262).  After the GPT forward pass, only the rows whose next-token distribution is
 // needed (the positions that predict a continuation token) go through ln_f and the LM head:
-//     logits[m, :] = LN_f(resid[rows[m], :]) @ W_lm^T (+ b_lm)          wgmma GEMM (gemm.cu: sgpt_scores)
+//     logits[m, :] = LN_f(resid[rows[m], :]) @ W_lm^T (+ b_lm)          wgmma GEMM (gemm.cu: launch_lm_logits)
 //     logprob[m]   = logits[m, target[m]] - logsumexp(logits[m, :])     == F.log_softmax(...).gather(...)  (:221, :247)
 // The [rows, vocab] fp32 logits live only in the caller's workspace, a chunk of rows at a time; the full
 // [batch, seq, vocab] tensor of the reference (:221) is never formed.

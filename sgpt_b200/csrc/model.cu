@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "../../include/sgpt_b200.h"
+#include "gemm_api.h"
 #include "host_utils.h"
 
 struct sgpt_model {
@@ -254,6 +255,8 @@ extern "C" int sgpt_lm_logprobs(sgpt_model_t m, const void* lm_head_w, const flo
   SGPT_REQUIRE(ws != nullptr && ws_bytes >= sgpt_lm_logprobs_workspace_bytes(d, vocab, rows_per_chunk),
                "sgpt_lm_logprobs: workspace too small (%lld < %lld bytes)", (long long)ws_bytes,
                (long long)sgpt_lm_logprobs_workspace_bytes(d, vocab, rows_per_chunk));
+  // the gathered rows are read by TMA, which needs 16-byte aligned addresses
+  SGPT_REQUIRE(reinterpret_cast<uintptr_t>(ws) % 16 == 0, "sgpt_lm_logprobs: ws must be 16-byte aligned");
   uint8_t* w = static_cast<uint8_t*>(ws);
   void* xsel = w;
   float* logits = reinterpret_cast<float*>(w + lm_align(static_cast<int64_t>(rows_per_chunk) * d * 2));
@@ -262,7 +265,7 @@ extern "C" int sgpt_lm_logprobs(sgpt_model_t m, const void* lm_head_w, const flo
     const int mc = (M - m0 < rows_per_chunk) ? M - m0 : rows_per_chunk;
     // hidden_states[-1] of the selected positions: ln_f of the residual stream the last sgpt_forward left behind
     SGPT_TRY(sgpt_layernorm_gather(m->resid, rows + m0, m->w.lnf_g, m->w.lnf_b, xsel, mc, d, m->cfg.ln_eps, stream));
-    SGPT_TRY(sgpt_scores(xsel, lm_head_w, nullptr, nullptr, logits, lds, mc, vocab, d, stream));
+    SGPT_TRY(launch_lm_logits(xsel, lm_head_w, logits, lds, mc, vocab, d, static_cast<cudaStream_t>(stream)));
     SGPT_TRY(sgpt_token_logprobs(logits, lds, mc, vocab, lm_head_bias, targets + m0, token_logprobs + m0,
                                  greedy ? greedy + m0 : nullptr, stream));
   }

@@ -144,12 +144,12 @@ class LazyF32Weights(dict):
         return dict.__getitem__(self, key).float()
 
 
-def full_size_weights(arch, spec, seed, device="cuda:0"):
+def full_size_weights(arch, spec, seed, device="cuda:0", host_copy=True):
     """Random weights of a FULL-SIZE model (BASELINE.json configs[2..4]) drawn on the GPU (torch.randn on the CPU needs
     a minute per billion parameters), linear weights in bf16 — exactly the values the CUDA path stores — LayerNorm
     parameters and biases in fp32.  Key names follow the HF state_dict of the architecture (oracle/*.py:init_weights
     use the same construction at small sizes).  Returns (device dict for sgpt_b200.Encoder, LazyF32Weights for the CPU
-    oracle holding the same values)."""
+    oracle holding the same values, or None with host_copy=False)."""
     import math
 
     g = torch.Generator(device=device).manual_seed(seed)
@@ -203,4 +203,4 @@ def full_size_weights(arch, spec, seed, device="cuda:0"):
     else:
         raise ValueError(arch)
     w["ln_f.weight"], w["ln_f.bias"] = rnd(d, sd=0.1, mean=1.0, dtype=f32), rnd(d, sd=0.05, dtype=f32)
-    return w, LazyF32Weights({k: v.cpu() for k, v in w.items()})
+    return w, (LazyF32Weights({k: v.cpu() for k, v in w.items()}) if host_copy else None)
