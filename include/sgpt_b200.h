@@ -353,6 +353,68 @@ int sgpt_range_search_i8(const void* Q, const void* C, const float* q_scale, con
                          int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * fp8 linear layers: every nn.Linear of an encoder block as an e4m3 x e4m3 wgmma GEMM with fp32 accumulation (the
+ * H100's fp8 tensor-core rate).  Everything else (embedding, LayerNorm, attention, the bf16 residual stream, pooling,
+ * ln_f, the LM head) is the bf16 flow unchanged.
+ *
+ * Row quantization (weights and activations alike), a row x of K bf16 values widened to fp32, fp32 round-to-nearest:
+ *   amax = max |x_j|;
+ *   a row holding a NaN or +-inf: q = 0, scale = NaN (every output of the row / output channel is NaN, as the bf16
+ *     GEMM's would be; it never turns finite);
+ *   amax == 0: inv = 0, q = +-0 (the signs of the zeros), scale = 0;
+ *   otherwise inv = min(448.0f / amax, FLT_MAX) (the min only acts for amax < 1.3e-36), q_j = cvt.rn.satfinite.e4m3(x_j *
+ *     inv) (round to nearest even, e4m3 subnormals kept, |q| <= 448), scale = amax / 448.0f.
+ * Weights: one row per output channel of the [out, in] weight, from the bf16 values the bf16 path stores, quantized once.
+ * Activations: one row per token of the GEMM's A operand, i.e. the bf16 tensor the bf16 path feeds that GEMM: the
+ *   LayerNorm output (quantized once and shared by QKV and fc on GPT-J's parallel branch), the attention output and the
+ *   gelu output, each quantized in a pass of its own.
+ * GEMM: acc = sum_k q_x[m,k] q_w[n,k] on the tensor cores (fp32 accumulator), then v = (acc * x_scale[m]) * w_scale[n] in
+ *   this order, then the bf16 path's epilogue unchanged (bias, gelu_new, GPT-J rotary, bf16 reduce-add).
+ * Accumulation precision (measured on an H100 80GB HBM3 at a 700 W power limit, tools/bench_fp8.py): with columns that
+ *   cancel exactly, so that the output is the accumulation error alone, the e4m3 accumulator stays within 2.9e-4
+ *   (~2^-11.8) of sum_k |x_k w_k| (median 6e-6 to 9e-6) at every K from 768 to 16384, against 7e-7 for the bf16 GEMM:
+ *   the hardware keeps far fewer accumulator bits for fp8, but the error does not grow with K.  No split accumulator is
+ *   used; the encoders' error against a quantization-aware fp32 reference is dominated by e4m3 codes that flip between
+ *   the fp32 reference and the GPU's bf16 intermediates (tests/test_gpu_fp8.py), not by the accumulation.
+ *
+ * sgpt_quantize_rows_fp8: x bf16[n, K] (16-byte aligned) -> q_out e4m3[n, K] (16-byte aligned), scale_out fp32[n];
+ *   K % 16 == 0.
+ * sgpt_linear_fp8: sgpt_linear with xq e4m3[M, K] (pitch ldx bytes), x_scale fp32[M], wq e4m3[N, K] (pitch ldw),
+ *   w_scale fp32[N]; K, ldx, ldw multiples of 16; the three epilogues of sgpt_linear.  Split-K is not supported
+ *   (SGPT_GEMM_SPLITK > 1 is rejected).
+ * sgpt_linear_qkv_rotary_fp8: sgpt_linear_qkv_rotary with xq e4m3[M, d] (pitch ldx), x_scale fp32[M], wq_qkv e4m3[3d, d],
+ *   w_scale fp32[3d].
+ * sgpt_model_create_fp8: sgpt_model_create whose linear layers run in fp8: fp8_layers is a HOST array of n_layer entries
+ *   (copied at create) of borrowed device (e4m3 weight, fp32 scale) pairs, the weights quantized by
+ *   sgpt_quantize_rows_fp8 in the layouts of sgpt_layer_weights.  The bf16 linear pointers of w->layers are not read
+ *   and may be NULL.  The handle additionally owns an e4m3 activation buffer [max_tokens, max(d_model, d_ff)] and
+ *   fp32 scales [max_tokens].  sgpt_encode, sgpt_forward, sgpt_lm_logprobs, sgpt_model_read_residual and
+ *   sgpt_model_set_position_weights take the handle unchanged.
+ * Arguments are checked (sizes, K % 16, null operands or scales, unknown epilogue, split-K) before any CUDA call.
+ * ------------------------------------------------------------------------------------------------------------------ */
+int sgpt_quantize_rows_fp8(const void* x, void* q_out, float* scale_out, int64_t n, int K, sgpt_stream_t stream);
+int sgpt_linear_fp8(const void* xq, int64_t ldx, const float* x_scale, const void* wq, int64_t ldw, const float* w_scale,
+                    const float* bias, void* out, int64_t ldo, const void* resid, int M, int N, int K, int epilogue,
+                    sgpt_stream_t stream);
+int sgpt_linear_qkv_rotary_fp8(const void* xq, int64_t ldx, const float* x_scale, const void* wq_qkv,
+                               const float* w_scale, void* qkv, const int32_t* pos, const float* cos_sin, int M,
+                               int d_model, int head_dim, int rotary_dim, int max_pos, sgpt_stream_t stream);
+
+typedef struct sgpt_fp8_layer_weights {
+  const void* w_qkv;   /* e4m3[3d, d] */
+  const float* s_qkv;  /* fp32[3d] */
+  const void* w_o;     /* e4m3[d, d] */
+  const float* s_o;    /* fp32[d] */
+  const void* w_fc;    /* e4m3[ff, d] */
+  const float* s_fc;   /* fp32[ff] */
+  const void* w_proj;  /* e4m3[d, ff] */
+  const float* s_proj; /* fp32[d] */
+} sgpt_fp8_layer_weights;
+
+int sgpt_model_create_fp8(const sgpt_model_config* cfg, const sgpt_model_weights* w,
+                          const sgpt_fp8_layer_weights* fp8_layers, sgpt_model_t* out);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * §8e without a collective library call: the per-shard top-k lists are PUSHED into every rank's gather buffer by the
  * final selection kernel itself (stores through NVLink peer mappings + a system-scope release per query) and merged by
  * a kernel that acquires those per-query counters — the reference's sequential chunk/heapq merge (XS:80-132) with

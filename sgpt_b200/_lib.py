@@ -34,6 +34,11 @@ class LayerWeightsC(C.Structure):
                 ("_pad", i32)]
 
 
+class Fp8LayerWeightsC(C.Structure):
+    _fields_ = [("w_qkv", vp), ("s_qkv", vp), ("w_o", vp), ("s_o", vp), ("w_fc", vp), ("s_fc", vp), ("w_proj", vp),
+                ("s_proj", vp)]
+
+
 class ModelWeightsC(C.Structure):
     _fields_ = [("wte", vp), ("wpe", vp), ("lnf_g", vp), ("lnf_b", vp), ("layers", C.POINTER(LayerWeightsC)),
                 ("emb_ln_g", vp), ("emb_ln_b", vp)]
@@ -111,6 +116,11 @@ _SIGNATURES = {
     "sgpt_rerank_workspace_bytes": (i64, [i32, i64]),
     "sgpt_rerank": (i32, [i32, vp, vp, vp, vp, i32, i64, i32, i64, vp, i64, i32, vp, vp, vp, i64, vp]),
     "sgpt_quantize_rows_b1": (i32, [vp, i32, vp, vp, vp, i64, i32, vp]),
+    "sgpt_quantize_rows_fp8": (i32, [vp, vp, vp, i64, i32, vp]),
+    "sgpt_linear_fp8": (i32, [vp, i64, vp, vp, i64, vp, vp, vp, i64, vp, i32, i32, i32, i32, vp]),
+    "sgpt_linear_qkv_rotary_fp8": (i32, [vp, i64, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
+    "sgpt_model_create_fp8": (i32, [C.POINTER(ModelConfigC), C.POINTER(ModelWeightsC), C.POINTER(Fp8LayerWeightsC),
+                                    C.POINTER(vp)]),
 }
 DTYPE_BF16, DTYPE_I8, DTYPE_B1 = 0, 1, 3
 

@@ -44,8 +44,9 @@ class LogLikelihoodScorer:
     ``lm_head.weight`` (+ ``lm_head.bias`` for GPT-J) when present, else the tied token embedding."""
 
     def __init__(self, cfg: ModelConfig, state_dict: Dict[str, torch.Tensor], device="cuda:0", max_tokens: int = 32768,
-                 max_batch: int = 256, rows_per_chunk: int = 1024):
-        self.encoder = Encoder(cfg, state_dict, device=device, max_tokens=max_tokens, max_batch=max_batch)
+                 max_batch: int = 256, rows_per_chunk: int = 1024, precision: str = "bf16"):
+        self.encoder = Encoder(cfg, state_dict, device=device, max_tokens=max_tokens, max_batch=max_batch,
+                               precision=precision)
         self.cfg, self.device = cfg, self.encoder.device
         sd = {(k[len("transformer."):] if k.startswith("transformer.") else k): v for k, v in state_dict.items()}
         emb_key = "word_embeddings.weight" if cfg.arch == "bloom" else "wte.weight"

@@ -48,27 +48,30 @@ static int launch_gemm(const void* a, int64_t lda, const void* b, int64_t ldb, i
 // nn.Linear dispatch: gemm_linear_kernel, 128 x 128 tiles.  Tile rasterisation (gemm.cuh TileMap::band): banded
 // M-fastest order once the weight matrix no longer fits in the H100's 50 MB L2 next to the activations.
 // SGPT_GEMM_BAND=<g> forces a band height (0 = N fastest) for A/B measurements; read per call.
-static int pick_band(int M, int N, int K) {
+static int pick_band(int M, int N, int K, int w_elem_bytes = 2) {
   if (const char* e = getenv("SGPT_GEMM_BAND")) return atoi(e);
-  const long long w_bytes = 2ll * N * K;
+  const long long w_bytes = static_cast<long long>(w_elem_bytes) * N * K;
   const int m_tiles = (M + kGemmBM - 1) / kGemmBM;
   return (w_bytes >= (32ll << 20) && m_tiles >= 16) ? 8 : 0;
 }
 
-template <class Op>
+// kOp = kE4M3: x, w, ldx, ldw and K in bytes (e4m3 elements), UINT8 tensor maps with 128-element K boxes
+template <class Op, Operand kOp = Operand::kBF16>
 static int launch_linear(const void* x, int64_t ldx, const void* w, int64_t ldw, int M, int N, int K,
                          const typename Op::Params& p, cudaStream_t stream, int ksplit = 1) {
+  constexpr bool kF8 = kOp == Operand::kE4M3;
   TileMap tm;
   tm.ksplit = ksplit;
-  tm.band = pick_band(M, N, K);
+  tm.band = pick_band(M, N, K, kF8 ? 1 : 2);
+  auto make_map = kF8 ? make_tma_2d_u8 : make_tma_2d_bf16;
+  const uint32_t box_k = kF8 ? 2 * kGemmBK : kGemmBK;  // one 128-byte row segment per box row
   CUtensorMap ta, tb;
-  int rc = make_tma_2d_bf16(&ta, x, static_cast<uint64_t>(M), static_cast<uint64_t>(K), static_cast<uint64_t>(ldx),
-                            kGemmBM, kGemmBK);
+  int rc = make_map(&ta, x, static_cast<uint64_t>(M), static_cast<uint64_t>(K), static_cast<uint64_t>(ldx), kGemmBM,
+                    box_k);
   if (rc != SGPT_OK) return rc;
-  rc = make_tma_2d_bf16(&tb, w, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldw), kLinBN,
-                        kGemmBK);
+  rc = make_map(&tb, w, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldw), kLinBN, box_k);
   if (rc != SGPT_OK) return rc;
-  auto kern = gemm_linear_kernel<Op>;
+  auto kern = gemm_linear_kernel<Op, kOp>;
   static PerDeviceOnce attr_once;
   if (attr_once.first()) {
     SGPT_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, LinearCfg::kSmemBytes));
@@ -387,4 +390,78 @@ extern "C" int sgpt_scores_i8(const void* Q, const void* C, const float* q_scale
   SGPT_REQUIRE(lds >= n, "sgpt_scores_i8: lds < n");
   SGPT_REQUIRE(nq == 0 || n == 0 || scores != nullptr, "sgpt_scores_i8: null output");
   return launch_scores(Q, C, q_scale, c_scale, scores, lds, nq, static_cast<int>(n), D, DocMask(), Operand::kS8, stream);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// fp8 linear layers (include/sgpt_b200.h): e4m3 x e4m3 with fp32 accumulation, the bf16 epilogues behind
+// OpDequantE4M3.  No split-K.
+// ---------------------------------------------------------------------------------------------------------------
+static int check_fp8_operands(const char* fn, const void* xq, int64_t ldx, const float* x_scale, const void* wq,
+                              int64_t ldw, const float* w_scale, int M, int N, int K) {
+  SGPT_REQUIRE(M >= 0 && N > 0 && K > 0, "%s: bad sizes M=%d N=%d K=%d", fn, M, N, K);
+  SGPT_REQUIRE(K % 16 == 0 && ldx % 16 == 0 && ldw % 16 == 0,
+               "%s: K, ldx and ldw must be multiples of 16 (e4m3 rows of 16-byte multiples)", fn);
+  SGPT_REQUIRE(ldx >= K && ldw >= K, "%s: row pitch smaller than the row", fn);
+  SGPT_REQUIRE(M == 0 || (xq != nullptr && wq != nullptr && x_scale != nullptr && w_scale != nullptr),
+               "%s: null operand or scale", fn);
+  return SGPT_OK;
+}
+
+extern "C" int sgpt_linear_fp8(const void* xq, int64_t ldx, const float* x_scale, const void* wq, int64_t ldw,
+                               const float* w_scale, const float* bias, void* out, int64_t ldo, const void* resid, int M,
+                               int N, int K, int epilogue, sgpt_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const int rc0 = check_fp8_operands("sgpt_linear_fp8", xq, ldx, x_scale, wq, ldw, w_scale, M, N, K);
+  if (rc0 != SGPT_OK) return rc0;
+  SGPT_REQUIRE(ldo >= N && ldo % 8 == 0, "sgpt_linear_fp8: ldo must be >= N and a multiple of 8");
+  SGPT_REQUIRE(epilogue == SGPT_EPI_BF16 || epilogue == SGPT_EPI_GELU_BF16 || epilogue == SGPT_EPI_RESID_BF16,
+               "sgpt_linear_fp8: unknown epilogue %d", epilogue);
+  SGPT_REQUIRE(epilogue != SGPT_EPI_RESID_BF16 || (resid != nullptr && resid == out),
+               "sgpt_linear_fp8: SGPT_EPI_RESID_BF16 updates the bf16 residual stream in place (resid must alias out)");
+  if (const char* e = getenv("SGPT_GEMM_SPLITK"))
+    SGPT_REQUIRE(atoi(e) <= 1, "sgpt_linear_fp8: split-K is not supported for fp8 operands (SGPT_GEMM_SPLITK=%s)", e);
+  if (M == 0) return SGPT_OK;
+  CUtensorMap om;
+  int rc = make_tma_2d_bf16(&om, out, static_cast<uint64_t>(M), static_cast<uint64_t>(N), static_cast<uint64_t>(ldo), 32,
+                            64);
+  if (rc != SGPT_OK) return rc;
+  constexpr Operand kF8 = Operand::kE4M3;
+  if (epilogue == SGPT_EPI_RESID_BF16) {
+    using Op = OpDequantE4M3<OpTmaResidAddBF16>;
+    Op::Params p{{om, bias}, x_scale, w_scale};
+    return launch_linear<Op, kF8>(xq, ldx, wq, ldw, M, N, K, p, stream);
+  }
+  if (epilogue == SGPT_EPI_BF16) {
+    using Op = OpDequantE4M3<OpTmaBiasActBF16<false>>;
+    Op::Params p{{om, bias}, x_scale, w_scale};
+    return launch_linear<Op, kF8>(xq, ldx, wq, ldw, M, N, K, p, stream);
+  }
+  using Op = OpDequantE4M3<OpTmaBiasActBF16<true>>;
+  Op::Params p{{om, bias}, x_scale, w_scale};
+  return launch_linear<Op, kF8>(xq, ldx, wq, ldw, M, N, K, p, stream);
+}
+
+extern "C" int sgpt_linear_qkv_rotary_fp8(const void* xq, int64_t ldx, const float* x_scale, const void* wq_qkv,
+                                          const float* w_scale, void* qkv, const int32_t* pos, const float* cos_sin, int M,
+                                          int d_model, int head_dim, int rotary_dim, int max_pos,
+                                          sgpt_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const int rc0 = check_fp8_operands("sgpt_linear_qkv_rotary_fp8", xq, ldx, x_scale, wq_qkv, d_model, w_scale, M,
+                                     3 * d_model, d_model);
+  if (rc0 != SGPT_OK) return rc0;
+  SGPT_REQUIRE(head_dim > 0 && d_model % head_dim == 0 && head_dim % 8 == 0,
+               "sgpt_linear_qkv_rotary_fp8: bad head_dim %d", head_dim);
+  SGPT_REQUIRE(rotary_dim >= 0 && rotary_dim <= head_dim && rotary_dim % 8 == 0,
+               "sgpt_linear_qkv_rotary_fp8: rotary_dim %d must be a multiple of 8 and <= head_dim", rotary_dim);
+  SGPT_REQUIRE(pos != nullptr && cos_sin != nullptr && max_pos > 0, "sgpt_linear_qkv_rotary_fp8: pos / cos_sin missing");
+  if (M == 0) return SGPT_OK;
+  const int N = 3 * d_model;
+  CUtensorMap om;
+  int rc = make_tma_2d_bf16(&om, qkv, static_cast<uint64_t>(M), static_cast<uint64_t>(N), static_cast<uint64_t>(N), 32,
+                            64);
+  if (rc != SGPT_OK) return rc;
+  using Op = OpDequantE4M3<OpTmaRotaryBF16>;
+  Op::Params p{{om, pos, reinterpret_cast<const float2*>(cos_sin), M, d_model, head_dim, rotary_dim, max_pos}, x_scale,
+               w_scale};
+  return launch_linear<Op, Operand::kE4M3>(xq, ldx, wq_qkv, d_model, M, N, d_model, p, stream);
 }

@@ -389,12 +389,19 @@ struct LinearCfg {
 // named barriers of gemm_linear_kernel (0 is __syncthreads): all consumers; turn of consumer c; epilogue of consumer c
 constexpr int kBarConsumers = 1, kBarTurn = 2, kBarEpi = 4;
 
-template <class Op>
+// kOp: kBF16, or kE4M3 (fp8 linear layers): a K-block is then 128 e4m3 = the same 128 bytes per row as 64 bf16, so the
+// stages, TMA boxes, ring and the +32-byte descriptor step per MMA are unchanged; 4 m64n128k32 per k-block and operand
+// half instead of 4 m64n128k16, fp32 accumulators either way (Op is the dequantizing OpDequantE4M3<...>).
+template <class Op, Operand kOp = Operand::kBF16>
 __global__ void __launch_bounds__(kLinThreads, 1)
 gemm_linear_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, int M, int N,
                    int K, const __grid_constant__ typename Op::Params ep, TileMap tmap) {
   using Cfg = LinearCfg;
   constexpr int kStages = Cfg::kStages;
+  static_assert(kOp == Operand::kBF16 || kOp == Operand::kE4M3, "linear-layer operand type");
+  constexpr bool kF8 = kOp == Operand::kE4M3;
+  constexpr int kBK = kF8 ? 2 * kGemmBK : kGemmBK;  // K elements per k-block (128 bytes per row either way)
+  constexpr int kMmaK = kF8 ? 32 : 16;              // K elements per wgmma
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_tiles = smem;
@@ -407,7 +414,7 @@ gemm_linear_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
   const int n_tiles = (N + kLinBN - 1) / kLinBN;
   const int ksplit = tmap.ksplit;
   const int num_units = m_tiles * n_tiles * ksplit;
-  const int num_kb = (K + kGemmBK - 1) / kGemmBK;
+  const int num_kb = (K + kBK - 1) / kBK;
   const int kb_per = (num_kb + ksplit - 1) / ksplit;  // k-blocks per slice (the host keeps every slice non-empty)
 
   if (threadIdx.x == 0) {
@@ -437,8 +444,8 @@ gemm_linear_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem_tiles + stage * Cfg::kStageBytes;
           mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-          tma_load_2d(sa, &tma_a, &full_bar[stage], kb * kGemmBK, mg * kGemmBM);
-          tma_load_2d(sa + Cfg::kABytes, &tma_b, &full_bar[stage], kb * kGemmBK, nt * kLinBN);
+          tma_load_2d(sa, &tma_a, &full_bar[stage], kb * kBK, mg * kGemmBM);
+          tma_load_2d(sa + Cfg::kABytes, &tma_b, &full_bar[stage], kb * kBK, nt * kLinBN);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
@@ -485,10 +492,15 @@ gemm_linear_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
       wgmma_fence_acc(acc1);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < kGemmBK / 16; ++k) {
+      for (int k = 0; k < kBK / kMmaK; ++k) {
         const int scale_d = (kb > kb_begin || k > 0) ? 1 : 0;
-        wgmma_bf16_m64n128(acc0, da0 + 2 * k, db + 2 * k, scale_d);
-        wgmma_bf16_m64n128(acc1, da1 + 2 * k, db + 2 * k, scale_d);
+        if constexpr (kF8) {
+          wgmma_e4m3_m64n128(acc0, da0 + 2 * k, db + 2 * k, scale_d);
+          wgmma_e4m3_m64n128(acc1, da1 + 2 * k, db + 2 * k, scale_d);
+        } else {
+          wgmma_bf16_m64n128(acc0, da0 + 2 * k, db + 2 * k, scale_d);
+          wgmma_bf16_m64n128(acc1, da1 + 2 * k, db + 2 * k, scale_d);
+        }
       }
       wgmma_commit();
       wgmma_fence_acc(acc0);
@@ -653,6 +665,48 @@ struct OpTmaResidAddBF16 {
   }
   static __device__ __forceinline__ void issue(const Params& p, const void* box, int n, int m0) {
     tma_reduce_add_2d(&p.out_map, box, n, m0);
+  }
+};
+
+// fp8 linear layers (include/sgpt_b200.h): the e4m3 accumulator is dequantized as v = (acc * x_scale[m]) * w_scale[n],
+// in this order, and handed to the bf16 path's Op unchanged.  Scales of rows / columns beyond M / N are read from the
+// last valid entry (their outputs are clipped by the tensor map).
+template <class Op>
+struct OpDequantE4M3 {
+  struct Params {
+    typename Op::Params op;
+    const float* x_scale;  // [M] per token
+    const float* w_scale;  // [N] per output channel
+  };
+  struct Rows {
+    typename Op::Rows op;
+    float s[4];
+  };
+  struct Col {
+    typename Op::Col op;
+    float2 s;
+  };
+  static __device__ __forceinline__ void rows(const Params& p, Rows& rw, int r0, int M) {
+    Op::rows(p.op, rw.op, r0, M);
+#pragma unroll
+    for (int ri = 0; ri < 4; ++ri) {
+      const int row = r0 + 8 * (ri & 1) + 64 * (ri >> 1);
+      rw.s[ri] = __ldg(p.x_scale + (row < M ? row : M - 1));
+    }
+  }
+  static __device__ __forceinline__ Col col(const Params& p, int c, int N, bool first_slice) {
+    Col cl;
+    cl.op = Op::col(p.op, c, N, first_slice);
+    cl.s = make_float2(__ldg(p.w_scale + (c < N ? c : N - 1)), __ldg(p.w_scale + (c + 1 < N ? c + 1 : N - 1)));
+    return cl;
+  }
+  static __device__ __forceinline__ uint32_t pair(const Params& p, const Rows& rw, const Col& cl, int ri, float x0,
+                                                  float x1) {
+    return Op::pair(p.op, rw.op, cl.op, ri, __fmul_rn(__fmul_rn(x0, rw.s[ri]), cl.s.x),
+                    __fmul_rn(__fmul_rn(x1, rw.s[ri]), cl.s.y));
+  }
+  static __device__ __forceinline__ void issue(const Params& p, const void* box, int n, int m0) {
+    Op::issue(p.op, box, n, m0);
   }
 };
 

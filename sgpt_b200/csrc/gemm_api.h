@@ -13,7 +13,8 @@ constexpr int kMaxDimB1 = 65536;
 
 // Operand type of the similarity GEMM (gemm.cuh gemm_bf16_tn_kernel): bf16 rows, int8 rows, or packed sign bits (D / 8
 // bytes per row, include/sgpt_b200.h binary corpus shards).  Functions below take D in dimensions for every type.
-enum class Operand : int { kBF16 = 0, kS8 = 1, kB1 = 2 };
+// kE4M3: fp8 rows of the linear-layer GEMM only (gemm.cuh gemm_linear_kernel, include/sgpt_b200.h fp8 linear layers).
+enum class Operand : int { kBF16 = 0, kS8 = 1, kB1 = 2, kE4M3 = 3 };
 
 // Geometry of the candidate lists the filter GEMM writes for a launch over `tiles` corpus tiles: every (CTA, column
 // half) is a group with a private list of `L` entries per query (worst case: every score of every visited tile).

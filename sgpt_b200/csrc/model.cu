@@ -10,6 +10,8 @@
 // The handle borrows the caller's weight buffers and owns only its activation workspace, laid out for a ragged batch
 // of at most cfg.max_tokens rows:
 //     resid bf16[T,d] | xb bf16[T,d] | qkv bf16[T,3d] | attn bf16[T,d] | ffn bf16[T,ff] | stats fp32[2T+B]
+// and, with fp8 linear layers (sgpt_model_create_fp8), the quantized A operand of the next GEMM:
+//     xq e4m3[T, max(d,ff)] | xs fp32[T]
 //
 // Each block runs LayerNorm as a pass of its own (residual stream -> bf16 xb), then GEMMs with bias / gelu epilogues for
 // the layers that read xb and bf16 reduce-add epilogues for the layers that update the bf16 residual stream.
@@ -26,6 +28,9 @@ struct sgpt_model {
   sgpt_model_config cfg;
   sgpt_model_weights w;
   std::vector<sgpt_layer_weights> layers;
+  std::vector<sgpt_fp8_layer_weights> fp8_layers;  // non-empty: the linear layers run in fp8
+  void* xq = nullptr;     // fp8: e4m3 rows of the GEMM's A operand
+  float* xs = nullptr;    // fp8: their scales
   int device = 0;
   void* resid = nullptr;  // the residual stream, bf16
   void* xn = nullptr;     // xb: LayerNorm output, the A operand of the QKV / c_fc GEMMs
@@ -58,7 +63,9 @@ static std::vector<float> alibi_slopes(int n_head) {
   return s;
 }
 
-extern "C" int sgpt_model_create(const sgpt_model_config* cfg, const sgpt_model_weights* w, sgpt_model_t* out) {
+// fp8_layers == nullptr: the bf16 handle (sgpt_model_create)
+static int model_create(const sgpt_model_config* cfg, const sgpt_model_weights* w,
+                        const sgpt_fp8_layer_weights* fp8_layers, sgpt_model_t* out) {
   SGPT_REQUIRE(cfg != nullptr && w != nullptr && out != nullptr, "sgpt_model_create: null argument");
   *out = nullptr;
   SGPT_REQUIRE(cfg->arch == SGPT_ARCH_GPT_NEO || cfg->arch == SGPT_ARCH_GPTJ || cfg->arch == SGPT_ARCH_BLOOM,
@@ -83,11 +90,15 @@ extern "C" int sgpt_model_create(const sgpt_model_config* cfg, const sgpt_model_
   m->w = *w;
   m->layers.assign(w->layers, w->layers + cfg->n_layer);
   m->w.layers = m->layers.data();
+  if (fp8_layers != nullptr) m->fp8_layers.assign(fp8_layers, fp8_layers + cfg->n_layer);
   for (int l = 0; l < cfg->n_layer; ++l) {
     const sgpt_layer_weights& lw = m->layers[l];
     const bool need_ln2 = cfg->arch != SGPT_ARCH_GPTJ;
-    if (!lw.ln1_g || !lw.ln1_b || !lw.w_qkv || !lw.w_o || !lw.w_fc || !lw.w_proj ||
-        (need_ln2 && (!lw.ln2_g || !lw.ln2_b))) {
+    const bool linear_ok = fp8_layers != nullptr
+                               ? (fp8_layers[l].w_qkv && fp8_layers[l].s_qkv && fp8_layers[l].w_o && fp8_layers[l].s_o &&
+                                  fp8_layers[l].w_fc && fp8_layers[l].s_fc && fp8_layers[l].w_proj && fp8_layers[l].s_proj)
+                               : (lw.w_qkv && lw.w_o && lw.w_fc && lw.w_proj);
+    if (!lw.ln1_g || !lw.ln1_b || !linear_ok || (need_ln2 && (!lw.ln2_g || !lw.ln2_b))) {
       delete m;
       set_error("sgpt_model_create: layer %d has missing weights", l);
       return SGPT_ERR_INVALID;
@@ -102,6 +113,10 @@ extern "C" int sgpt_model_create(const sgpt_model_config* cfg, const sgpt_model_
   if (e == cudaSuccess) e = cudaMalloc(&m->ffn, T * static_cast<size_t>(cfg->d_ff) * 2);
   // (mean, rstd) per row for ln_f, then the per-sequence sums of squares of the normalisation (sgpt_pool)
   if (e == cudaSuccess) e = cudaMalloc(&m->stats, (2 * T + static_cast<size_t>(cfg->max_batch)) * 4);
+  if (e == cudaSuccess && fp8_layers != nullptr) {
+    e = cudaMalloc(&m->xq, T * static_cast<size_t>(cfg->d_ff > cfg->d_model ? cfg->d_ff : cfg->d_model));
+    if (e == cudaSuccess) e = cudaMalloc(&m->xs, T * 4);
+  }
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
   if (e == cudaSuccess && cfg->arch == SGPT_ARCH_GPTJ) {
     // create_sinusoidal_positions, HF:gptj/modeling_gptj.py:45-48: angle(p, i) = p * 10000^(-2i/rotary_dim), fp32
@@ -131,6 +146,16 @@ extern "C" int sgpt_model_create(const sgpt_model_config* cfg, const sgpt_model_
   return SGPT_OK;
 }
 
+extern "C" int sgpt_model_create(const sgpt_model_config* cfg, const sgpt_model_weights* w, sgpt_model_t* out) {
+  return model_create(cfg, w, nullptr, out);
+}
+
+extern "C" int sgpt_model_create_fp8(const sgpt_model_config* cfg, const sgpt_model_weights* w,
+                                     const sgpt_fp8_layer_weights* fp8_layers, sgpt_model_t* out) {
+  SGPT_REQUIRE(fp8_layers != nullptr, "sgpt_model_create_fp8: null fp8 layer weights");
+  return model_create(cfg, w, fp8_layers, out);
+}
+
 extern "C" void sgpt_model_destroy(sgpt_model_t m) {
   if (!m) return;
   cudaFree(m->resid);
@@ -141,6 +166,8 @@ extern "C" void sgpt_model_destroy(sgpt_model_t m) {
   cudaFree(m->stats);
   cudaFree(m->rotary);
   cudaFree(m->alibi);
+  cudaFree(m->xq);
+  cudaFree(m->xs);
   delete m;
 }
 
@@ -187,39 +214,60 @@ extern "C" int sgpt_encode(sgpt_model_t m, const int32_t* ids, const int32_t* po
   if (c.arch == SGPT_ARCH_BLOOM)
     SGPT_TRY(sgpt_layernorm(m->resid, m->w.emb_ln_g, m->w.emb_ln_b, m->resid, T, d, c.ln_eps, stream));
   const int n_run = layer_idx;  // hidden_states[i] is the input of block i; hidden_states[L] is ln_f(output of block L-1)
+  // fp8 linear layers: `quant` turns the bf16 A operand of the next GEMM(s) into m->xq / m->xs, `lin` runs a GEMM on it
+  const bool f8 = !m->fp8_layers.empty();
+  auto quant = [&](const void* x, int K) { return f8 ? sgpt_quantize_rows_fp8(x, m->xq, m->xs, T, K, stream) : SGPT_OK; };
+  auto lin = [&](const void* x, int K, const void* w, const void* wq, const float* ws, const float* b, void* out, int N,
+                 int epi) {
+    const void* resid = epi == SGPT_EPI_RESID_BF16 ? out : nullptr;
+    if (f8) return sgpt_linear_fp8(m->xq, K, m->xs, wq, K, ws, b, out, N, resid, T, N, K, epi, stream);
+    return sgpt_linear(x, K, w, K, b, out, N, resid, T, N, K, epi, stream);
+  };
   for (int l = 0; l < n_run && l < c.n_layer; ++l) {
     const sgpt_layer_weights& lw = m->layers[l];
+    const sgpt_fp8_layer_weights fw = f8 ? m->fp8_layers[l] : sgpt_fp8_layer_weights{};
     if (all_layers)  // hidden_states[l] = the residual stream entering block l (no ln_f)
       SGPT_TRY(sgpt_pool(m->resid, 1, pos, cu_seqlens, nullptr, nullptr, c.ln_eps, nullptr, 0, out, nullptr, B, T, d,
                          base_mode, clamp_denominator, 0, /*accumulate=*/l > 0, layer_scale, stream));
     SGPT_TRY(sgpt_layernorm(m->resid, lw.ln1_g, lw.ln1_b, m->xn, T, d, c.ln_eps, stream));
+    SGPT_TRY(quant(m->xn, d));
     if (c.arch == SGPT_ARCH_GPT_NEO) {
-      SGPT_TRY(sgpt_linear(m->xn, d, lw.w_qkv, d, lw.b_qkv, m->qkv, 3 * d, nullptr, T, 3 * d, d, SGPT_EPI_BF16, stream));
+      SGPT_TRY(lin(m->xn, d, lw.w_qkv, fw.w_qkv, fw.s_qkv, lw.b_qkv, m->qkv, 3 * d, SGPT_EPI_BF16));
       const int window = (lw.local_attention && c.window > 0 && max_seqlen > c.window) ? c.window : 0;
       SGPT_TRY(sgpt_attention(m->qkv, m->attn, cu_seqlens, B, T, H, hd, /*scale=*/1.0f, window, max_seqlen, nullptr, 0,
                               stream));
-      SGPT_TRY(sgpt_linear(m->attn, d, lw.w_o, d, lw.b_o, m->resid, d, m->resid, T, d, d, SGPT_EPI_RESID_BF16, stream));
+      SGPT_TRY(quant(m->attn, d));
+      SGPT_TRY(lin(m->attn, d, lw.w_o, fw.w_o, fw.s_o, lw.b_o, m->resid, d, SGPT_EPI_RESID_BF16));
       SGPT_TRY(sgpt_layernorm(m->resid, lw.ln2_g, lw.ln2_b, m->xn, T, d, c.ln_eps, stream));
-      SGPT_TRY(sgpt_linear(m->xn, d, lw.w_fc, d, lw.b_fc, m->ffn, ff, nullptr, T, ff, d, SGPT_EPI_GELU_BF16, stream));
-      SGPT_TRY(sgpt_linear(m->ffn, ff, lw.w_proj, ff, lw.b_proj, m->resid, d, m->resid, T, d, ff,
-                           SGPT_EPI_RESID_BF16, stream));
+      SGPT_TRY(quant(m->xn, d));
+      SGPT_TRY(lin(m->xn, d, lw.w_fc, fw.w_fc, fw.s_fc, lw.b_fc, m->ffn, ff, SGPT_EPI_GELU_BF16));
+      SGPT_TRY(quant(m->ffn, ff));
+      SGPT_TRY(lin(m->ffn, ff, lw.w_proj, fw.w_proj, fw.s_proj, lw.b_proj, m->resid, d, SGPT_EPI_RESID_BF16));
     } else if (c.arch == SGPT_ARCH_GPTJ) {
-      SGPT_TRY(sgpt_linear_qkv_rotary(m->xn, d, lw.w_qkv, m->qkv, pos, m->rotary, T, d, hd, c.rotary_dim, c.max_pos,
-                                      stream));
+      if (f8)
+        SGPT_TRY(sgpt_linear_qkv_rotary_fp8(m->xq, d, m->xs, fw.w_qkv, fw.s_qkv, m->qkv, pos, m->rotary, T, d, hd,
+                                            c.rotary_dim, c.max_pos, stream));
+      else
+        SGPT_TRY(sgpt_linear_qkv_rotary(m->xn, d, lw.w_qkv, m->qkv, pos, m->rotary, T, d, hd, c.rotary_dim, c.max_pos,
+                                        stream));
       SGPT_TRY(sgpt_attention(m->qkv, m->attn, cu_seqlens, B, T, H, hd, inv_sqrt_hd, 0, max_seqlen, nullptr, 0, stream));
-      // both branches read the same ln_1 output and are accumulated into the residual stream (attn + mlp + residual)
-      SGPT_TRY(sgpt_linear(m->xn, d, lw.w_fc, d, lw.b_fc, m->ffn, ff, nullptr, T, ff, d, SGPT_EPI_GELU_BF16, stream));
-      SGPT_TRY(sgpt_linear(m->attn, d, lw.w_o, d, lw.b_o, m->resid, d, m->resid, T, d, d, SGPT_EPI_RESID_BF16, stream));
-      SGPT_TRY(sgpt_linear(m->ffn, ff, lw.w_proj, ff, lw.b_proj, m->resid, d, m->resid, T, d, ff,
-                           SGPT_EPI_RESID_BF16, stream));
+      // both branches read the same ln_1 output and are accumulated into the residual stream (attn + mlp + residual);
+      // with fp8 the quantized ln_1 output is still in xq here
+      SGPT_TRY(lin(m->xn, d, lw.w_fc, fw.w_fc, fw.s_fc, lw.b_fc, m->ffn, ff, SGPT_EPI_GELU_BF16));
+      SGPT_TRY(quant(m->attn, d));
+      SGPT_TRY(lin(m->attn, d, lw.w_o, fw.w_o, fw.s_o, lw.b_o, m->resid, d, SGPT_EPI_RESID_BF16));
+      SGPT_TRY(quant(m->ffn, ff));
+      SGPT_TRY(lin(m->ffn, ff, lw.w_proj, fw.w_proj, fw.s_proj, lw.b_proj, m->resid, d, SGPT_EPI_RESID_BF16));
     } else {  // BLOOM
-      SGPT_TRY(sgpt_linear(m->xn, d, lw.w_qkv, d, lw.b_qkv, m->qkv, 3 * d, nullptr, T, 3 * d, d, SGPT_EPI_BF16, stream));
+      SGPT_TRY(lin(m->xn, d, lw.w_qkv, fw.w_qkv, fw.s_qkv, lw.b_qkv, m->qkv, 3 * d, SGPT_EPI_BF16));
       SGPT_TRY(sgpt_attention(m->qkv, m->attn, cu_seqlens, B, T, H, hd, inv_sqrt_hd, 0, max_seqlen, m->alibi, 0, stream));
-      SGPT_TRY(sgpt_linear(m->attn, d, lw.w_o, d, lw.b_o, m->resid, d, m->resid, T, d, d, SGPT_EPI_RESID_BF16, stream));
+      SGPT_TRY(quant(m->attn, d));
+      SGPT_TRY(lin(m->attn, d, lw.w_o, fw.w_o, fw.s_o, lw.b_o, m->resid, d, SGPT_EPI_RESID_BF16));
       SGPT_TRY(sgpt_layernorm(m->resid, lw.ln2_g, lw.ln2_b, m->xn, T, d, c.ln_eps, stream));
-      SGPT_TRY(sgpt_linear(m->xn, d, lw.w_fc, d, lw.b_fc, m->ffn, ff, nullptr, T, ff, d, SGPT_EPI_GELU_BF16, stream));
-      SGPT_TRY(sgpt_linear(m->ffn, ff, lw.w_proj, ff, lw.b_proj, m->resid, d, m->resid, T, d, ff,
-                           SGPT_EPI_RESID_BF16, stream));
+      SGPT_TRY(quant(m->xn, d));
+      SGPT_TRY(lin(m->xn, d, lw.w_fc, fw.w_fc, fw.s_fc, lw.b_fc, m->ffn, ff, SGPT_EPI_GELU_BF16));
+      SGPT_TRY(quant(m->ffn, ff));
+      SGPT_TRY(lin(m->ffn, ff, lw.w_proj, fw.w_proj, fw.s_proj, lw.b_proj, m->resid, d, SGPT_EPI_RESID_BF16));
     }
   }
   if (pool_mode == kNoPooling) return SGPT_OK;

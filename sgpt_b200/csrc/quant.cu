@@ -1,6 +1,9 @@
 // Row quantization for int8 corpus shards and their queries (include/sgpt_b200.h sgpt_quantize_rows_i8): one warp per
 // row, two passes over the row (absolute maximum, then quantize and sum the squares; the second pass hits L1/L2).
 // Sign bits for binary corpus shards (sgpt_quantize_rows_b1): one warp per row, one ballot per 32 dimensions.
+// e4m3 rows for the fp8 linear layers (sgpt_quantize_rows_fp8): one warp per row, two passes as for int8.
+#include <cuda_fp8.h>
+
 #include "../../include/sgpt_b200.h"
 #include "common.cuh"
 #include "gemm_api.h"
@@ -121,7 +124,70 @@ __global__ void __launch_bounds__(kQuantThreads) quantize_rows_b1_kernel(const v
   if (lane == 0) popc[row] = count;
 }
 
+// Row of K bf16 -> K e4m3 + one fp32 scale (include/sgpt_b200.h fp8 linear layers).  Lane l handles 4 consecutive
+// elements (one 8-byte load, one 4-byte store) of every 128-element step; the second pass hits L1/L2.
+__global__ void __launch_bounds__(kQuantThreads) quantize_rows_fp8_kernel(const uint16_t* __restrict__ x,
+                                                                           uint8_t* __restrict__ q,
+                                                                           float* __restrict__ scale, long long n,
+                                                                           int K) {
+  pdl_sync();
+  const long long row = static_cast<long long>(blockIdx.x) * kQuantRows + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (row >= n) return;  // warp-uniform
+  const long long base = row * K;
+  float amax = 0.f;
+  bool finite = true;
+  for (int i = 4 * lane; i < K; i += 128) {
+    float v[4];
+    load4(x, 1, base + i, v);
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      finite = finite && isfinite(v[u]);
+      amax = fmaxf(amax, fabsf(v[u]));
+    }
+  }
+  amax = warp_max(amax);
+  finite = __all_sync(0xffffffffu, finite);
+  uint32_t* qr = reinterpret_cast<uint32_t*>(q + base);
+  if (!finite) {  // NaN / inf anywhere: q = 0 and scale = NaN, so every output of the row is NaN
+    for (int i = 4 * lane; i < K; i += 128) qr[i >> 2] = 0u;
+    if (lane == 0) scale[row] = __int_as_float(0x7fc00000);
+    return;
+  }
+  // zero row: inv = 0, q = +-0, scale = 0; inv stays finite even for the tiniest bf16 amax
+  const float inv = amax > 0.f ? fminf(__fdiv_rn(448.0f, amax), 3.40282347e38f) : 0.f;
+  for (int i = 4 * lane; i < K; i += 128) {
+    float v[4];
+    load4(x, 1, base + i, v);
+    const __nv_fp8x2_storage_t lo = __nv_cvt_float2_to_fp8x2(make_float2(__fmul_rn(v[0], inv), __fmul_rn(v[1], inv)),
+                                                             __NV_SATFINITE, __NV_E4M3);
+    const __nv_fp8x2_storage_t hi = __nv_cvt_float2_to_fp8x2(make_float2(__fmul_rn(v[2], inv), __fmul_rn(v[3], inv)),
+                                                             __NV_SATFINITE, __NV_E4M3);
+    qr[i >> 2] = static_cast<uint32_t>(lo) | (static_cast<uint32_t>(hi) << 16);
+  }
+  if (lane == 0) scale[row] = __fdiv_rn(amax, 448.0f);
+}
+
 }  // namespace
+
+extern "C" int sgpt_quantize_rows_fp8(const void* x, void* q_out, float* scale_out, int64_t n, int K,
+                                      sgpt_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  SGPT_REQUIRE(n >= 0, "sgpt_quantize_rows_fp8: bad row count n=%lld", (long long)n);
+  SGPT_REQUIRE(K > 0 && K % 16 == 0, "sgpt_quantize_rows_fp8: K=%d must be a positive multiple of 16", K);
+  if (n == 0) return SGPT_OK;
+  SGPT_REQUIRE(x != nullptr && q_out != nullptr && scale_out != nullptr, "sgpt_quantize_rows_fp8: null argument");
+  SGPT_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(q_out) & 15) == 0 &&
+                   (reinterpret_cast<uintptr_t>(scale_out) & 3) == 0,
+               "sgpt_quantize_rows_fp8: x and q_out must be 16-byte aligned, scale_out 4-byte aligned");
+  const long long blocks = (n + kQuantRows - 1) / kQuantRows;
+  SGPT_REQUIRE(blocks < (1ll << 31), "sgpt_quantize_rows_fp8: too many rows");
+  LaunchScope _ls(kCatMisc, stream);
+  SGPT_CHECK_CUDA(launch_kernel(quantize_rows_fp8_kernel, dim3(static_cast<unsigned>(blocks)), dim3(kQuantThreads), 0,
+                                stream, static_cast<const uint16_t*>(x), static_cast<uint8_t*>(q_out), scale_out,
+                                static_cast<long long>(n), K));
+  return SGPT_OK;
+}
 
 extern "C" int sgpt_quantize_rows_b1(const void* x, int x_bf16, const float* thresholds, void* bits_out,
                                      int32_t* popc_out, int64_t n, int D, sgpt_stream_t stream_) {

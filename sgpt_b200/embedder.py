@@ -66,10 +66,11 @@ class CustomEmbedder:
                  save_emb: bool = False, reinit: bool = False, layeridx: int = -1, method: str = "mean",
                  dataset: str = "scifact", specb: bool = False, maxseqlen: Optional[int] = None, *,
                  config: Optional[ModelConfig] = None, state_dict: Optional[Dict[str, torch.Tensor]] = None,
-                 tokenizer=None, max_tokens: Optional[int] = None, **kwargs):
+                 tokenizer=None, max_tokens: Optional[int] = None, precision: str = "bf16", **kwargs):
         """Keywords up to ``maxseqlen`` are the reference's (BDR:107-120).  ``config``/``state_dict``/``tokenizer`` let a
         caller hand the model over directly (no hub access offline); otherwise they are loaded with HF
-        ``AutoConfig``/``AutoModel``/``AutoTokenizer`` from ``model_name`` exactly like BDR:123,138."""
+        ``AutoConfig``/``AutoModel``/``AutoTokenizer`` from ``model_name`` exactly like BDR:123,138.  ``precision``:
+        ``"bf16"`` or ``"fp8"`` linear layers (Encoder)."""
         if method not in METHODS:
             raise NotImplementedError(f"pooling method {method!r}: built: {METHODS} (poolout needs a pooler head the "
                                       "GPT models of the reference do not have, BDR:303-304)")
@@ -116,7 +117,7 @@ class CustomEmbedder:
         seq_cap = self.max_token_len + (2 if specb else 0)
         self.encoder = Encoder(config, state_dict, device=device,
                                max_tokens=max_tokens or max(batch_size * min(seq_cap, 512), 8192),
-                               max_batch=max(batch_size, 1))
+                               max_batch=max(batch_size, 1), precision=precision)
         self.device = self.encoder.device
 
     # ------------------------------------------------------------------------------------------------------------
@@ -256,7 +257,8 @@ class SentenceEncoder:
     def __init__(self, config: ModelConfig, state_dict: Dict[str, torch.Tensor], tokenizer, device: str = "cuda:0",
                  pooling: str = "weightedmean", max_seq_length: int = 300, batch_capacity: int = 256,
                  max_tokens: Optional[int] = None, position_weights: Optional[torch.Tensor] = None,
-                 heads: Optional[Sequence] = None, asym=None, normalize: bool = False, do_lower_case: bool = False):
+                 heads: Optional[Sequence] = None, asym=None, normalize: bool = False, do_lower_case: bool = False,
+                 precision: str = "bf16"):
         if pooling not in ST_POOLING:
             raise NotImplementedError(f"pooling mode {pooling!r} not in {ST_POOLING}")
         if position_weights is not None and pooling != "weightedmean":
@@ -265,7 +267,8 @@ class SentenceEncoder:
         self.max_seq_length = max_seq_length
         self.do_lower_case = do_lower_case
         self.encoder = Encoder(config, state_dict, device=device,
-                               max_tokens=max_tokens or batch_capacity * max_seq_length, max_batch=batch_capacity)
+                               max_tokens=max_tokens or batch_capacity * max_seq_length, max_batch=batch_capacity,
+                               precision=precision)
         self.device = self.encoder.device
         if position_weights is not None:
             if position_weights.numel() < max_seq_length:
@@ -284,7 +287,8 @@ class SentenceEncoder:
     # ---- construction from a saved sentence-transformers directory -----------------------------------------------
     @classmethod
     def from_spec(cls, spec, tokenizer=None, device: str = "cuda:0", batch_capacity: int = 256,
-                  max_seq_length: Optional[int] = None, max_tokens: Optional[int] = None) -> "SentenceEncoder":
+                  max_seq_length: Optional[int] = None, max_tokens: Optional[int] = None,
+                  precision: str = "bf16") -> "SentenceEncoder":
         """Build from ``st_loader.load_st_directory(path)``; the tokenizer defaults to ``AutoTokenizer`` of the model
         directory (models/Transformer.py:40)."""
         from .heads import AsymHeads, DenseHead
@@ -303,7 +307,8 @@ class SentenceEncoder:
         asym = AsymHeads({k: [mk(d) for d in v] for k, v in spec.asym.items()}) if spec.asym else None
         return cls(spec.config, spec.state_dict, tokenizer, device=device, pooling=spec.pooling, max_seq_length=msl,
                    batch_capacity=batch_capacity, max_tokens=max_tokens, position_weights=spec.position_weights,
-                   heads=heads, asym=asym, normalize=spec.normalize, do_lower_case=spec.do_lower_case)
+                   heads=heads, asym=asym, normalize=spec.normalize, do_lower_case=spec.do_lower_case,
+                   precision=precision)
 
     @classmethod
     def from_pretrained(cls, model_path: str, device: str = "cuda:0", **kwargs) -> "SentenceEncoder":

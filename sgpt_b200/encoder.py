@@ -54,10 +54,17 @@ class Encoder:
     or ``BloomModel`` (``word_embeddings.weight``, ``h.0.self_attention.query_key_value.weight``, ...); a
     ``transformer.`` prefix as in the ``*ForCausalLM`` checkpoints is accepted.  Linear weights are stored in bf16,
     LayerNorm parameters and biases in fp32.
+
+    precision: ``"bf16"`` (default) or ``"fp8"``: every linear layer of every block runs as an e4m3 x e4m3 GEMM with
+    per-output-channel weight scales and per-token activation scales (include/sgpt_b200.h, fp8 linear layers).  The bf16
+    linear weights are quantized on the device by the library and only the e4m3 copies and their scales are kept.
     """
 
     def __init__(self, cfg: ModelConfig, state_dict: Dict[str, torch.Tensor], device="cuda:0", max_tokens: int = 32768,
-                 max_batch: int = 1024):
+                 max_batch: int = 1024, precision: str = "bf16"):
+        if precision not in ("bf16", "fp8"):
+            raise ValueError(f"precision must be 'bf16' or 'fp8', got {precision!r}")
+        self.precision = precision
         self.cfg = cfg
         self.device = torch.device(device)
         if self.device.type != "cuda":
@@ -79,6 +86,24 @@ class Encoder:
         def p16(t):
             return dev(t, torch.bfloat16).data_ptr()
 
+        fp8 = precision == "fp8"
+        fp8_layers = (_lib.Fp8LayerWeightsC * cfg.n_layer)()
+
+        def plin(i, name, t):
+            """Linear weight `name` of layer i: its bf16 device pointer, or with fp8 None after the bf16 values the bf16
+            path would store have been quantized per output channel into fp8_layers[i].w_<name> / s_<name>."""
+            if not fp8:
+                return p16(t)
+            w16 = t.detach().to(device=self.device, dtype=torch.bfloat16).contiguous()
+            q = torch.empty(w16.shape, dtype=torch.uint8, device=self.device)
+            sc = torch.empty(w16.shape[0], dtype=torch.float32, device=self.device)
+            _lib.check(self._lib.sgpt_quantize_rows_fp8(w16.data_ptr(), q.data_ptr(), sc.data_ptr(), w16.shape[0],
+                                                        w16.shape[1], _lib.current_stream()), "sgpt_quantize_rows_fp8")
+            self._keep += [q, sc]
+            setattr(fp8_layers[i], "w_" + name, q.data_ptr())
+            setattr(fp8_layers[i], "s_" + name, sc.data_ptr())
+            return None
+
         with torch.cuda.device(self.device):
             d, H, hd = cfg.d_model, cfg.n_head, cfg.head_dim
             layers = (_lib.LayerWeightsC * cfg.n_layer)()
@@ -92,14 +117,15 @@ class Encoder:
                     p, lw = f"h.{i}.", layers[i]
                     a = p + "attn.attention."
                     lw.ln1_g, lw.ln1_b = p32(p + "ln_1.weight"), p32(p + "ln_1.bias")
-                    lw.w_qkv = p16(torch.cat([sd[a + "q_proj.weight"], sd[a + "k_proj.weight"], sd[a + "v_proj.weight"]], 0))
+                    lw.w_qkv = plin(i, "qkv", torch.cat([sd[a + "q_proj.weight"], sd[a + "k_proj.weight"],
+                                                         sd[a + "v_proj.weight"]], 0))
                     if (a + "q_proj.bias") in sd:
                         lw.b_qkv = dev(torch.cat([sd[a + "q_proj.bias"], sd[a + "k_proj.bias"], sd[a + "v_proj.bias"]], 0),
                                        torch.float32).data_ptr()
-                    lw.w_o, lw.b_o = p16(sd[a + "out_proj.weight"]), p32(a + "out_proj.bias")
+                    lw.w_o, lw.b_o = plin(i, "o", sd[a + "out_proj.weight"]), p32(a + "out_proj.bias")
                     lw.ln2_g, lw.ln2_b = p32(p + "ln_2.weight"), p32(p + "ln_2.bias")
-                    lw.w_fc, lw.b_fc = p16(sd[p + "mlp.c_fc.weight"]), p32(p + "mlp.c_fc.bias")
-                    lw.w_proj, lw.b_proj = p16(sd[p + "mlp.c_proj.weight"]), p32(p + "mlp.c_proj.bias")
+                    lw.w_fc, lw.b_fc = plin(i, "fc", sd[p + "mlp.c_fc.weight"]), p32(p + "mlp.c_fc.bias")
+                    lw.w_proj, lw.b_proj = plin(i, "proj", sd[p + "mlp.c_proj.weight"]), p32(p + "mlp.c_proj.bias")
                     lw.local_attention = 1 if cfg.attention_layers[i] == "local" else 0
                 arch_id = _lib.ARCH_GPT_NEO
             elif cfg.arch == "gptj":  # keys of HF GPTJModel.state_dict(); no attention biases, single LayerNorm per block
@@ -107,11 +133,11 @@ class Encoder:
                 for i in range(cfg.n_layer):
                     p, lw = f"h.{i}.", layers[i]
                     lw.ln1_g, lw.ln1_b = p32(p + "ln_1.weight"), p32(p + "ln_1.bias")
-                    lw.w_qkv = p16(torch.cat([sd[p + "attn.q_proj.weight"], sd[p + "attn.k_proj.weight"],
-                                              sd[p + "attn.v_proj.weight"]], 0))
-                    lw.w_o = p16(sd[p + "attn.out_proj.weight"])
-                    lw.w_fc, lw.b_fc = p16(sd[p + "mlp.fc_in.weight"]), p32(p + "mlp.fc_in.bias")
-                    lw.w_proj, lw.b_proj = p16(sd[p + "mlp.fc_out.weight"]), p32(p + "mlp.fc_out.bias")
+                    lw.w_qkv = plin(i, "qkv", torch.cat([sd[p + "attn.q_proj.weight"], sd[p + "attn.k_proj.weight"],
+                                                         sd[p + "attn.v_proj.weight"]], 0))
+                    lw.w_o = plin(i, "o", sd[p + "attn.out_proj.weight"])
+                    lw.w_fc, lw.b_fc = plin(i, "fc", sd[p + "mlp.fc_in.weight"]), p32(p + "mlp.fc_in.bias")
+                    lw.w_proj, lw.b_proj = plin(i, "proj", sd[p + "mlp.fc_out.weight"]), p32(p + "mlp.fc_out.bias")
                 arch_id = _lib.ARCH_GPTJ
             else:  # bloom: keys of HF BloomModel.state_dict()
                 mw.wte = p16(sd["word_embeddings.weight"])
@@ -123,13 +149,14 @@ class Encoder:
                     # regroup to [q_all | k_all | v_all], the layout the attention kernel reads
                     wq = sd[p + "self_attention.query_key_value.weight"].view(H, 3, hd, d)
                     bq = sd[p + "self_attention.query_key_value.bias"].view(H, 3, hd)
-                    lw.w_qkv = p16(wq.permute(1, 0, 2, 3).reshape(3 * d, d))
+                    lw.w_qkv = plin(i, "qkv", wq.permute(1, 0, 2, 3).reshape(3 * d, d))
                     lw.b_qkv = dev(bq.permute(1, 0, 2).reshape(3 * d), torch.float32).data_ptr()
-                    lw.w_o, lw.b_o = p16(sd[p + "self_attention.dense.weight"]), p32(p + "self_attention.dense.bias")
+                    lw.w_o, lw.b_o = plin(i, "o", sd[p + "self_attention.dense.weight"]), p32(p + "self_attention.dense.bias")
                     lw.ln2_g, lw.ln2_b = (p32(p + "post_attention_layernorm.weight"),
                                           p32(p + "post_attention_layernorm.bias"))
-                    lw.w_fc, lw.b_fc = p16(sd[p + "mlp.dense_h_to_4h.weight"]), p32(p + "mlp.dense_h_to_4h.bias")
-                    lw.w_proj, lw.b_proj = p16(sd[p + "mlp.dense_4h_to_h.weight"]), p32(p + "mlp.dense_4h_to_h.bias")
+                    lw.w_fc, lw.b_fc = plin(i, "fc", sd[p + "mlp.dense_h_to_4h.weight"]), p32(p + "mlp.dense_h_to_4h.bias")
+                    lw.w_proj, lw.b_proj = (plin(i, "proj", sd[p + "mlp.dense_4h_to_h.weight"]),
+                                            p32(p + "mlp.dense_4h_to_h.bias"))
                 arch_id = _lib.ARCH_BLOOM
             mw.lnf_g, mw.lnf_b = p32("ln_f.weight"), p32("ln_f.bias")
             mw.layers = layers
@@ -138,7 +165,12 @@ class Encoder:
                                    vocab=cfg.vocab, max_pos=cfg.max_pos, window=cfg.window, rotary_dim=cfg.rotary_dim,
                                    ln_eps=cfg.ln_eps, max_tokens=self.max_tokens, max_batch=self.max_batch)
             handle = C.c_void_p()
-            _lib.check(self._lib.sgpt_model_create(C.byref(mc), C.byref(mw), C.byref(handle)), "sgpt_model_create")
+            if fp8:
+                self._fp8_layers = fp8_layers
+                _lib.check(self._lib.sgpt_model_create_fp8(C.byref(mc), C.byref(mw), fp8_layers, C.byref(handle)),
+                           "sgpt_model_create_fp8")
+            else:
+                _lib.check(self._lib.sgpt_model_create(C.byref(mc), C.byref(mw), C.byref(handle)), "sgpt_model_create")
             self._handle = handle
         # two pinned staging buffers for [ids | pos | cu] and their device twins: one H2D copy per batch, and the
         # host may pack batch i+1 while the GPU still runs batch i
