@@ -659,6 +659,57 @@ int sgpt_rerank(int dtype, const void* Q, const void* C, const float* q_scale, c
                 int D, int64_t id_base, const int64_t* cand_ids, int64_t kc, int k, float* out_scores,
                 int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Graph index: a fixed-degree, pruned k-NN graph over a stored shard, searched by a beam search (one CTA per query, one
+ * launch per batch).  Positions are local rows of the shard (0 .. n-1); results carry global ids id_base + position.
+ *
+ * sgpt_graph_prune: rank-based detour pruning of k-NN lists, an exact integer contract.
+ *   knn      int32 [n, K] (device): row a lists its candidate neighbours, best first.  An entry outside [0, n), equal to
+ *            a, or equal to an earlier entry of the same row is empty; the others are the row's valid entries.
+ *   detours  for each valid entry i of row a: d_i = #{ j < i : knn[a][j] is valid and knn[a][i] occurs in
+ *            knn[knn[a][j]][0 .. i-1] } (raw entries of that row, valid or not).
+ *   out      int32 [n, degree] (device): the valid entries of row a ordered by (d_i ascending, i ascending), cut to
+ *            degree, padded with -1.
+ *   The counts are integers, so the output does not depend on the order of the atomics that count them.
+ *   SGPT_ERR_INVALID, before any CUDA call, for n outside [0, 2^31), degree not a multiple of 16 in [16, 128], K outside
+ *   [degree, 256] and null pointers.
+ *
+ * sgpt_graph_search: per query, a beam search over graph int32 [n, degree] (device; entries outside [0, n) are empty).
+ *   dtype, Q, C, q_scale, c_scale, D, n and id_base mean what they mean in sgpt_rerank (bf16 and int8 only), and
+ *   s(q, x) is sgpt_rerank's score of query q against position x, bit for bit.  Keys order entries by score descending
+ *   (-0 = +0) and ties by ascending position; scores are never NaN (NaN counts as -1).
+ *   seeds    int32 [nq, num_seeds] (device) of positions, or NULL for hashed seeds.
+ *   mask     shared bitmap of the ALLOWED positions (the format of the masked searches, pitch 0), or NULL.
+ *   out_scores fp32 [nq, k], out_ids int64 [nq, k], out_visited int32 [nq] or NULL (device).
+ *   Per query q (q = its row in this call):
+ *     V = {} (visited), B = [] (entries (s, x, expanded), kept in key order)
+ *     S = seeds[q][0 .. num_seeds-1] (entries outside [0, n) skipped), or, with seeds == NULL,
+ *         S_j = h(seed, q, j) mod n for j < num_seeds, where h is, in uint32 arithmetic (mod 2^32):
+ *           x = seed + 0x9E3779B1 q + 0x85EBCA77 j; x ^= x >> 16; x *= 0x85EBCA6B; x ^= x >> 13; x *= 0xC2B2AE35;
+ *           x ^= x >> 16; h = x
+ *     every x in S not in V: add x to V and score it; B = the best itopk of them, all unexpanded
+ *     for t in 0 .. max_iterations-1:
+ *       P = the first search_width unexpanded entries of B; stop if P is empty; mark them expanded
+ *       every e in graph[p][0 .. degree-1] for p in P with 0 <= e < n and e not in V: add e to V and score it
+ *       B = the best itopk entries of B and the newly scored ones (flags carried)
+ *     output: the first k entries of B whose position the mask allows, as (s, id_base + x); tail (-inf, -1)
+ *     out_visited[q] = |V|
+ *   The result does not depend on the order in which threads insert into V.  Disallowed (deleted) positions are still
+ *   scored and expanded; they are only never returned.  The visited set is an exact table of
+ *   next_pow2(2 (num_seeds + max_iterations search_width degree)) slots in shared memory, never more than half full.
+ *   SGPT_ERR_INVALID, before any CUDA call, for a dtype other than bf16 and int8, nq < 0, the D rules of the dtype,
+ *   n outside [1, 2^31), id_base < 0 or id_base + n > 2^31, itopk not a multiple of 32 in [32, 512], k outside
+ *   [1, itopk], degree < 1, search_width outside [1, 8], search_width x degree > 512, num_seeds outside [1, 512],
+ *   max_iterations < 1 or 2 (num_seeds + max_iterations search_width degree) > 32768, null Q, C, graph, out_scores or
+ *   out_ids, and an unaligned Q or C.
+ * ------------------------------------------------------------------------------------------------------------------ */
+int sgpt_graph_prune(const int32_t* knn, int64_t n, int K, int degree, int32_t* out, sgpt_stream_t stream);
+int sgpt_graph_search(int dtype, const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq,
+                      int64_t n, int D, int64_t id_base, const int32_t* graph, int degree, const int32_t* seeds,
+                      int num_seeds, uint32_t seed, int itopk, int search_width, int max_iterations, int k,
+                      const uint32_t* mask, float* out_scores, int64_t* out_ids, int32_t* out_visited,
+                      sgpt_stream_t stream);
+
 /* bf16 -> fp32 conversion of count elements (count % 4 == 0), e.g. of the residual stream. */
 int sgpt_bf16_to_f32(const void* x, float* y, int64_t count, sgpt_stream_t stream);
 

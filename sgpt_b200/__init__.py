@@ -14,7 +14,7 @@ from .config import ModelConfig, preset  # noqa: F401
 
 __all__ = ["ModelConfig", "preset", "Encoder", "CustomEmbedder", "SentenceEncoder", "SentenceBERTBOSEOS",
            "SentenceBERTAsym", "DenseRetrievalExactSearch", "CorpusShard", "merge_topk", "semantic_search",
-           "merge_topk_packed", "unpack_topk", "pack_mask", "IVFIndex", "IVFPQIndex", "sharded_search", "PeerGather", "ShardedDenseRetrievalExactSearch", "DenseHead", "AsymHeads", "load_st_directory", "GenericDataLoader", "EvaluateRetrieval",
+           "merge_topk_packed", "unpack_topk", "pack_mask", "IVFIndex", "IVFPQIndex", "GraphIndex", "sharded_search", "PeerGather", "ShardedDenseRetrievalExactSearch", "DenseHead", "AsymHeads", "load_st_directory", "GenericDataLoader", "EvaluateRetrieval",
            "InformationRetrievalEvaluator", "paraphrase_mining", "paraphrase_mining_embeddings", "community_detection"]
 
 
@@ -49,6 +49,9 @@ def __getattr__(name):  # lazy: torch / CUDA pieces are imported on first use
     if name == "IVFPQIndex":
         from .ivfpq import IVFPQIndex
         return IVFPQIndex
+    if name == "GraphIndex":
+        from .graph import GraphIndex
+        return GraphIndex
     if name in ("paraphrase_mining", "paraphrase_mining_embeddings", "community_detection"):
         from . import mining
         return getattr(mining, name)

@@ -18,6 +18,7 @@
 #include "gemm_api.h"
 #include "host_utils.h"
 #include "ivf.cuh"
+#include "rerank.cuh"
 #include "topk.cuh"
 
 using namespace sgpt;
@@ -298,36 +299,7 @@ __global__ void __launch_bounds__(kThreads) rerank_kernel(const uint8_t* __restr
   const uint4* qp = reinterpret_cast<const uint4*>(Q + q * row_bytes);
   const uint4* cp = reinterpret_cast<const uint4*>(C + row * row_bytes);
   const int units = static_cast<int>(row_bytes / 16);
-  float x;
-  if constexpr (kS8) {
-    int acc = 0;  // exact: |sum| <= 65536 x 128 x 128
-    for (int u = lane; u < units; u += 32) {
-      const uint4 a = __ldg(qp + u), b = __ldg(cp + u);
-      acc = __dp4a(static_cast<int>(a.x), static_cast<int>(b.x), acc);
-      acc = __dp4a(static_cast<int>(a.y), static_cast<int>(b.y), acc);
-      acc = __dp4a(static_cast<int>(a.z), static_cast<int>(b.z), acc);
-      acc = __dp4a(static_cast<int>(a.w), static_cast<int>(b.w), acc);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-    x = __int2float_rn(acc);
-  } else {
-    // lane l: 16-byte units l, l + 32, ... in order, the 8 elements of a unit in order; every bf16 x bf16 product is exact
-    // in fp32, so fmaf adds it with one rounding.  Then the xor butterfly over the lanes (offsets 16, 8, 4, 2, 1): lanes
-    // i and i ^ o add the same two values, so every lane ends with the same sum
-    float acc = 0.f;
-    auto dot2 = [](uint32_t a, uint32_t b, float s) {
-      return fmaf(bf16_hi(a), bf16_hi(b), fmaf(bf16_lo(a), bf16_lo(b), s));
-    };
-#pragma unroll 2
-    for (int u = lane; u < units; u += 32) {
-      const uint4 a = __ldg(qp + u), b = __ldg(cp + u);
-      acc = dot2(a.w, b.w, dot2(a.z, b.z, dot2(a.y, b.y, dot2(a.x, b.x, acc))));
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-    x = acc;
-  }
+  float x = rerank_dot<kS8>(qp, cp, units, lane);
   // the filter epilogue's order: (acc * q_scale) * c_scale, NaN -> -1
   x = x * (q_scale != nullptr ? __ldg(q_scale + q) : 1.f) * (c_scale != nullptr ? __ldg(c_scale + row) : 1.f);
   x = (x != x) ? -1.f : x;

@@ -25,16 +25,6 @@
 
 namespace sgpt {
 
-// -0.0 takes the key of +0.0: equal scores, so their order is decided by the ids like any other tie
-__device__ __forceinline__ uint32_t score_key(float x) {
-  uint32_t u = __float_as_uint(x);
-  u = (u == 0x80000000u) ? 0u : u;
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float key_score(uint32_t k) {
-  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-
 struct Elem {
   uint32_t key;  // 0 = invalid / empty
   long long id;
