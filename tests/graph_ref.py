@@ -1,5 +1,6 @@
 """numpy restatement of the graph index (include/sgpt_b200.h sgpt_graph_prune / sgpt_graph_search and
-sgpt_b200.graph.merge_reverse), written from the documented definitions, for tests to compare against bit for bit."""
+sgpt_b200.graph.merge_reverse / self_knn), written from the documented definitions, for tests to compare against bit for
+bit."""
 import numpy as np
 
 M32 = 0xFFFFFFFF
@@ -59,6 +60,41 @@ def merge(pruned: np.ndarray) -> np.ndarray:
         row = row[:degree]
         out[a, :len(row)] = row
     return out
+
+
+def self_knn(table: np.ndarray, K: int, allowed=None, id_base: int = 0) -> np.ndarray:
+    """sgpt_b200.graph.self_knn from table fp32 [n, n] (table[a, x] = the exact search's score of row a's stored vector
+    against position x): the exact top-(K + 1) of the allowed positions by (score descending, position ascending), tail
+    -1; then row a's own id removed, or the last entry dropped when a is not among them.  Global ids int64 [n, K]."""
+    n = table.shape[0]
+    cand = np.arange(n) if allowed is None else np.nonzero(allowed)[0]
+    out = np.full((n, K), -1, dtype=np.int64)
+    for a in range(n):
+        top = cand[np.lexsort((cand, -table[a, cand].astype(np.float64)))][:K + 1].tolist()  # -0 == +0
+        top = [x for x in top if x != a][:K]
+        out[a, :len(top)] = np.asarray(top, dtype=np.int64) + id_base
+    return out
+
+
+def score_table(score_block, nq: int, n: int, id_base: int = 0, block: int = 4096) -> np.ndarray:
+    """The table fp32 [nq, n] that drives `search`, from a top-m scorer of at most `block` candidates per call:
+    score_block(global ids int64 [m]) -> (scores [nq, m], global ids [nq, m]) in any order.  A candidate's score does not
+    depend on the other candidates, so blocks of ids give the table of one call over all n.  Every position must come
+    back exactly once per query; NaN counts as -1."""
+    table = np.full((nq, n), np.nan, dtype=np.float32)
+    seen = np.zeros((nq, n), dtype=np.int64)
+    rows = np.arange(nq)[:, None]
+    for c in range(0, n, block):
+        m = min(block, n - c)
+        s, i = score_block(np.arange(c, c + m, dtype=np.int64) + id_base)
+        i = np.asarray(i, dtype=np.int64) - id_base
+        if i.shape != (nq, m) or not ((i >= c) & (i < c + m)).all():
+            raise AssertionError(f"block [{c}, {c + m}) came back with ids outside it")
+        table[rows, i] = np.asarray(s, dtype=np.float32)
+        np.add.at(seen, (np.broadcast_to(rows, i.shape), i), 1)
+    if not (seen == 1).all():
+        raise AssertionError("a position was scored more or less than once")
+    return np.where(np.isnan(table), np.float32(-1), table)
 
 
 def seed_hash(seed: int, q: int, j: int) -> int:

@@ -19,13 +19,21 @@ _DUMMY = np.zeros(64, dtype=np.int64)
 P = _DUMMY.ctypes.data  # 16-byte aligned host memory, never dereferenced: every call below is rejected first
 
 
-@pytest.mark.parametrize("n,K,x,message", [
+QUANTIZE_REJECTIONS = [
     (4, 24, P, b"K=24 must be a positive multiple of 16"),
     (4, 0, P, b"K=0 must be a positive multiple of 16"),
     (-1, 16, P, b"bad row count"),
     (4, 16, None, b"null argument"),
     (4, 16, P + 8, b"16-byte aligned"),
-])
+]
+
+
+def _quantize_case_id(n, K, x, message):
+    """The pointer as an offset from P: P itself is a heap address, which differs from one process to the next."""
+    return f"{n}-{K}-{'None' if x is None else f'P+{x - P}'}-{message.decode()}"
+
+
+@pytest.mark.parametrize("n,K,x,message", QUANTIZE_REJECTIONS, ids=[_quantize_case_id(*c) for c in QUANTIZE_REJECTIONS])
 def test_quantize_rows_fp8_rejects_bad_arguments(n, K, x, message):
     lib = _lib()
     assert lib.sgpt_quantize_rows_fp8(x, P, P, n, K, None) == 1

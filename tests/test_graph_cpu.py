@@ -248,3 +248,43 @@ def test_restated_prune_and_merge_on_a_hand_worked_case():
 def test_seed_hash_is_32_bit():
     vals = {graph_ref.seed_hash(s, q, j) for s in (0, 7) for q in range(20) for j in range(50)}
     assert len(vals) == 2000 and max(vals) < 2 ** 32
+
+
+def test_restated_self_knn_ties_own_id_and_deletions():
+    # rows 0-4 are copies of one vector (all score 3 against each other), row 5 is another (score 1 against the copies,
+    # 5 against itself); position 2 is deleted
+    t = np.array([[3, 3, 3, 3, 3, 1]] * 5 + [[1, 1, 1, 1, 1, 5]], dtype=np.float32)
+    t[0, 5] = -0.0  # -0 ties with +0, broken by position
+    allowed = np.array([True, True, False, True, True, True])
+    got = graph_ref.self_knn(t, 2, allowed, id_base=100)
+    # top-3 of row 0 over {0, 1, 3, 4, 5}: 0, 1, 3 -> own id 0 removed
+    assert got[0].tolist() == [101, 103]
+    # row 2 is deleted, so it is absent from its own top-3 {0, 1, 3}: the last entry is dropped
+    assert got[2].tolist() == [100, 101]
+    # row 5: its own id first, then the copies by position
+    assert got[5].tolist() == [100, 101]
+    full = graph_ref.self_knn(t, 4, None)
+    assert full[4].tolist() == [0, 1, 2, 3]  # the row is the 5th of its ties: removed from the top-5
+    few = graph_ref.self_knn(t, 5, np.array([True, False, False, False, False, True]))
+    assert few[0].tolist() == [5, -1, -1, -1, -1]  # fewer than K + 1 allowed: tail -1
+
+
+def test_score_table_from_blocks_of_top_k():
+    g = np.random.default_rng(3)
+    nq, n, base = 3, 30, 50
+    want = g.integers(-3, 4, (nq, n)).astype(np.float32)
+    want[1, 4] = np.nan
+    want[2, 9] = -np.inf
+
+    def top_m(ids, shift=0):
+        s = want[:, ids - base]
+        order = np.lexsort((np.broadcast_to(ids, s.shape), -np.nan_to_num(s, nan=-1)), axis=-1)
+        return np.take_along_axis(s, order, 1), ids[order] + shift
+
+    got = graph_ref.score_table(top_m, nq, n, id_base=base, block=7)
+    assert np.array_equal(got, np.where(np.isnan(want), np.float32(-1), want))
+    with pytest.raises(AssertionError, match="outside"):
+        graph_ref.score_table(lambda ids: top_m(ids, 1), nq, n, id_base=base, block=7)
+    with pytest.raises(AssertionError, match="more or less than once"):
+        graph_ref.score_table(lambda ids: (want[:, ids - base], np.broadcast_to(ids[:1], (nq, len(ids)))), nq, n,
+                              id_base=base, block=7)
