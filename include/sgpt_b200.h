@@ -702,6 +702,29 @@ int sgpt_rerank(int dtype, const void* Q, const void* C, const float* q_scale, c
  *   [1, itopk], degree < 1, search_width outside [1, 8], search_width x degree > 512, num_seeds outside [1, 512],
  *   max_iterations < 1 or 2 (num_seeds + max_iterations search_width degree) > 32768, null Q, C, graph, out_scores or
  *   out_ids, and an unaligned Q or C.
+ *
+ * sgpt_graph_search_filtered: sgpt_graph_search with a filter, shared or per query, in the mask format of the masked
+ *   searches: mask_pitch_words = 0: one bitmap [ceil(n/32)] of the ALLOWED positions, or NULL (every position allowed);
+ *   mask_pitch_words >= ceil(n/32): one bitmap per query, [nq][pitch].  Bits at or past n are ignored.
+ *   The walk does not see the mask: V, B, every P, the stopping rule and out_visited are exactly those of
+ *   sgpt_graph_search with the same arguments, and disallowed positions are still scored and expanded.
+ *     output: the best k entries of {x in V : the mask allows x for query q} in key order (score descending, ties by
+ *     ascending position), as (s, id_base + x), s bit for bit sgpt_rerank's score; tail (-inf, -1)
+ *   The final B is the top-itopk of V, so with a NULL or all-ones mask the output equals sgpt_graph_search's with
+ *   mask = NULL, bit for bit.  A tail (-inf, -1) means V holds fewer than k allowed positions, not that the shard does.
+ *   The best k allowed keys are kept in next_pow2(k + max(num_seeds, search_width degree)) further 8-byte slots of shared
+ *   memory (at most 8 KB).  SGPT_ERR_INVALID, before any CUDA call, for every rejection of sgpt_graph_search and, as in
+ *   the masked searches, a negative pitch, 0 < pitch < ceil(n/32) and a non-zero pitch with a NULL mask.
+ *
+ * sgpt_graph_prune_append: the detour pruning of m rows appended to a graph over n_old rows, for rows a = n_old + r,
+ *   r < m.  Row a's list is L = knn[r] (int32 [m, K], device, local positions); an entry is empty if it lies outside
+ *   [0, n_old + m), equals a, or repeats an earlier entry of L.  The list of a position b is graph[b][0 .. degree-1]
+ *   (int32 [n_old, degree], device) for b < n_old and knn[b - n_old] for b >= n_old.  d_i = #{ j < i : L[j] is valid and
+ *   L[i] occurs in list(L[j])[0 .. i-1] } (raw entries); out[r] (int32 [m, degree], device) holds the valid entries of
+ *   L ordered by (d_i ascending, i ascending), cut to degree, padded with -1.  One CTA per new row; the old rows are
+ *   never launched over.  With n_old = 0 (graph may then be NULL) this is exactly sgpt_graph_prune of knn.
+ *   SGPT_ERR_INVALID, before any CUDA call, for a negative n_old or m, n_old + m >= 2^31, degree not a multiple of 16 in
+ *   [16, 128], K outside [degree, 256], a null graph with n_old > 0, and a null knn or out.
  * ------------------------------------------------------------------------------------------------------------------ */
 int sgpt_graph_prune(const int32_t* knn, int64_t n, int K, int degree, int32_t* out, sgpt_stream_t stream);
 int sgpt_graph_search(int dtype, const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq,
@@ -709,6 +732,13 @@ int sgpt_graph_search(int dtype, const void* Q, const void* C, const float* q_sc
                       int num_seeds, uint32_t seed, int itopk, int search_width, int max_iterations, int k,
                       const uint32_t* mask, float* out_scores, int64_t* out_ids, int32_t* out_visited,
                       sgpt_stream_t stream);
+int sgpt_graph_search_filtered(int dtype, const void* Q, const void* C, const float* q_scale, const float* c_scale,
+                               int nq, int64_t n, int D, int64_t id_base, const int32_t* graph, int degree,
+                               const int32_t* seeds, int num_seeds, uint32_t seed, int itopk, int search_width,
+                               int max_iterations, int k, const uint32_t* mask, int64_t mask_pitch_words,
+                               float* out_scores, int64_t* out_ids, int32_t* out_visited, sgpt_stream_t stream);
+int sgpt_graph_prune_append(const int32_t* graph, int64_t n_old, int degree, const int32_t* knn, int64_t m, int K,
+                            int32_t* out, sgpt_stream_t stream);
 
 /* bf16 -> fp32 conversion of count elements (count % 4 == 0), e.g. of the residual stream. */
 int sgpt_bf16_to_f32(const void* x, float* y, int64_t count, sgpt_stream_t stream);

@@ -118,6 +118,9 @@ _SIGNATURES = {
     "sgpt_graph_prune": (i32, [vp, i64, i32, i32, vp, vp]),
     "sgpt_graph_search": (i32, [i32, vp, vp, vp, vp, i32, i64, i32, i64, vp, i32, vp, i32, C.c_uint32, i32, i32, i32,
                                 i32, vp, vp, vp, vp, vp]),
+    "sgpt_graph_search_filtered": (i32, [i32, vp, vp, vp, vp, i32, i64, i32, i64, vp, i32, vp, i32, C.c_uint32, i32,
+                                         i32, i32, i32, vp, i64, vp, vp, vp, vp]),
+    "sgpt_graph_prune_append": (i32, [vp, i64, i32, vp, i64, i32, vp, vp]),
     "sgpt_quantize_rows_b1": (i32, [vp, i32, vp, vp, vp, i64, i32, vp]),
     "sgpt_quantize_rows_fp8": (i32, [vp, vp, vp, i64, i32, vp]),
     "sgpt_linear_fp8": (i32, [vp, i64, vp, vp, i64, vp, vp, vp, i64, vp, i32, i32, i32, i32, vp]),
