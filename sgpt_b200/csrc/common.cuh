@@ -114,6 +114,34 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Thread-block clusters
+// ---------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// Every non-exited thread of every CTA of the cluster arrives (release) and waits (acquire).  Not .aligned: the threads
+// of a warp may reach it from different places.
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// shared::cta address of this CTA -> the shared::cluster address of the same offset in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
+  uint32_t r;
+  asm("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+  return r;
+}
+// Arrive on an mbarrier of any CTA of the cluster (a shared::cluster address from mapa_shared), with the default
+// .release.cta semantics.  For a consumer releasing a ring stage that is enough: the reads it orders are wgmma operand
+// reads that wgmma.wait_group has already completed, and the writes they guard are TMA loads the partner's producer
+// issues only after it has seen the barrier's phase flip.  .release.cluster would put a MEMBAR.GPU after every
+// arrive, which stalls the issuing warp for the wgmma group still in flight.
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+}
+
 // generic-proxy writes to smem -> visible to the async proxy (TMA stores / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -131,6 +159,18 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* d
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       :
       : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+      : "memory");
+}
+// The same box written to the same shared-memory offset of every CTA in `cta_mask` (bit r = cluster rank r), each
+// destination's copy signalling the mbarrier at `bar`'s offset in that CTA with its bytes.
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* desc, uint64_t* bar, int c0,
+                                                      int c1, uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;"
+      :
+      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
+        "h"(cta_mask)
       : "memory");
 }
 // L2 cache-hinted variant (createpolicy-encoded 64-bit hints as used by the driver's canonical policies).

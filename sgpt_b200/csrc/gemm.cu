@@ -69,19 +69,45 @@ static int launch_linear(const void* x, int64_t ldx, const void* w, int64_t ldw,
   int rc = make_map(&ta, x, static_cast<uint64_t>(M), static_cast<uint64_t>(K), static_cast<uint64_t>(ldx), kGemmBM,
                     box_k);
   if (rc != SGPT_OK) return rc;
-  rc = make_map(&tb, w, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldw), kLinBN, box_k);
+  // each CTA of a cluster loads one half of the weight tile's rows and multicasts it to both
+  rc = make_map(&tb, w, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldw), LinearCfg::kBRows,
+                box_k);
   if (rc != SGPT_OK) return rc;
   auto kern = gemm_linear_kernel<Op, kOp>;
   static PerDeviceOnce attr_once;
   if (attr_once.first()) {
     SGPT_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, LinearCfg::kSmemBytes));
   }
-  const long long units = static_cast<long long>((M + kGemmBM - 1) / kGemmBM) * ((N + kLinBN - 1) / kLinBN) * ksplit;
+  // The persistent grid is as many clusters as can be resident at once: GPC sizes can leave fewer than sm_count() / 2
+  // pairs of SMs for two-CTA clusters.  Cached per device.
+  static int max_clusters[64] = {};
+  int dev = 0;
+  SGPT_CHECK_CUDA(cudaGetDevice(&dev));
+  SGPT_REQUIRE(dev >= 0 && dev < 64, "launch_linear: device %d out of range", dev);
+  if (max_clusters[dev] == 0) {
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = kLinCluster;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(static_cast<unsigned>(kLinCluster * sm_count()));
+    cfg.blockDim = dim3(kLinThreads);
+    cfg.dynamicSmemBytes = LinearCfg::kSmemBytes;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    int n = 0;
+    SGPT_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
+    SGPT_REQUIRE(n > 0, "launch_linear: no %d-CTA cluster of the linear-layer GEMM fits on device %d", kLinCluster, dev);
+    max_clusters[dev] = n;  // benign race: every thread writes the same value
+  }
+  const int m_pairs = ((M + kGemmBM - 1) / kGemmBM + kLinCluster - 1) / kLinCluster;
+  const long long units = static_cast<long long>(m_pairs) * ((N + kLinBN - 1) / kLinBN) * ksplit;  // pair units
   if (units == 0) return SGPT_OK;
-  const long long ctas = units < sm_count() ? units : sm_count();
+  const long long clusters = units < max_clusters[dev] ? units : max_clusters[dev];
   LaunchScope _ls(kCatGemm, stream);
-  SGPT_CHECK_CUDA(launch_kernel(kern, dim3(static_cast<unsigned>(ctas)), dim3(kLinThreads), LinearCfg::kSmemBytes, stream,
-                                ta, tb, M, N, K, p, tm));
+  SGPT_CHECK_CUDA(launch_kernel_cluster(kern, dim3(static_cast<unsigned>(kLinCluster * clusters)), dim3(kLinThreads),
+                                        LinearCfg::kSmemBytes, stream, kLinCluster, ta, tb, M, N, K, p, tm));
   return SGPT_OK;
 }
 
@@ -336,11 +362,11 @@ extern "C" int sgpt_linear(const void* x, int64_t ldx, const void* w, int64_t ld
       OpTmaResidAddBF16::Params p{om, bias};
       return launch_linear<OpTmaResidAddBF16>(x, ldx, w, ldw, M, N, K, p, stream, pick_ksplit(K));
     }
-    case 100:
-    case 101: {  // profiling aids: the mainloop and the fp32 accumulator hand-over alone (100) / + its read-back (101)
+    case 100:  // profiling aid: gemm_linear_kernel without its global stores (the product kernel's mainloop and epilogue)
+      return launch_linear<OpNoStoreBF16>(x, ldx, w, ldw, M, N, K, {0}, stream);
+    case 101: {  // profiling aid: gemm_bf16_tn_kernel's mainloop, fp32 accumulator hand-over and read-back
       TileMap tm;
       tm.band = pick_band(M, N, K);
-      if (epilogue == 100) return launch_gemm<128, EpiDebugNull<false>>(x, ldx, w, ldw, M, N, K, {0}, stream, kCatGemm, tm);
       return launch_gemm<128, EpiDebugNull<true>>(x, ldx, w, ldw, M, N, K, {0}, stream, kCatGemm, tm);
     }
     default:

@@ -359,15 +359,24 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
 // ---------------------------------------------------------------------------------------------------------------
 // Linear-layer GEMM: out[M,N] (bf16) = Op(A[M,K] B[N,K]^T), written by TMA as a tensor store or a reduce-add.
 //
-// Roles (3 warpgroups = 384 threads, 1 CTA per SM):
+// Roles (3 warpgroups = 384 threads, 1 CTA per SM, clusters of 2 CTAs):
 //   warpgroup 0      TMA producer (one lane), lowered to 40 registers per thread (setmaxnreg.dec)
 //   warpgroups 1, 2  consumers, raised to 232 registers per thread (setmaxnreg.inc).  Consumer c takes work units
 //                    c, c + 2, c + 4, ... of the CTA's sequence and computes each whole 128 x 128 tile (two m64n128k16
 //                    per K step, 128 fp32 accumulators per thread), then runs its epilogue.
+// Cluster pairing: a work unit is a pair of vertically adjacent M-tiles on one N-tile (and one K slice with split-K);
+// cluster rank r computes M-tile 2 mp + r of pair mp, and both CTAs walk the same unit sequence and k-blocks, which is
+// all that keeps their rings in step.  Per k-block each producer loads its own A box (128 x 64) and one 64-row half of
+// the shared B tile, multicast into the same stage of both CTAs: 24 KB of L2 reads per CTA instead of 32 KB.  A stage
+// therefore holds bytes written by both producers, and it is refilled only once the owning consumer of BOTH CTAs has
+// read it: its empty barrier takes 8 arrivals, each consumer warp arriving on its own CTA's barrier and on the
+// partner's.  With an odd number of M-tiles, rank 1 of the last pair loads a box wholly past M (TMA zero fill, its full
+// byte count) and stores nothing, but takes part in every load, multicast and barrier like any other unit.  No CTA
+// leaves before the final cluster barrier: its partner may still multicast into its shared memory or arrive on its
+// barriers until then.
 // Ping-pong: once a consumer has issued its last k-block it arrives at the other consumer's turn barrier, so one
 // consumer's mainloop runs while the other runs its epilogue (kBarTurn + c, 256 threads: every arrive is matched by the
-// one wait of the next unit).  The producer walks the same unit sequence (TileMap banding, split-K); each ring stage is
-// read by the one consumer that owns the unit, so it is released by 4 arrivals, one per warp of that warpgroup.
+// one wait of the next unit).  The producer walks the same unit sequence (TileMap banding over pair units, split-K).
 // Epilogue: Op::pair maps each fp32 accumulator pair to two bf16 in registers; the words go to the consumer's own 32 KB
 // output tile (8 SWIZZLE_128B boxes of 32 rows x 64 columns, the box of the output tensor map) and one thread hands the
 // boxes to the TMA engine.  The tile is rewritten only once the previous tile's stores have read it (wait_group.read),
@@ -376,15 +385,20 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int kLinThreads = 384;
 constexpr int kLinBN = 128;
+constexpr int kLinCluster = 2;  // CTAs per cluster: two M-tiles sharing each weight tile
 struct LinearCfg {
   static constexpr int kABytes = kGemmBM * kGemmBK * 2;
+  static constexpr int kBRows = kLinBN / kLinCluster;                 // B rows each CTA loads and multicasts
+  static constexpr int kBPartBytes = kBRows * kGemmBK * 2;            // 8 KB
   static constexpr int kStageBytes = kABytes + kLinBN * kGemmBK * 2;  // 32 KB
-  static constexpr int kStages = 4;
+  static constexpr int kStages = 5;  // 5 x 32 KB: measured faster than 4 with the cluster pairing (DESIGN.md)
   static constexpr int kOutBytes = kGemmBM * kLinBN * 2;              // one consumer's bf16 output tile
   static constexpr int kBarrierBytes = 512;
   // smem: [<=1024 align slack][stages * (A|B)][2 output tiles][barriers]
   static constexpr int kSmemBytes = 1024 + kStages * kStageBytes + 2 * kOutBytes + kBarrierBytes;
   static_assert(kSmemBytes <= 232448, "exceeds the 227 KB per-CTA shared memory limit");
+  // the B parts stack into the layout of one 128-row SWIZZLE_128B box (the swizzle repeats every 8 rows = 1 KB)
+  static_assert(kBPartBytes % 1024 == 0 && kBPartBytes * kLinCluster == kLinBN * kGemmBK * 2, "B tile split");
 };
 // named barriers of gemm_linear_kernel (0 is __syncthreads): all consumers; turn of consumer c; epilogue of consumer c
 constexpr int kBarConsumers = 1, kBarTurn = 2, kBarEpi = 4;
@@ -410,23 +424,30 @@ gemm_linear_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
   uint64_t* empty_bar = full_bar + kStages;
   uint64_t* probe = empty_bar + kStages;  // clock probe: start cycle and time (kept out of the consumers' registers)
 
+  const int rank = static_cast<int>(cluster_ctarank());  // M-tile of the pair this CTA computes
+  const int cid = blockIdx.x / kLinCluster, ncl = gridDim.x / kLinCluster;  // cluster / number of clusters
   const int m_tiles = (M + kGemmBM - 1) / kGemmBM;
+  const int m_pairs = (m_tiles + kLinCluster - 1) / kLinCluster;
   const int n_tiles = (N + kLinBN - 1) / kLinBN;
   const int ksplit = tmap.ksplit;
-  const int num_units = m_tiles * n_tiles * ksplit;
+  const int num_units = m_pairs * n_tiles * ksplit;
   const int num_kb = (K + kBK - 1) / kBK;
   const int kb_per = (num_kb + ksplit - 1) / ksplit;  // k-blocks per slice (the host keeps every slice non-empty)
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tma_a);
     tma_prefetch_desc(&tma_b);
+    // full: the local producer's arrive.expect_tx (the bytes come from both producers)
+    // empty: one arrive per warp of the stage's consumer, in this CTA and in the partner
+    constexpr uint32_t kFullArrivals = 1, kEmptyArrivals = 4 * kLinCluster;
+    static_assert(kEmptyArrivals == 8, "4 local + 4 remote consumer warps release a stage");
     for (int i = 0; i < kStages; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 4);  // one arrive per warp of the consumer that owns the stage's unit
+      mbar_init(&full_bar[i], kFullArrivals);
+      mbar_init(&empty_bar[i], kEmptyArrivals);
     }
     fence_mbar_init();
   }
-  __syncthreads();
+  cluster_sync();  // both CTAs' barriers are initialised before any multicast or remote arrive can reach them
   pdl_sync();  // everything above overlapped the previous kernel's tail; global memory is touched only below
 
   if (threadIdx.x < 128) {
@@ -435,21 +456,24 @@ gemm_linear_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
+      for (int unit = cid; unit < num_units; unit += ncl) {
         const int tile = unit / ksplit, ks = unit - tile * ksplit;
-        int mg, nt;
-        tmap.coords(tile, m_tiles, n_tiles, mg, nt);
+        int mp, nt;
+        tmap.coords(tile, m_pairs, n_tiles, mp, nt);
+        const int m0 = (kLinCluster * mp + rank) * kGemmBM, nb = nt * kLinBN + rank * Cfg::kBRows;
         const int kb_end = min(num_kb, (ks + 1) * kb_per);
         for (int kb = ks * kb_per; kb < kb_end; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
+          mbar_wait(&empty_bar[stage], phase ^ 1);  // read by the owning consumer of both CTAs
           uint8_t* sa = smem_tiles + stage * Cfg::kStageBytes;
           mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-          tma_load_2d(sa, &tma_a, &full_bar[stage], kb * kBK, mg * kGemmBM);
-          tma_load_2d(sa + Cfg::kABytes, &tma_b, &full_bar[stage], kb * kBK, nt * kLinBN);
+          tma_load_2d(sa, &tma_a, &full_bar[stage], kb * kBK, m0);
+          tma_load_2d_multicast(sa + Cfg::kABytes + rank * Cfg::kBPartBytes, &tma_b, &full_bar[stage], kb * kBK, nb,
+                                (1u << kLinCluster) - 1);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
     }
+    cluster_sync();
     return;
   }
 
@@ -466,10 +490,15 @@ gemm_linear_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
     probe[0] = static_cast<uint64_t>(clock64());
     probe[1] = global_timer_ns();
   }
+  // a stage is released on this CTA's empty barrier and on the partner's (its B part came from there)
+  auto release = [&](int s) {
+    mbar_arrive(&empty_bar[s]);
+    mbar_arrive_cluster(mapa_shared(smem_u32(&empty_bar[s]), cluster_ctarank() ^ 1u));
+  };
   int stage = 0;
   uint32_t phase = 0;
-  int i = 0;  // position of the unit in this CTA's sequence
-  for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x, ++i) {
+  int i = 0;  // position of the unit in this cluster's sequence
+  for (int unit = cid; unit < num_units; unit += ncl, ++i) {
     const int tile = unit / ksplit, ks = unit - tile * ksplit;
     const int kb_begin = ks * kb_per, kb_end = min(num_kb, kb_begin + kb_per);
     if ((i & 1) != c) {  // the other consumer's unit: step over its k-blocks in the ring
@@ -507,19 +536,19 @@ gemm_linear_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
       wgmma_fence_acc(acc1);
       // one k-block stays in flight: the stage of the PREVIOUS k-block has been read once its group completed
       wgmma_wait<1>();
-      if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+      if (prev_stage >= 0 && lane == 0) release(prev_stage);
       prev_stage = stage;
       if (++stage == kStages) { stage = 0; phase ^= 1; }
     }
-    if (unit + static_cast<int>(gridDim.x) < num_units) named_bar_arrive(kBarTurn + (c ^ 1), 256);
+    if (unit + ncl < num_units) named_bar_arrive(kBarTurn + (c ^ 1), 256);
     wgmma_wait<0>();
     wgmma_fence_acc(acc0);
     wgmma_fence_acc(acc1);
-    if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+    if (prev_stage >= 0 && lane == 0) release(prev_stage);
 
-    int mg, nt;
-    tmap.coords(tile, m_tiles, n_tiles, mg, nt);
-    const int m0 = mg * kGemmBM, n0 = nt * kLinBN;
+    int mp, nt;
+    tmap.coords(tile, m_pairs, n_tiles, mp, nt);
+    const int m0 = (kLinCluster * mp + rank) * kGemmBM, n0 = nt * kLinBN;
     // epilogue: all results are computed before any is stored, so the loads inside Op::rows / Op::col / Op::pair are
     // ordinary loads the compiler batches up front (the volatile smem stores would otherwise fence them apart)
     typename Op::Rows rw;
@@ -565,6 +594,7 @@ gemm_linear_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
     atomicAdd(&g_gemm_clock[0], static_cast<unsigned long long>(clock64()) - probe[0]);
     atomicAdd(&g_gemm_clock[1], static_cast<unsigned long long>(global_timer_ns()) - probe[1]);
   }
+  cluster_sync();  // the partner's last multicasts into this CTA and arrives on its barriers are over
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -605,6 +635,22 @@ struct OpTmaBiasActBF16 {
   static __device__ __forceinline__ void issue(const Params& p, const void* box, int n, int m0) {
     tma_store_2d(&p.out_map, box, n, m0);
   }
+};
+
+// Profiling aid (sgpt_linear epilogue 100): the whole kernel, epilogue arithmetic and output-tile writes included, but no
+// stores to global memory, so that the product time minus this time is what the stores cost on the same kernel.
+struct OpNoStoreBF16 {
+  struct Params {
+    int unused;
+  };
+  using Rows = NoRows;
+  using Col = float2;
+  static __device__ __forceinline__ void rows(const Params&, Rows&, int, int) {}
+  static __device__ __forceinline__ Col col(const Params&, int, int, bool) { return make_float2(0.f, 0.f); }
+  static __device__ __forceinline__ uint32_t pair(const Params&, const Rows&, Col, int, float x0, float x1) {
+    return pack_bf16(x0, x1);
+  }
+  static __device__ __forceinline__ void issue(const Params&, const void*, int, int) {}
 };
 
 // GPT-J fused q/k/v projection: out_bf16[m, n] = rotary(acc) for the first `rotary_dim` dims of every q and k head
@@ -1216,8 +1262,8 @@ using EpiIvfRows = EpiIvfRowsT<false>;
 using EpiIvfRowsMasked = EpiIvfRowsT<true>;
 
 
-// Profiling aids (sgpt_linear epilogue codes 100, 101): the mainloop and the accumulator hand-over with no epilogue work
-// at all, or with the accumulator loads only.
+// Profiling aid of gemm_bf16_tn_kernel (sgpt_linear epilogue code 101: kLoad): the mainloop and the accumulator hand-over
+// with no epilogue work at all, or with the accumulator loads only.
 template <bool kLoad>
 struct EpiDebugNull {
   struct Params { int dummy; };

@@ -49,21 +49,38 @@ struct PerDeviceOnce {
 // Programmatic dependent launch is on unless SGPT_PDL=0 is set in the environment (A/B measurements).
 bool pdl_enabled();
 
-// Launch with the programmatic-stream-serialization attribute (common.cuh: pdl_wait / pdl_launch_dependents).
+// Launch with the programmatic-stream-serialization attribute (common.cuh: pdl_wait / pdl_launch_dependents) and, for
+// cluster > 1, in thread-block clusters of `cluster` CTAs along x.
 template <class... KArgs, class... Args>
-inline cudaError_t launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                                 Args&&... args) {
+inline cudaError_t launch_kernel_cluster(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem,
+                                         cudaStream_t stream, int cluster, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute attr[2];
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = 0;
+  if (pdl_enabled()) {
+    attr[cfg.numAttrs].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[cfg.numAttrs].val.programmaticStreamSerializationAllowed = 1;
+    ++cfg.numAttrs;
+  }
+  if (cluster > 1) {
+    attr[cfg.numAttrs].id = cudaLaunchAttributeClusterDimension;
+    attr[cfg.numAttrs].val.clusterDim.x = static_cast<unsigned>(cluster);
+    attr[cfg.numAttrs].val.clusterDim.y = 1;
+    attr[cfg.numAttrs].val.clusterDim.z = 1;
+    ++cfg.numAttrs;
+  }
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
+}
+
+template <class... KArgs, class... Args>
+inline cudaError_t launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
+                                 Args&&... args) {
+  return launch_kernel_cluster(kern, grid, block, smem, stream, 1, static_cast<Args&&>(args)...);
 }
 
 }  // namespace sgpt

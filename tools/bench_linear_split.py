@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Where the time of the SGPT-125M linear layers goes: for each of the four shapes of a block at M = 32768 tokens, the
-product GEMM with its real epilogue, the same launch with the mainloop alone (sgpt_linear's profiling epilogue 100:
-mainloop and accumulator hand-over, no output written) and torch.nn.functional.linear (cuBLAS) on the same operands.
+product GEMM with its real epilogue, the same kernel with no global stores (sgpt_linear's profiling epilogue 100: the
+mainloop and the epilogue arithmetic, no output written) and torch.nn.functional.linear (cuBLAS) on the same operands.
 The variants alternate inside each round, every timed window is at least --window seconds of back-to-back launches
 between two CUDA events, and the median and min-max over --rounds rounds are printed as one JSON line per shape.
 
@@ -22,7 +22,7 @@ M = 32768
 # MLP c_fc (gelu_new + bias), MLP c_proj (reduce-add)
 SHAPES = [("qkv", 2304, 768, "bf16"), ("out_proj", 768, 768, "resid"), ("c_fc", 3072, 768, "gelu"),
           ("c_proj", 768, 3072, "resid")]
-EPI_NULL = 100  # gemm.cu: mainloop only
+EPI_NULL = 100  # gemm.cu: gemm_linear_kernel without its global stores
 
 
 def card():
