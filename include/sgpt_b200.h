@@ -624,6 +624,17 @@ int sgpt_ivf_range_search(int dtype, const void* Q, const void* C, const float* 
  *   with m % 32 != 0, and an unaligned lut or codes.  The workspace query returns -1 for the size arguments the search
  *   rejects.  The workspace does not depend on the code width: sgpt_ivfpq_search_workspace_bytes serves both widths.
  *
+ * sgpt_ivfpq_search_masked: sgpt_ivfpq_search_nbits with a filter, shared or per query, in the mask format of
+ *   sgpt_ivf_search_masked, indexed by list position (the rows of codes): mask_pitch_words = 0: one bitmap
+ *   [ceil(n/32)] shared by all queries; mask_pitch_words >= ceil(n/32): one bitmap per query, [nq][pitch]; NULL with
+ *   pitch 0: every position allowed.  Bits at or past n are ignored.  A position the mask does not allow is an empty
+ *   slot, as a negative doc_ids entry is, so the result is the top-k by ADC score over the probed positions that query
+ *   q's bitmap allows and whose doc_ids entry is >= 0 (same scores, order and tie rule, tail (-inf, -1)); a masked
+ *   position never appears.  The probes are the caller's and do not see the mask.  sgpt_ivfpq_search[_nbits](..., mask,
+ *   ...) is this call with pitch 0, and the workspace is the same (sgpt_ivfpq_search_workspace_bytes).
+ *   SGPT_ERR_INVALID, before any CUDA call, for sgpt_ivfpq_search_nbits's rejections and, as in sgpt_ivf_search_masked,
+ *   a negative pitch, 0 < pitch < ceil(n/32) and a non-zero pitch with a NULL mask.
+ *
  * sgpt_rerank: the exact score of each candidate against a stored shard, then its top-k.  dtype, Q, C, q_scale,
  *   c_scale, D, n and id_base mean what they mean in sgpt_search_masked (Q and C 16-byte aligned).  cand_ids int64
  *   [nq, kc] (device): global ids; a candidate < 0 or outside [id_base, id_base + n) is an empty slot, and the valid
@@ -654,6 +665,11 @@ int sgpt_ivfpq_search_nbits(const float* lut, const float* base, const uint8_t* 
                             int nbits, const int64_t* list_offsets, int nlist, int64_t max_list_len,
                             const int32_t* doc_ids, const int32_t* probes, int nprobe, int k, const uint32_t* mask,
                             float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream);
+int sgpt_ivfpq_search_masked(const float* lut, const float* base, const uint8_t* codes, int nq, int64_t n, int m,
+                             int nbits, const int64_t* list_offsets, int nlist, int64_t max_list_len,
+                             const int32_t* doc_ids, const int32_t* probes, int nprobe, int k, const uint32_t* mask,
+                             int64_t mask_pitch_words, float* out_scores, int64_t* out_ids, void* ws, int64_t ws_bytes,
+                             sgpt_stream_t stream);
 int64_t sgpt_rerank_workspace_bytes(int nq, int64_t kc);
 int sgpt_rerank(int dtype, const void* Q, const void* C, const float* q_scale, const float* c_scale, int nq, int64_t n,
                 int D, int64_t id_base, const int64_t* cand_ids, int64_t kc, int k, float* out_scores,

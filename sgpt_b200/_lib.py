@@ -113,6 +113,8 @@ _SIGNATURES = {
     "sgpt_pq_tables_nbits": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp]),
     "sgpt_ivfpq_search_nbits": (i32, [vp, vp, vp, i32, i64, i32, i32, vp, i32, i64, vp, vp, i32, i32, vp, vp, vp, vp,
                                       i64, vp]),
+    "sgpt_ivfpq_search_masked": (i32, [vp, vp, vp, i32, i64, i32, i32, vp, i32, i64, vp, vp, i32, i32, vp, i64, vp, vp,
+                                       vp, i64, vp]),
     "sgpt_rerank_workspace_bytes": (i64, [i32, i64]),
     "sgpt_rerank": (i32, [i32, vp, vp, vp, vp, i32, i64, i32, i64, vp, i64, i32, vp, vp, vp, i64, vp]),
     "sgpt_graph_prune": (i32, [vp, i64, i32, i32, vp, vp]),

@@ -9,7 +9,8 @@
 //            list tile (kTile documents) per step with cp.async.bulk on an mbarrier, double-buffered so that the next
 //            step's copies overlap this step's lookups.  Thread = document: it sums its m table entries in subspace order
 //            (its partial sum carries across the chunks of a tile) and writes (score bits, global id) of its position to
-//            the pair's candidate list, the layout of ivf.cu, two slots per 16-byte store.
+//            the pair's candidate list, the layout of ivf.cu, two slots per 16-byte store.  A position its query's
+//            bitmap does not allow is written as an empty slot (id -1), like a negative doc_ids entry.
 //   select   launch_ivf_select: launch_topk_select over G = nprobe packed lists per query (global ids).
 // The list offsets and probes are device data: offsets are clamped (list_range) and skipped probes never read, so
 // inconsistent inputs give wrong results, never an out-of-bounds access.
@@ -116,7 +117,8 @@ struct ScanArgs {
   const int32_t* doc_ids;   // [n]
   const int32_t* probes;    // [nb][nprobe]
   int nprobe;
-  const uint32_t* mask;     // shared bitmap of allowed positions or null
+  const uint32_t* mask;     // bitmap of allowed positions of the block's first query, or null
+  long long mask_pitch;     // words between the queries' bitmaps; 0: one bitmap shared by every query
   uint2* cand;              // [nb * nprobe][Ls]
   long long Ls;
   int slice;                // probes per work unit
@@ -162,6 +164,8 @@ __global__ void __launch_bounds__(kThreads, kBits == 8 ? 1 : kMinBlocks4) ivfpq_
   pdl_sync();
   const float* lut_q = a.lut + static_cast<long long>(ql) * m * kK;
   const int32_t* probes_q = a.probes + static_cast<long long>(ql) * a.nprobe;
+  // a unit belongs to one query (with tile groups too), so its bitmap is fixed for the unit
+  const uint32_t* mask_q = a.mask != nullptr ? a.mask + ql * a.mask_pitch : nullptr;
 
   auto seek = [&](Step& s) {  // first probed list at or after probe s.p that has a tile in [t_lo, t_hi)
     for (; s.p < p_hi; ++s.p) {
@@ -259,7 +263,7 @@ __global__ void __launch_bounds__(kThreads, kBits == 8 ? 1 : kMinBlocks4) ivfpq_
         float x = acc + __ldg(a.base + static_cast<long long>(ql) * a.nprobe + cur.p);
         x = (x != x) ? -1.f : x;
         int g = __ldg(a.doc_ids + pos);
-        if (a.mask != nullptr && !((__ldg(a.mask + (pos >> 5)) >> (pos & 31)) & 1u)) g = -1;
+        if (mask_q != nullptr && !((__ldg(mask_q + (pos >> 5)) >> (pos & 31)) & 1u)) g = -1;
         sb = __float_as_uint(x);
         gid = static_cast<uint32_t>(g);
       }
@@ -465,8 +469,8 @@ cudaError_t scan_launch(int m, ScanLaunch& l) {
 
 int ivfpq_search(const char* fn, const float* lut, const float* base, const uint8_t* codes, int nq, int64_t n, int m,
                  int nbits, const int64_t* list_offsets, int nlist, int64_t max_list_len, const int32_t* doc_ids,
-                 const int32_t* probes, int nprobe, int k, const uint32_t* mask, float* out_scores, int64_t* out_ids,
-                 void* ws, int64_t ws_bytes, cudaStream_t stream) {
+                 const int32_t* probes, int nprobe, int k, const uint32_t* mask, int64_t mask_pitch, float* out_scores,
+                 int64_t* out_ids, void* ws, int64_t ws_bytes, cudaStream_t stream) {
   if (check_pq_sizes(fn, nq, nlist, nprobe, max_list_len, m) != SGPT_OK) return SGPT_ERR_INVALID;
   if (check_nbits(fn, m, nbits) != SGPT_OK) return SGPT_ERR_INVALID;
   SGPT_REQUIRE(n >= 0 && n < (1ll << 31), "%s: corpus size n=%lld outside [0, 2^31)", fn, (long long)n);
@@ -477,6 +481,7 @@ int ivfpq_search(const char* fn, const float* lut, const float* base, const uint
   SGPT_REQUIRE(aligned16(lut) && aligned16(codes), "%s: lut and codes must be 16-byte aligned", fn);
   SGPT_REQUIRE(k >= 1 && k <= 4096, "%s: k=%d outside [1, 4096]", fn, k);
   SGPT_REQUIRE(out_scores != nullptr && out_ids != nullptr, "%s: null output", fn);
+  if (check_doc_mask(fn, n, DocMask{mask, mask_pitch}) != SGPT_OK) return SGPT_ERR_INVALID;
   const PqLayout w = make_pq_layout(nq, nlist, nprobe, max_list_len);
   SGPT_REQUIRE(ws != nullptr && ws_bytes >= w.total, "%s: workspace too small (%lld < %lld bytes)", fn,
                (long long)ws_bytes, (long long)w.total);
@@ -509,10 +514,11 @@ int ivfpq_search(const char* fn, const float* lut, const float* base, const uint
     const long long group_tiles = (tiles_max + groups - 1) / groups;
     groups = (tiles_max + group_tiles - 1) / group_tiles;
     const long long units = static_cast<long long>(nb) * ((nprobe + slice - 1) / slice) * groups;
+    const uint32_t* block_mask = mask != nullptr ? mask + static_cast<long long>(q0) * mask_pitch : nullptr;
     ScanArgs a{lut + ((static_cast<long long>(q0) * m) << nbits), base + static_cast<long long>(q0) * nprobe, codes,
                static_cast<int>(n), m, list_offsets, nlist, static_cast<long long>(max_list_len), doc_ids, pr, nprobe,
-               mask, cand, static_cast<long long>(w.Ls), static_cast<int>(slice), static_cast<int>(groups),
-               static_cast<int>(group_tiles)};
+               block_mask, static_cast<long long>(mask_pitch), cand, static_cast<long long>(w.Ls),
+               static_cast<int>(slice), static_cast<int>(groups), static_cast<int>(group_tiles)};
     {
       LaunchScope _ls(kCatScores, stream);
       SGPT_CHECK_CUDA(launch_kernel(sl.kernel, dim3(static_cast<unsigned>(units)), dim3(kThreads), sl.smem, stream, a));
@@ -551,7 +557,17 @@ extern "C" int sgpt_ivfpq_search_nbits(const float* lut, const float* base, cons
                                        const uint32_t* mask, float* out_scores, int64_t* out_ids, void* ws,
                                        int64_t ws_bytes, sgpt_stream_t stream) {
   return ivfpq_search("sgpt_ivfpq_search_nbits", lut, base, codes, nq, n, m, nbits, list_offsets, nlist, max_list_len,
-                      doc_ids, probes, nprobe, k, mask, out_scores, out_ids, ws, ws_bytes,
+                      doc_ids, probes, nprobe, k, mask, 0, out_scores, out_ids, ws, ws_bytes,
+                      static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int sgpt_ivfpq_search_masked(const float* lut, const float* base, const uint8_t* codes, int nq, int64_t n,
+                                        int m, int nbits, const int64_t* list_offsets, int nlist, int64_t max_list_len,
+                                        const int32_t* doc_ids, const int32_t* probes, int nprobe, int k,
+                                        const uint32_t* mask, int64_t mask_pitch_words, float* out_scores,
+                                        int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream) {
+  return ivfpq_search("sgpt_ivfpq_search_masked", lut, base, codes, nq, n, m, nbits, list_offsets, nlist, max_list_len,
+                      doc_ids, probes, nprobe, k, mask, mask_pitch_words, out_scores, out_ids, ws, ws_bytes,
                       static_cast<cudaStream_t>(stream));
 }
 
@@ -560,7 +576,7 @@ extern "C" int sgpt_ivfpq_search(const float* lut, const float* base, const uint
                                  const int32_t* probes, int nprobe, int k, const uint32_t* mask, float* out_scores,
                                  int64_t* out_ids, void* ws, int64_t ws_bytes, sgpt_stream_t stream) {
   return ivfpq_search("sgpt_ivfpq_search", lut, base, codes, nq, n, m, 8, list_offsets, nlist, max_list_len, doc_ids,
-                      probes, nprobe, k, mask, out_scores, out_ids, ws, ws_bytes, static_cast<cudaStream_t>(stream));
+                      probes, nprobe, k, mask, 0, out_scores, out_ids, ws, ws_bytes, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int64_t sgpt_rerank_workspace_bytes(int nq, int64_t kc) {

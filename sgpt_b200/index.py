@@ -185,6 +185,18 @@ def _check_allow(allow, device, n: int, nq: int) -> torch.Tensor:
     return allow
 
 
+def _allow_mask(allow: Optional[torch.Tensor], deleted: Optional[torch.Tensor], device, n: int, nq: int
+                ) -> Tuple[Optional[torch.Tensor], int]:
+    """(bitmap, pitch in words) of a search of nq queries over n documents: `allow` (bool [n] or [nq, n], or None)
+    packed with the `deleted` bits (int32 words, or None) cleared; (None, 0) when every document is allowed."""
+    if allow is None:
+        return (None, 0) if deleted is None else (torch.bitwise_not(deleted).contiguous(), 0)
+    m = pack_mask(_check_allow(allow, device, n, nq))
+    if deleted is not None:
+        m = m & torch.bitwise_not(deleted)
+    return m.contiguous(), (m.shape[1] if m.dim() == 2 and n > 0 else 0)
+
+
 def _mask_rows(mask: Tuple[Optional[torch.Tensor], int], first: int) -> Tuple[Optional[torch.Tensor], int]:
     """The (bitmap, pitch) of a search's queries first .. : per-query bitmaps lose their first rows, a shared one stays."""
     return (mask[0][first:], mask[1]) if mask[1] > 0 else mask
@@ -430,12 +442,7 @@ class CorpusShard:
         """(bitmap, pitch in words) of a search of nq queries: `allow` (bool [n] or [nq, n], or None) without the deleted
         documents; (None, 0) when every document is allowed."""
         deleted = _bit_slice(self._deleted["words"], self._deleted_at, self.n) if self._deleted["any"] else None
-        if allow is None:
-            return (None, 0) if deleted is None else (torch.bitwise_not(deleted).contiguous(), 0)
-        m = pack_mask(_check_allow(allow, self.device, self.n, nq))
-        if deleted is not None:
-            m = m & torch.bitwise_not(deleted)
-        return m.contiguous(), (m.shape[1] if m.dim() == 2 and self.n > 0 else 0)
+        return _allow_mask(allow, deleted, self.device, self.n, nq)
 
     def _dtype_id(self) -> int:
         """The `dtype` argument of the masked entry points for this shard's format."""

@@ -80,6 +80,14 @@ def _kmeans(x: torch.Tensor, nlist: int, n_iter: int, g: torch.Generator, score_
     return cent
 
 
+def _list_order(allow: Optional[torch.Tensor], ids: torch.Tensor, id_base: int, nq: int) -> Optional[torch.Tensor]:
+    """`allow` of a search of nq queries (boolean [n] or [nq, n] indexed by global id - id_base, checked here) permuted to
+    the list order of an index whose position p holds global id ids[p], with one gather; None stays None."""
+    if allow is None:
+        return None
+    return _check_allow(allow, ids.device, ids.numel(), nq).index_select(-1, ids - id_base)
+
+
 def _merge_lists(offsets: torch.Tensor, lists: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """Destinations of an append to list-ordered storage (``IVFIndex.add``, ``IVFPQIndex.add``): the n old positions
     (offsets int64 [nlist + 1], device) and m new rows whose lists are `lists` int64 [m].  Every list keeps its rows in
@@ -242,12 +250,9 @@ class IVFIndex:
         return self._ws
 
     def _list_mask(self, allow: Optional[torch.Tensor], nq: int) -> Tuple[Optional[torch.Tensor], int]:
-        """(bitmap, pitch) over list positions: `allow` (document order) permuted to list order with one gather, then
+        """(bitmap, pitch) over list positions: `allow` (document order) permuted to list order (``_list_order``), then
         packed with the deletions ANDed in (``CorpusShard._mask``)."""
-        if allow is None:
-            return self.shard._mask(None, nq)
-        allow = _check_allow(allow, self.device, self.n, nq)
-        return self.shard._mask(allow.index_select(-1, self.ids - self.id_base), nq)
+        return self.shard._mask(_list_order(allow, self.ids, self.id_base, nq), nq)
 
     def _search_rows(self, qb, q_scale, c_scale, probes, k: int, mask) -> Tuple[torch.Tensor, torch.Tensor]:
         """sgpt_ivf_search (shared or no bitmap) or sgpt_ivf_search_masked (per-query bitmaps) of prepared rows."""

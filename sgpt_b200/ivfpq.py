@@ -9,8 +9,10 @@ its ``nprobe`` nearest lists (``IVFIndex.probe``'s rule), and the scan scores ev
 query's lookup tables (include/sgpt_b200.h, IVF-PQ search): m shared-memory lookups per document instead of a D-long dot
 product.  The scores are approximations (asymmetric distance computation, ADC); ``search(..., refine=shard)`` re-ranks
 the PQ pass's best ``k_refine`` documents with their exact scores from a ``CorpusShard`` holding the same documents.
+``search(..., allow=)`` takes a boolean filter, shared ([n]) or per query ([Q, n]), as every other search does: the scan
+skips the positions it does not allow, so the refine pass re-ranks allowed documents only.
 
-Not supported: ``allow=`` filters, range search, paraphrase mining / community detection over an IVF-PQ index, code
+Not supported: range search, paraphrase mining / community detection over an IVF-PQ index, code
 sizes other than 4 and 8 bits, OPQ rotations, fp16 tables and indexes spread over several GPUs.
 """
 from __future__ import annotations
@@ -23,14 +25,15 @@ import numpy as np
 import torch
 
 from . import _lib
-from .index import CorpusShard, _bit_slice, _check_score_function, pack_mask, unpack_mask
-from .ivf import _assign, _kmeans, _merge_lists, _rows_f32
+from .index import CorpusShard, _allow_mask, _bit_slice, _check_allow, _check_score_function, pack_mask, unpack_mask
+from .ivf import _assign, _kmeans, _list_order, _merge_lists, _rows_f32
 
 FORMAT = "sgpt_b200.IVFPQIndex/1"
 NBITS = 8                 # the default code width
 _NBITS = (4, 8)           # the supported code widths
 _BATCH_BYTES = 256 << 20  # fp32 rows per encoding batch
-_QUERY_BLOCK = 1024       # queries per table / scan call with 8-bit codes (the tables take m KB per query)
+_QUERY_BLOCK = 1024       # queries per table / scan call with 8-bit codes (the tables take m KB per query), and with a
+                          # per-query filter at either width (packing a block's filter takes 8 bytes per bit on the way)
 
 
 def _check_pq_shape(D: int, m: int, nbits: int = NBITS) -> None:
@@ -271,9 +274,18 @@ class IVFPQIndex:
         _lib.check(rc, "sgpt_pq_tables_nbits")
         return lut, base
 
-    def scan(self, lut: torch.Tensor, base: torch.Tensor, probes: torch.Tensor, k: int
-             ) -> Tuple[torch.Tensor, torch.Tensor]:
-        """``sgpt_ivfpq_search_nbits`` of prepared tables: the top-k by ADC score of the undeleted probed documents."""
+    def _list_mask(self, allow: Optional[torch.Tensor], nq: int) -> Tuple[Optional[torch.Tensor], int]:
+        """(bitmap, pitch) over list positions of a search of nq queries: `allow` (document order, boolean [n] or
+        [nq, n], or None) permuted to list order (``_list_order``) and packed with the deletions ANDed in."""
+        return _allow_mask(_list_order(allow, self.ids, self.id_base, nq), self._deleted, self.device, self.n, nq)
+
+    def scan(self, lut: torch.Tensor, base: torch.Tensor, probes: torch.Tensor, k: int,
+             mask: Optional[Tuple[Optional[torch.Tensor], int]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``sgpt_ivfpq_search_masked`` of prepared tables: the top-k by ADC score of the allowed probed documents.
+        ``mask``: (bitmap int32, pitch in words) over list positions, as ``_list_mask`` makes it (deletions already
+        cleared); None allows every undeleted document."""
+        if mask is None:
+            mask = self._list_mask(None, probes.shape[0])
         nq, nprobe = probes.shape
         out_s = torch.full((nq, k), -float("inf"), dtype=torch.float32, device=self.device)
         out_i = torch.full((nq, k), -1, dtype=torch.int64, device=self.device)
@@ -285,25 +297,31 @@ class IVFPQIndex:
             raise ValueError(f"sgpt_ivfpq_search rejects these arguments: {lib.sgpt_last_error().decode()}")
         if self._ws is None or self._ws.numel() < need:
             self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
-        mask = None if self._deleted is None else torch.bitwise_not(self._deleted).contiguous()
         with torch.cuda.device(self.device):
-            rc = lib.sgpt_ivfpq_search_nbits(lut.data_ptr(), base.data_ptr(), self.codes.data_ptr(), nq, self.n,
-                                             self.m, self.nbits, self.offsets.data_ptr(), self.nlist, self.max_list_len,
-                                             self.ids.data_ptr(), probes.data_ptr(), nprobe, k, _lib.ptr(mask),
-                                             out_s.data_ptr(), out_i.data_ptr(), self._ws.data_ptr(), self._ws.numel(),
-                                             _lib.current_stream())
-        _lib.check(rc, "sgpt_ivfpq_search_nbits")
+            rc = lib.sgpt_ivfpq_search_masked(lut.data_ptr(), base.data_ptr(), self.codes.data_ptr(), nq, self.n,
+                                              self.m, self.nbits, self.offsets.data_ptr(), self.nlist, self.max_list_len,
+                                              self.ids.data_ptr(), probes.data_ptr(), nprobe, k, _lib.ptr(mask[0]),
+                                              mask[1], out_s.data_ptr(), out_i.data_ptr(), self._ws.data_ptr(),
+                                              self._ws.numel(), _lib.current_stream())
+        _lib.check(rc, "sgpt_ivfpq_search_masked")
         return out_s, out_i
 
     def search(self, queries: torch.Tensor, k: int, nprobe: int, refine: Optional[CorpusShard] = None,
-               k_refine: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+               k_refine: Optional[int] = None, allow: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
         """Top-k of the undeleted documents in each query's ``nprobe`` probed lists by ADC score, for fp32/bf16 queries
         [Q, D]: (scores fp32 [Q, k] descending, global ids int64 [Q, k]), ties by ascending id, tail (-inf, -1).
+
+        ``allow``: boolean device tensor [n] (all queries) or [Q, n] (one row per query), indexed by global id - id_base
+        as in ``CorpusShard.search``: only those documents may be returned.  The result is the top-k by ADC score of the
+        allowed, undeleted documents in each query's probed lists.  The probes do not depend on the filter (they are
+        still the ``nprobe`` nearest centroids), so a selective filter can return fewer than k documents even where the
+        whole index holds more; nothing falls back to an exact search.
 
         ``refine``: a ``CorpusShard`` holding the same documents (same id_base and n, e.g. the source of ``build``).  The
         PQ pass then selects ``k_refine`` candidates (default min(4096, 10 k)) and the result is the top-k of their exact
         scores in the shard (``sgpt_rerank``: the bits of ``refine.search``).  The shard's own deletions are not
-        consulted: delete documents through the index (``remove``), which leaves them out of the candidates."""
+        consulted: delete documents through the index (``remove``), which leaves them out of the candidates.  With
+        ``allow`` the candidates are allowed documents only, so a refined filtered search re-ranks only those."""
         k = int(k)
         if not 1 <= k <= 4096:
             raise ValueError(f"k={k} must lie in [1, 4096]")
@@ -318,13 +336,21 @@ class IVFPQIndex:
             if (refine.id_base, refine.n, refine.dim) != (self.id_base, self.n, self.dim):
                 raise ValueError(f"refine shard (id_base={refine.id_base}, n={refine.n}, dim={refine.dim}) does not hold "
                                  f"the index's documents (id_base={self.id_base}, n={self.n}, dim={self.dim})")
+        nq = queries.shape[0]
+        if allow is not None:
+            allow = _check_allow(allow, self.device, self.n, nq)
+        per_query = allow is not None and allow.dim() == 2
+        mask = None if per_query else self._list_mask(allow, nq)
         queries = queries.to(self.device)
         outs = []
-        block = _QUERY_BLOCK * (256 >> self.nbits)  # the same table bytes per call: 16x the queries with 4-bit codes
-        for a in range(0, max(queries.shape[0], 1), block):
+        # the same table bytes per call: 16x the queries with 4-bit codes, unless a per-query filter is packed per block
+        block = _QUERY_BLOCK if per_query else _QUERY_BLOCK * (256 >> self.nbits)
+        for a in range(0, max(nq, 1), block):
             q = queries[a:a + block]
+            if per_query:
+                mask = self._list_mask(allow[a:a + block], q.shape[0])
             probes = self.probe(q, nprobe)
-            s, i = self.scan(*self.tables(q, probes), probes, kk)
+            s, i = self.scan(*self.tables(q, probes), probes, kk, mask)
             outs.append((s, i) if refine is None else rerank(refine, q, i, k, self.score_function))
         return torch.cat([o[0] for o in outs]), torch.cat([o[1] for o in outs])
 
